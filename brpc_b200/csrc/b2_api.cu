@@ -249,7 +249,7 @@ extern "C" int b2_ctx_create(const b2_options* o, b2_ctx** out) {
     if (const char* e = getenv("B2_PACK")) c->use_tma_pack = strcmp(e, "reg") != 0;
     if (const char* e = getenv("B2_SMALL")) c->use_fused_small = strcmp(e, "off") != 0;
     if (const char* e = getenv("B2_FUSED")) c->use_fused = strcmp(e, "off") != 0;
-    CU(cudaFuncSetAttribute(k_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(FusedWarpSmem) * kFusedWarps)));
+    CU(cudaFuncSetAttribute(k_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(FusedWarpSmem) * (kFusedWarps > kFusedWarpsDense ? kFusedWarps : kFusedWarpsDense))));
     CU(cudaFuncSetAttribute(k_small, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmallSmem)));
     *out = c;
     return B2_OK;
@@ -459,7 +459,9 @@ static int launch_pipeline(b2_ctx* c) {
     }
     if (fused) {
         // one pass over the bytes: decode + echo + pack per live tile (k_frame_table / k_decode / k_scan / k_pack_tma are not needed)
-        if (c->n_tiles) { k_fused<<<sms, kFusedWarps * 32, sizeof(FusedWarpSmem) * kFusedWarps, s>>>(B, C); launches++; mark("fused"); }
+        // (before a context's first batch has told the average frame size, a tile may hold many frames to walk again: the many-warp shape)
+        const uint32_t fw = c->avg_frame && !c->dense ? kFusedWarps : kFusedWarpsDense;
+        if (c->n_tiles) { k_fused<<<sms, fw * 32, sizeof(FusedWarpSmem) * fw, s>>>(B, C); launches++; mark("fused"); }
     } else {
     if (c->n_tiles) { k_frame_table<<<(uint32_t)(((uint64_t)c->n_tiles * C.spec_k + 255) / 256), 256, 0, s>>>(B, C); launches++; mark("frame_table"); }
     // message-count dependent kernels are persistent: fixed grids (multiples of the SM count)

@@ -2058,11 +2058,19 @@ __global__ void __launch_bounds__(kPackWarps * 32, 1) k_pack_tma(BatchPtrs B, De
 #ifndef B2_FUSED_BUF
 #define B2_FUSED_BUF 10240
 #endif
-// (16 x ~13.5 KB leave ~12 KB of the SM's shared memory to k_resolve of the next batch, which runs beside this kernel)
+// Warps per CTA, chosen per batch at launch.  Measured on an H100 80GB HBM3 (700 W limit, 1980 MHz SM clock), bench.py with two batches
+// in flight: 12 warps x 128 registers leave 16K registers and ~100 KB of shared memory per SM, room for a k_resolve or k_tile_search
+// block (256 threads x 40 registers) of the other batch beside this kernel: 1 KB requests 1086 M msgs/s (16 warps: ~1045 M), 4 KB
+// 274 M (264 M), 1024 connections x 256 KiB 1065 M (1005 M).  Dense tiles (small requests, several rounds per tile, or tiles whose
+// frames are walked again by lane 0 because the context did not know yet that they are small) want the whole register file instead:
+// 64 B requests 2980 M msgs/s with 16 warps, 2680 M with 12; 256 B 2248 M against 1995 M.
 #ifndef B2_FUSED_WARPS
-#define B2_FUSED_WARPS 16      // measured: 16 warps x 128 registers 115 us per 256 MiB batch; 20 x 96 the same (spills), 21 x 96 does not launch
+#define B2_FUSED_WARPS 12
 #endif
-constexpr uint32_t kFusedWarps = B2_FUSED_WARPS, kFusedBuf = B2_FUSED_BUF, kFusedRowStride = 176;
+#ifndef B2_FUSED_WARPS_DENSE
+#define B2_FUSED_WARPS_DENSE 16
+#endif
+constexpr uint32_t kFusedWarps = B2_FUSED_WARPS, kFusedWarpsDense = B2_FUSED_WARPS_DENSE, kFusedBuf = B2_FUSED_BUF, kFusedRowStride = 176;
 // The plain echo request exactly as PackRpcRequest emits it (baidu_rpc_protocol.cpp:1045-1133) — known fields once each, ascending,
 // one-byte tags and lengths, compress / content / checksum type 0, no attachment, no checksum bytes, body "0a <len> <message>" —
 // decoded, looked up and ANSWERED in ~300 instructions: descriptor to HBM, reply prefix written right in front of the payload
@@ -2167,10 +2175,7 @@ __device__ __forceinline__ void fused_store(uint8_t* resp, const uint8_t* img, u
 #ifndef B2_FUSED_REGS
 #define B2_FUSED_REGS 128
 #endif
-#ifndef B2_FUSED_PREFETCH
-#define B2_FUSED_PREFETCH 1
-#endif
-static_assert(B2_FUSED_REGS * B2_FUSED_WARPS * 32 <= 65536, "k_fused: registers x threads must fit the SM's register file");
+static_assert(B2_FUSED_REGS * (B2_FUSED_WARPS > B2_FUSED_WARPS_DENSE ? B2_FUSED_WARPS : B2_FUSED_WARPS_DENSE) * 32 <= 65536, "k_fused: registers x threads must fit the SM's register file");
 __global__ void __maxnreg__(B2_FUSED_REGS) k_fused(BatchPtrs B, DevConfig C) {
     extern __shared__ __align__(128) uint8_t fused_raw[];
     const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -2188,9 +2193,9 @@ __global__ void __maxnreg__(B2_FUSED_REGS) k_fused(BatchPtrs B, DevConfig C) {
     if (lane == 0) { mbar_init(&S.mbar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
     __syncwarp();
     uint32_t phase = 0;
-    const uint32_t n_warps = gridDim.x * kFusedWarps;
+    const uint32_t n_warps = gridDim.x * (blockDim.x >> 5);
     // the records of the NEXT tile are requested before the current one is worked on (they would otherwise cost a DRAM round trip per tile)
-    uint32_t t = blockIdx.x * kFusedWarps + wid;
+    uint32_t t = blockIdx.x * (blockDim.x >> 5) + wid;
     uint4 rec_raw = make_uint4(0, 0, 0, 0), ti = make_uint4(0, 0, 0, 0); uint32_t tbase = 0;
     if (t < B.n_tiles) { rec_raw = *reinterpret_cast<const uint4*>(B.tiles + t); ti = __ldg(B.tile_info + t); tbase = B.tile_base[t]; }
     for (; t < B.n_tiles; t += n_warps) {
@@ -2200,7 +2205,6 @@ __global__ void __maxnreg__(B2_FUSED_REGS) k_fused(BatchPtrs B, DevConfig C) {
         TileRec rec; *reinterpret_cast<uint4*>(&rec) = rec_cur;
         const uint32_t count = rec.count;
         if (!rec.live || count == 0) continue;
-        const uint4 ti_nx = ti;                                      // (the NEXT tile's run record, loaded above)
         const uint4 ti = ti_cur;
         const uint32_t r = ti.w & 0xffffffu, run_off = ti.x, run_len = ti.y;
         const bool client = ((ti.w >> 24) & B2_RUN_CLIENT) != 0, dump = ((ti.w >> 24) & B2_RUN_RPC_DUMP) != 0;
@@ -2236,18 +2240,8 @@ __global__ void __maxnreg__(B2_FUSED_REGS) k_fused(BatchPtrs B, DevConfig C) {
             const bool fits = span <= kFusedBuf;
             if (fits) {
                 // ---- the whole round in one buffer: load, decode in place, patch, store
+                // (no L2 prefetch of the next tile: on the H100 it cost a fifth of the kernel's time, tools/probes/fused_ceiling.cu)
                 if (lane == 0) { bulk_wait_read<0>(); mbar_arrive_expect_tx(&S.mbar, span); bulk_g2s(S.buf, B.bytes + lo16, span, &S.mbar); }
-#if B2_FUSED_PREFETCH
-                // while this tile is on its way: ask for the NEXT tile's bytes (its record arrived meanwhile) to be brought into L2, so that a
-                // warp has two tiles' worth of DRAM reads in flight with one staging buffer
-                if (lane == 0 && done == 0 && tn < B.n_tiles) {
-                    TileRec nx; *reinterpret_cast<uint4*>(&nx) = rec_raw;
-                    if (nx.live && nx.count) {
-                        const uint32_t plo = (ti_nx.x + nx.entry) & ~15u, phi = (ti_nx.x + nx.exit + 15u) & ~15u;
-                        if (phi > plo) bulk_prefetch_l2(B.bytes + plo, min(phi - plo, 2u * kFusedBuf));
-                    }
-                }
-#endif
                 __syncwarp();
                 mbar_wait(&S.mbar, phase & 1u); phase++;
                 bool in_place = false;
