@@ -36,6 +36,9 @@ H2_REQUEST_RESULT_DT = np.dtype([("status", "<i4"), ("stream_id", "<u4"), ("out_
 H2_MSG_DT = np.dtype([("run_idx", "<u4"), ("stream_id", "<u4"), ("headers_off", "<u4"), ("headers_len", "<u4"), ("n_headers", "<u4"),
                       ("body_off", "<u4"), ("body_len", "<u4"), ("http_method", "<u4"), ("content_type", "<u4"), ("flags", "<u4"),
                       ("method_idx", "<i4"), ("msg_off", "<u4"), ("msg_len", "<u4"), ("path_off", "<u4"), ("path_len", "<u4"), ("reserved", "<u4")])
+H2_CALL_DT = np.dtype([("run_idx", "<u4"), ("stream_id", "<u4"), ("how", "<u4"), ("status_code", "<i4"), ("error_code", "<i4"), ("grpc_status", "<i4"),
+                       ("headers_off", "<u4"), ("headers_len", "<u4"), ("n_headers", "<u4"), ("body_off", "<u4"), ("body_len", "<u4"),
+                       ("msg_off", "<u4"), ("msg_len", "<u4"), ("error_off", "<u4"), ("error_len", "<u4"), ("flags", "<u4")])   # == b2_h2_call, 64 bytes
 MSG_DT = np.dtype([("run_idx", "<u4"), ("frame_off", "<u4"), ("body_size", "<u4"), ("meta_size", "<u4"),
                    ("correlation_id", "<i8"), ("log_id", "<i8"),
                    ("attachment_size", "<i4"), ("compress_type", "<i4"), ("checksum_type", "<i4"), ("error_code", "<i4"),
@@ -132,6 +135,10 @@ def _load():
     l.b2_h2_pack_requests.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p]
     l.b2_h2_conn_set_next_stream_id.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32]
     l.b2_h2_conn_peer_update.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
+    l.b2_h2_client_conn_reset.argtypes = [C.c_void_p, C.c_uint32]
+    l.b2_h2_client_process_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32,
+                                             C.POINTER(C.c_uint32), C.c_void_p, C.c_uint32]
+    l.b2_h2_client_abandon_streams.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
     l.b2_h2_pack_responses.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     l.b2_pack_requests.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     l.b2_pack_responses.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
@@ -147,7 +154,8 @@ ABI_SYMBOLS = ["b2_ctx_create", "b2_ctx_destroy", "b2_last_error", "b2_version",
                "b2_set_server_identity", "b2_set_stream_handler", "b2_set_protocols", "b2_block_alloc", "b2_block_free", "b2_block_pool_host_allocs", "b2_set_modes", "b2_ring_start", "b2_ring_stop", "b2_ring_submit", "b2_ring_wait", "b2_ring_launches", "b2_ring_phase_ns", "b2_latency_probe", "b2_process_batch", "b2_batch_submit", "b2_batch_collect", "b2_batch_upload",
                "b2_batch_execute", "b2_batch_execute_many", "b2_batch_download", "b2_batch_launch", "b2_batch_wait",
                "b2_elapsed_ms", "b2_batch_info", "b2_device_pci_bus_id", "b2_stage_times", "b2_crc32c_batch", "b2_crc32c_extend", "b2_snappy_max_compressed_length", "b2_snappy_raw_compress", "b2_snappy_get_uncompressed_length", "b2_snappy_raw_uncompress", "b2_snappy_uncompress_batch", "b2_snappy_compress_batch", "b2_hpack_reset", "b2_hpack_decode_batch", "b2_pack_requests", "b2_pack_responses", "b2_h2_scan_batch", "b2_h2_conn_reset", "b2_h2_configure", "b2_h2_process_batch", "b2_h2_pack_responses", "b2_counters_read",
-               "b2_counters_device_ptr", "b2_counters_allreduce", "b2_h2_pack_requests", "b2_h2_conn_set_next_stream_id", "b2_h2_conn_peer_update"]
+               "b2_counters_device_ptr", "b2_counters_allreduce", "b2_h2_pack_requests", "b2_h2_conn_set_next_stream_id", "b2_h2_conn_peer_update",
+               "b2_h2_client_conn_reset", "b2_h2_client_process_batch", "b2_h2_client_abandon_streams"]
 
 ECHO_METHOD = dict(service_full_name=b"example.EchoService", service_name=b"EchoService", method_name=b"Echo",
                    request_type_name=b"example.EchoRequest", handler=1, echo_attachment=1,
@@ -466,6 +474,30 @@ class Context:
 
     def h2_conn_set_next_stream_id(self, conn, next_id):
         _check(lib.b2_h2_conn_set_next_stream_id(self._h, conn, next_id))
+
+    def h2_client_conn_reset(self, conn):
+        """A new client connection whose server frames the device parses (h2_client_process_batch)."""
+        _check(lib.b2_h2_client_conn_reset(self._h, conn))
+
+    def h2_client_process_batch(self, data, runs, call_cap=None, out_cap=None, out=None):
+        """The server's bytes of client connections (runs[i].socket_id = connection).  Returns (run_status, calls, out): one H2_CALL_DT per
+        stream that left its connection; header records, copied bodies and error texts live in out, the bytes to write back at ctrl_off."""
+        data = np.ascontiguousarray(data, dtype=np.uint8); runs = np.ascontiguousarray(runs, dtype=RUN_DT)
+        n = len(runs)
+        call_cap = call_cap or max(64, 128 * n)
+        out_cap = out_cap or max(1 << 16, n * (1 << 17))
+        rs = np.zeros(n, H2_RUN_STATUS_DT); calls = np.zeros(call_cap, H2_CALL_DT); nc = C.c_uint32(0)
+        if out is None:
+            out = np.empty(out_cap, np.uint8)
+        out_cap = out.nbytes
+        _check(lib.b2_h2_client_process_batch(self._h, data.ctypes.data, data.nbytes, runs.ctypes.data, n, rs.ctypes.data, calls.ctypes.data,
+                                              call_cap, C.byref(nc), out.ctypes.data, out_cap))
+        return rs, calls[:nc.value], out
+
+    def h2_client_abandon_streams(self, conn, stream_ids):
+        """Calls given up on (AddAbandonedStream): their streams are dropped at the end of the connection's next client parse."""
+        ids = np.ascontiguousarray(stream_ids, dtype=np.uint32)
+        _check(lib.b2_h2_client_abandon_streams(self._h, conn, ids.ctypes.data, len(ids)))
 
     def pack_requests(self, data, reqs, out_cap=None):
         """reqs: REQUEST_DT array (offsets into data).  Returns the packed frame of every request (b"" = rejected)."""

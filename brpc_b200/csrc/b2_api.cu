@@ -1283,7 +1283,7 @@ extern "C" int b2_h2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes
     CU(cudaMemcpyAsync(d_reqs, reqs, sizeof(b2_h2_request) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_res, results, sizeof(b2_h2_request_result) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_first, first.data(), 4 * first.size(), cudaMemcpyHostToDevice, c->stream));
-    k_h2_pack_req<<<(n_groups + kH2PackWarps - 1) / kH2PackWarps, kH2PackWarps * 32, 0, c->stream>>>(d_in, d_reqs, d_first, n_groups, c->d_h2, c->d_resp, d_res);
+    k_h2_pack_req<<<(n_groups + kH2PackWarps - 1) / kH2PackWarps, kH2PackWarps * 32, 0, c->stream>>>(d_in, d_reqs, d_first, n_groups, c->d_h2, c->d_resp, d_res, h2_pool(c));
     CU(cudaMemcpyAsync(results, d_res, sizeof(b2_h2_request_result) * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaMemcpyAsync(out, c->d_resp, (size_t)total, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
@@ -1312,6 +1312,77 @@ extern "C" int b2_h2_conn_set_next_stream_id(b2_ctx* c, uint32_t conn, uint32_t 
     CU(cudaSetDevice(c->opt.device));
     k_h2_set_next_stream_id<<<1, 1, 0, c->stream>>>(c->d_h2, conn, next_id);
     CU(cudaStreamSynchronize(c->stream));
+    return B2_OK;
+}
+
+// the receiving half of a client connection: see include/b2rpc.h
+extern "C" int b2_h2_client_conn_reset(b2_ctx* c, uint32_t conn) {
+    if (!c || conn >= c->h2_max_conns) { set_err("bad connection index"); return B2_E_INVAL; }
+    int rc = h2_ensure(c); if (rc != B2_OK) return rc;
+    CU(cudaSetDevice(c->opt.device));
+    k_h2_client_conn_reset<<<1, 1, 0, c->stream>>>(c->d_h2, c->d_hpack, conn, h2_pool(c));
+    CU(cudaStreamSynchronize(c->stream));
+    return B2_OK;
+}
+extern "C" int b2_h2_client_abandon_streams(b2_ctx* c, uint32_t conn, const uint32_t* stream_ids, uint32_t n) {
+    if (!c || (!stream_ids && n)) { set_err("null argument"); return B2_E_INVAL; }
+    if (conn >= c->h2_max_conns) { set_err("bad connection index"); return B2_E_INVAL; }
+    if ((uint64_t)n * 4 > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }   // (the ids go to the second half of the scratch)
+    if (n == 0) return B2_OK;
+    int rc = h2_ensure(c); if (rc != B2_OK) return rc;
+    CU(cudaSetDevice(c->opt.device));
+    uint32_t* d_ids = reinterpret_cast<uint32_t*>(c->d_unz + c->opt.max_resp_bytes);   // second half of the scratch (as b2_h2_pack_requests)
+    CU(cudaMemcpyAsync(d_ids, stream_ids, 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
+    k_h2_client_abandon<<<1, 1, 0, c->stream>>>(c->d_h2, conn, d_ids, n, h2_pool(c));
+    CU(cudaStreamSynchronize(c->stream));
+    return B2_OK;
+}
+extern "C" int b2_h2_client_process_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
+                                          b2_h2_run_status* rs, b2_h2_call* calls, uint32_t call_cap, uint32_t* n_calls,
+                                          void* out, uint32_t out_cap) {
+    if (!c || !bytes || !runs || !rs || !calls || !n_calls || !out) { set_err("null argument"); return B2_E_INVAL; }
+    static_assert(sizeof(b2_h2_call) == 64, "h2 call ABI layout");
+    if (nbytes > c->opt.max_batch_bytes || n_runs > c->opt.max_runs || out_cap > 2ull * c->opt.max_resp_bytes || call_cap > c->opt.max_msgs) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    *n_calls = 0;
+    if (n_runs == 0) return B2_OK;
+    for (uint32_t r = 0; r < n_runs; r++) {
+        if ((uint64_t)runs[r].offset + runs[r].length > nbytes) { set_err("run outside buffer"); return B2_E_INVAL; }
+        if (runs[r].socket_id >= c->h2_max_conns) { set_err("connection index out of range"); return B2_E_INVAL; }
+        for (uint32_t q = 0; q < r; q++) if (runs[q].socket_id == runs[r].socket_id) { set_err("one run per connection and batch"); return B2_E_INVAL; }
+    }
+    const uint32_t region = (out_cap / n_runs) & ~63u, per_run_calls = call_cap / n_runs;
+    if (region < 256 || per_run_calls == 0) { set_err("out_cap / call_cap too small for the number of runs"); return B2_E_CAPACITY; }
+    int rc = h2_ensure(c); if (rc != B2_OK) return rc;
+    CU(cudaSetDevice(c->opt.device));
+    b2_h2_run_status* d_rs = reinterpret_cast<b2_h2_run_status*>(c->d_run_status);
+    b2_h2_call* d_calls = reinterpret_cast<b2_h2_call*>(c->d_msgs);                    // 64 B each, like b2_msg_desc
+    c->h2_last_in = 0; c->h2_last_out = 0;       // the device copies of the last h2 batch are about to be overwritten
+    CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
+    CU(cudaMemcpyAsync(c->d_meta, runs, sizeof(b2_run) * (size_t)n_runs, cudaMemcpyHostToDevice, c->stream));
+    k_h2_client_consume<<<(n_runs + 31) / 32, 32, 0, c->stream>>>(c->d_bytes, (const b2_run*)c->d_meta, n_runs, c->d_h2, c->d_hpack,
+                                                                   d_rs, d_calls, per_run_calls, c->d_unz, region, h2_pool(c));
+    CU(cudaMemcpyAsync(rs, d_rs, sizeof(b2_h2_run_status) * (size_t)n_runs, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    // as b2_h2_process_batch: three strided copies of what was produced, then the calls are compacted into one list (run order)
+    uint32_t total = 0, max_calls = 0, max_ctrl = 0, max_blob = 0;
+    for (uint32_t r = 0; r < n_runs; r++) {
+        total += rs[r].n_msgs; if (rs[r].n_msgs > max_calls) max_calls = rs[r].n_msgs;
+        if (rs[r].ctrl_len > max_ctrl) max_ctrl = rs[r].ctrl_len;
+        if (rs[r].first_msg > max_blob) max_blob = rs[r].first_msg;             // (the kernel reports the blob bytes it used here)
+    }
+    std::vector<b2_h2_call> tmp((size_t)n_runs * (max_calls ? max_calls : 1));
+    if (max_calls) CU(cudaMemcpy2DAsync(tmp.data(), sizeof(b2_h2_call) * (size_t)max_calls, d_calls, sizeof(b2_h2_call) * (size_t)per_run_calls,
+                                        sizeof(b2_h2_call) * (size_t)max_calls, n_runs, cudaMemcpyDeviceToHost, c->stream));
+    if (max_ctrl) CU(cudaMemcpy2DAsync(out, region, c->d_unz, region, max_ctrl, n_runs, cudaMemcpyDeviceToHost, c->stream));
+    if (max_blob) CU(cudaMemcpy2DAsync((uint8_t*)out + region / 4, region, c->d_unz + region / 4, region, max_blob, n_runs, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    total = 0;
+    for (uint32_t r = 0; r < n_runs; r++) {
+        if (rs[r].n_msgs) memcpy(calls + total, tmp.data() + (size_t)r * max_calls, sizeof(b2_h2_call) * (size_t)rs[r].n_msgs);
+        rs[r].first_msg = total; total += rs[r].n_msgs;
+    }
+    *n_calls = total;                            // (h2_last_in / h2_last_out stay 0: b2_h2_pack_responses may not read a client batch)
+    c->uploaded = false; c->executed = false;
     return B2_OK;
 }
 

@@ -865,12 +865,13 @@ __global__ void __launch_bounds__(kH2PackWarps * 32) k_h2_pack(const uint8_t* by
 }
 
 // ---------------------------------------------------------------------------------------------------------
+constexpr uint32_t kH2ClientMode = 1u;                            // H2Conn::pad0 bit of a connection opened by k_h2_client_conn_reset
 // Client side: H2UnsentRequest::New (:1382-1453, the header list) + AppendAndDestroySelf (:1496-1592) + PackH2Message (:1310-1380).
 // The same split as k_h2_pack: one warp per connection, lane 0 runs the serial part (stream id, windows, HPACK encode against the
 // connection's table) into shared memory, the warp writes the frames.
 constexpr uint32_t kH2ReqFragCap = 2048;
 __global__ void __launch_bounds__(kH2PackWarps * 32) k_h2_pack_req(const uint8_t* bytes, const b2_h2_request* reqs, const uint32_t* group_first, uint32_t n_groups,
-                                                                   H2Conn* conns, uint8_t* out, b2_h2_request_result* results) {
+                                                                   H2Conn* conns, uint8_t* out, b2_h2_request_result* results, H2Pool pool) {
     __shared__ __align__(16) uint8_t s_buf[kH2PackWarps][2][kH2ReqFragCap];
     const uint32_t lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     const uint32_t g = blockIdx.x * kH2PackWarps + w;
@@ -885,12 +886,28 @@ __global__ void __launch_bounds__(kH2PackWarps * 32) k_h2_pack_req(const uint8_t
         if (lane == 0) {
             H2Conn& c = conns[R.conn];
             if (!c.preface_sent) { c.preface_sent = 1; pre = 1; }
-            if (c.last_sent_stream_id > 0x7FFFFFFFll) st = B2_H2_REQ_RUNOUT;                      // AllocateClientStreamId
+            // a connection whose frames the device parses (k_h2_client_conn_reset) also keeps the pending-stream map of
+            // AppendAndDestroySelf / TryToInsertStream (:1529-1564, :425-436); the pool slot is a device capacity checked up front
+            const bool client = c.pad0 & kH2ClientMode;
+            H2Stream* const S = pool.streams + (size_t)R.conn * pool.pending;
+            int slot = -1;
+            if (client && c.n_pending > c.r_max_concurrent_streams) st = B2_H2_REQ_ELIMIT;                      // no id consumed
+            else if (client && (slot = h2_find(S, pool.pending, -1)) < 0) st = B2_H2_REQ_NO_ROOM;
+            else if (c.last_sent_stream_id > 0x7FFFFFFFll) st = B2_H2_REQ_RUNOUT;                      // AllocateClientStreamId
             else {
                 sid = (uint32_t)c.last_sent_stream_id; c.last_sent_stream_id += 2;
                 // ConsumeWindowSize (:1199-1219) on a stream that starts with the peer's initial window (Init :1176-1181)
                 if (data_size && ((long long)c.r_stream_window_size < (long long)data_size || c.remote_window_left < (long long)data_size)) st = B2_H2_REQ_ELIMIT;
-                else {
+                else if (client && c.last_received_stream_id >= 0 && (int32_t)sid > c.last_received_stream_id) {   // after GOAWAY (_goaway_stream_id)
+                    c.remote_window_left -= (long long)data_size;                  // (taken by ConsumeWindowSize before TryToInsertStream refuses)
+                    st = B2_H2_REQ_LOGOFF;
+                } else {
+                    if (client) {
+                        H2Stream& ns = S[slot];
+                        ns.id = (int32_t)sid; ns.hdr_len = 0; ns.n_headers = 0; ns.body_len = 0; ns.stream_ended = 0; ns.body_input_off = 0;
+                        ns.remote_window_left = (long long)c.r_stream_window_size - (long long)data_size; ns.deferred_wu = 0;
+                        c.n_pending++;
+                    }
                     c.remote_window_left -= (long long)data_size;
                     const bool never = c.r_header_table_size == 0;
                     uint8_t* f = frag;
@@ -975,5 +992,517 @@ __global__ void k_h2_peer_update(H2Conn* conns, uint32_t conn, b2_h2_peer_update
     }
 }
 __global__ void k_h2_set_next_stream_id(H2Conn* conns, uint32_t conn, uint32_t next_id) { conns[conn].last_sent_stream_id = next_id; }
+
+// ---------------------------------------------------------------------------------------------------------
+// The receiving half of a client connection: ParseH2Message on a socket created by connect (H2Context::Consume :467-543, client
+// branches) -> H2StreamContext::OnEndStream (:825-846) / OnResetStream (:781-823) / OnGoAway (:959-1004) -> what ProcessHttpResponse
+// (policy/http_rpc_protocol.cpp:349-564) decides before the response body is parsed.  A connection opened by k_h2_client_conn_reset
+// carries kH2ClientMode in H2Conn::pad0; on such a connection H2Conn::last_received_stream_id holds _goaway_stream_id instead (the
+// client never updates _last_received_stream_id: it stays -1, which is what its GOAWAY frames carry).  Server connections never
+// reach this code, and this code never touches a server connection.
+constexpr uint32_t kH2Abandoned = 2u;                             // H2Stream::stream_ended bit on client streams: AddAbandonedStream
+constexpr uint32_t kH2ErrMax = 2048;                              // FLAGS_http_max_error_length (http_rpc_protocol.cpp)
+__global__ void k_h2_client_conn_reset(H2Conn* conns, HpackState* hps, uint32_t conn, H2Pool pool) {
+    // H2Context(socket, NULL) + Init (:324-371): at the default client flags _unack_local_settings equals H2Settings(), which is also
+    // _local_settings until the server ACKs, so l_stream_window_size / l_max_frame_size need no second copy
+    h2_conn_init(conns[conn], pool.streams + (size_t)conn * pool.pending, pool.pending);
+    conns[conn].pad0 = kH2ClientMode;                             // (last_received_stream_id = -1 = _goaway_stream_id)
+    HpackState& h = hps[conn]; h.max_size = 4096; h.size = 0; h.count = 0; h.head = 0; h.byte_head = 0;
+}
+// AddAbandonedStream (:1140-1143): marked now, dropped by the ClearAbandonedStreams of the connection's next client parse
+__global__ void k_h2_client_abandon(H2Conn* conns, uint32_t conn, const uint32_t* ids, uint32_t n, H2Pool pool) {
+    if (!(conns[conn].pad0 & kH2ClientMode)) return;
+    H2Stream* S = pool.streams + (size_t)conn * pool.pending;
+    for (uint32_t i = 0; i < n; i++) { const int k = h2_find(S, pool.pending, (int32_t)ids[i]); if (k >= 0) S[k].stream_ended |= kH2Abandoned; }
+}
+__device__ __forceinline__ int32_t h2c_status_of_error(uint32_t e) {                     // H2ErrorToStatusCode (http2.cpp:88-112)
+    switch (e) {
+    case 0: return 200;
+    case 4: return 504;
+    case 5: return 400;
+    case 7: case 8: case 11: return 503;
+    case 12: return 401;
+    case 13: return 505;
+    default: return 500;
+    }
+}
+// strtol(c_str, NULL, 10) cast to int: leading white space, a sign, digits; saturates at LONG_MIN / LONG_MAX like glibc
+__device__ __forceinline__ int32_t h2c_strtol(const uint8_t* v, uint32_t vl) {
+    const uint32_t m = cstr_len(v, vl);
+    uint32_t i = 0;
+    while (i < m && (v[i] == ' ' || (v[i] >= 9 && v[i] <= 13))) i++;
+    bool neg = false;
+    if (i < m && (v[i] == '+' || v[i] == '-')) { neg = v[i] == '-'; i++; }
+    unsigned long long acc = 0; bool sat = false;
+    for (; i < m && v[i] >= '0' && v[i] <= '9'; i++) {
+        if (acc > (0x7fffffffffffffffull - (v[i] - '0')) / 10) sat = true;
+        else acc = acc * 10 + (v[i] - '0');
+    }
+    long long r = sat ? (neg ? (long long)0x8000000000000000ull : 0x7fffffffffffffffll) : (neg ? -(long long)acc : (long long)acc);
+    return (int32_t)(uint32_t)(unsigned long long)r;
+}
+__device__ __forceinline__ int32_t h2c_grpc_errno(int32_t s) {                           // GrpcStatusToErrorCode (grpc.cpp:83-125)
+    switch (s) {
+    case 0: return 0;
+    case 1: return 125;                                          // ECANCELED
+    case 3: return 22;                                           // EINVAL
+    case 4: return 1008;                                         // ERPCTIMEDOUT
+    case 6: return 17;                                           // EEXIST
+    case 7: return 1;                                            // EPERM
+    case 8: return 2004;                                         // ELIMIT
+    case 12: return 1002;                                        // ENOMETHOD
+    case 16: return 1004;                                        // ERPCAUTH
+    default: return 2001;                                        // EINTERNAL
+    }
+}
+__device__ __forceinline__ const char* h2c_grpc_name(int32_t s) {                         // GrpcStatusToString (grpc.cpp:29-51)
+    const char* const names[18] = { "GRPC_OK", "GRPC_CANCELED", "GRPC_UNKNOWN", "GRPC_INVALIDARGUMENT", "GRPC_DEADLINEEXCEEDED", "GRPC_NOTFOUND",
+        "GRPC_ALREADYEXISTS", "GRPC_PERMISSIONDENIED", "GRPC_RESOURCEEXHAUSTED", "GRPC_FAILEDPRECONDITION", "GRPC_ABORTED", "GRPC_OUTOFRANGE",
+        "GRPC_UNIMPLEMENTED", "GRPC_INTERNAL", "GRPC_UNAVAILABLE", "GRPC_DATALOSS", "GRPC_UNAUTHENTICATED", "GRPC_MAX" };
+    return (s >= 0 && s < 18) ? names[s] : "Unknown-GrpcStatus";
+}
+__device__ __forceinline__ const char* h2c_reason(int32_t sc) {                           // HttpReasonPhrase (http_status_code.cpp:27-115)
+    switch (sc) {
+    case 100: return "Continue"; case 101: return "Switching Protocols";
+    case 200: return "OK"; case 201: return "Created"; case 202: return "Accepted"; case 203: return "Non-Authoritative Informational";
+    case 204: return "No Content"; case 205: return "Reset Content"; case 206: return "Partial Content";
+    case 300: return "Multiple Choices"; case 301: return "Move Permanently"; case 302: return "Found"; case 303: return "See Other";
+    case 304: return "Not Modified"; case 305: return "Use Proxy"; case 307: return "Temporary Redirect";
+    case 400: return "Bad Request"; case 401: return "Unauthorized"; case 402: return "Payment Required"; case 403: return "Forbidden";
+    case 404: return "Not Found"; case 405: return "Method Not Allowed"; case 406: return "Not Acceptable";
+    case 407: return "Proxy Authentication Required"; case 408: return "Request Timeout"; case 409: return "Conflict"; case 410: return "Gone";
+    case 411: return "Length Required"; case 412: return "Precondition Failed"; case 413: return "Request Entity Too Large";
+    case 414: return "Request-URI Too Long"; case 415: return "Unsupported Media Type"; case 416: return "Requested Range Not Satisfiable";
+    case 417: return "Expectation Failed";
+    case 500: return "Internal Server Error"; case 501: return "Not Implemented"; case 502: return "Bad Gateway"; case 503: return "Service Unavailable";
+    case 504: return "Gateway Timeout"; case 505: return "HTTP Version Not Supported";
+    default: return nullptr;                                     // "Unknown status code (%d)"
+    }
+}
+__device__ __forceinline__ uint32_t h2c_hex(uint8_t c) {                                   // hex_to_int (grpc.cpp:143-152)
+    return (c >= 'a' && c <= 'f') ? c - 'a' + 10u : (c >= 'A' && c <= 'F') ? c - 'A' + 10u : (c >= '0' && c <= '9') ? c - '0' : 0u;
+}
+// PercentDecode (grpc.cpp:154-170) of v[0..vl) into dst (NULL: length only); SetFailed("%s", decoded.c_str()) stops at the first NUL
+__device__ __forceinline__ uint32_t h2c_percent_decode(const uint8_t* v, uint32_t vl, uint8_t* dst) {
+    uint32_t o = 0;
+    for (uint32_t i = 0; i < vl; i++) {
+        uint8_t ch = v[i];
+        if (ch == '%' && i + 2 < vl) { ch = (uint8_t)(h2c_hex(v[i + 1]) * 16 + h2c_hex(v[i + 2])); i += 2; }
+        if (ch == 0) break;
+        if (dst) dst[o] = ch;
+        o++;
+    }
+    return o;
+}
+// the record of header `name` in the MERGED list (what HttpHeader::GetHeader sees): value pointer and length, false if absent.  GetHeader
+// compares case-insensitively; an exact compare is the same here because HPacker::Decode lowercases every name (hpack.cpp:755) and the
+// decoder above does too, so no upper-case name reaches the records
+__device__ __forceinline__ bool h2c_get(const uint8_t* recs, uint32_t len, const char* name, const uint8_t*& v, uint32_t& vl) {
+    for (uint32_t q = 0; q < len;) {
+        const uint32_t nl = recs[q] | ((uint32_t)recs[q + 1] << 8), l2 = recs[q + 2] | ((uint32_t)recs[q + 3] << 8);
+        if (lit_eq(recs + q + 4, cstr_len(recs + q + 4, nl), name)) { v = recs + q + 4 + nl; vl = l2; return true; }
+        q += 4 + nl + l2;
+    }
+    return false;
+}
+__device__ __forceinline__ bool h2c_name_eq(const uint8_t* a, uint32_t an, const uint8_t* b, uint32_t bn) {   // case-insensitive, as c_str
+    an = cstr_len(a, an); bn = cstr_len(b, bn);
+    if (an != bn) return false;
+    for (uint32_t i = 0; i < an; i++) if (lc(a[i]) != lc(b[i])) return false;
+    return true;
+}
+// The stream's decoded fields (every record, pseudo-headers included, in wire order) folded the way ConsumeHeaders fills HttpHeader
+// (:1233-1288): ":status" -> status_code (strtol, last one wins), "content-type" -> set_content_type (the last value wins, one record at
+// the place of the first), "set-cookie" -> one record each (AddHeader), every other name -> AppendHeader (http_header.cpp:100-117): the
+// first record of a name (case-insensitive) takes the values of all later ones, joined with "," ("; " for "cookie"), an empty value is
+// replaced instead of joined.  brpc's header map has no order; the records here keep the order in which names first appear.
+__device__ __forceinline__ uint32_t h2c_merge(const uint8_t* raw, uint32_t raw_len, uint8_t* out, uint32_t& n_out, int32_t& status) {
+    uint32_t o = 0; n_out = 0;
+    for (uint32_t q = 0; q < raw_len;) {
+        const uint32_t nl = raw[q] | ((uint32_t)raw[q + 1] << 8), vl = raw[q + 2] | ((uint32_t)raw[q + 3] << 8);
+        const uint8_t* nm = raw + q + 4; const uint8_t* v = nm + nl;
+        const uint32_t cn = cstr_len(nm, nl);
+        const uint32_t next = q + 4 + nl + vl;
+        if (cn && nm[0] == ':') {
+            if (lit_eq(nm, cn, ":status")) status = h2c_strtol(v, vl);
+            q = next; continue;
+        }
+        const bool ct = lit_eq(nm, cn, "content-type"), cookie_set = h2c_name_eq(nm, nl, (const uint8_t*)"set-cookie", 10);
+        bool first = true;
+        if (!cookie_set) for (uint32_t p = 0; p < q && first;) {   // an earlier record of the same header already took this one
+            const uint32_t pl = raw[p] | ((uint32_t)raw[p + 1] << 8), pv = raw[p + 2] | ((uint32_t)raw[p + 3] << 8);
+            const uint8_t* pn = raw + p + 4;
+            const uint32_t pc = cstr_len(pn, pl);
+            if (!(pc && pn[0] == ':')) {
+                if (ct) { if (lit_eq(pn, pc, "content-type")) first = false; }
+                else if (!lit_eq(pn, pc, "content-type") && h2c_name_eq(pn, pl, nm, nl)) first = false;
+            }
+            p += 4 + pl + pv;
+        }
+        if (!first) { q = next; continue; }
+        uint8_t* rec = out + o;
+        for (uint32_t i = 0; i < nl; i++) rec[4 + i] = nm[i];
+        uint32_t ol = 0;
+        uint8_t* val = rec + 4 + nl;
+        if (cookie_set) { for (uint32_t i = 0; i < vl; i++) val[i] = v[i]; ol = vl; }
+        else {
+            const bool semi = h2c_name_eq(nm, nl, (const uint8_t*)"cookie", 6);
+            for (uint32_t p = q; p < raw_len;) {
+                const uint32_t pl = raw[p] | ((uint32_t)raw[p + 1] << 8), pv = raw[p + 2] | ((uint32_t)raw[p + 3] << 8);
+                const uint8_t* pn = raw + p + 4; const uint8_t* pvp = pn + pl;
+                const uint32_t pc = cstr_len(pn, pl);
+                const bool same = !(pc && pn[0] == ':') && (ct ? lit_eq(pn, pc, "content-type") : (!lit_eq(pn, pc, "content-type") && h2c_name_eq(pn, pl, nm, nl)));
+                if (same) {
+                    if (ct || ol == 0) { for (uint32_t i = 0; i < pv; i++) val[i] = pvp[i]; ol = pv; }
+                    else {
+                        if (semi) { val[ol++] = ';'; val[ol++] = ' '; } else val[ol++] = ',';
+                        for (uint32_t i = 0; i < pv; i++) val[ol + i] = pvp[i];
+                        ol += pv;
+                    }
+                }
+                p += 4 + pl + pv;
+            }
+        }
+        rec[0] = (uint8_t)nl; rec[1] = (uint8_t)(nl >> 8); rec[2] = (uint8_t)ol; rec[3] = (uint8_t)(ol >> 8);
+        o += 4 + nl + ol; n_out++;
+        q = next;
+    }
+    return o;
+}
+__device__ __forceinline__ uint32_t h2c_puts(uint8_t* dst, uint32_t o, const char* s) { for (uint32_t i = 0; s[i]; i++) { if (dst) dst[o] = (uint8_t)s[i]; o++; } return o; }
+__device__ __forceinline__ uint32_t h2c_putd(uint8_t* dst, uint32_t o, int32_t v) {
+    uint8_t tmp[12]; const uint32_t n = put_dec_i32_h2(tmp, v);
+    for (uint32_t i = 0; i < n; i++) { if (dst) dst[o] = tmp[i]; o++; }
+    return o;
+}
+// ProcessHttpResponse's decisions for a protobuf-typed call (http_rpc_protocol.cpp:390-533, up to the body parse): the error code and the
+// text SetFailed receives (written to dst unless NULL), from the merged header records and the body (gRPC: without its prefix)
+__device__ __forceinline__ uint32_t h2c_verdict(const uint8_t* recs, uint32_t rlen, int32_t sc, bool is_grpc, bool prefix_ok, bool compressed,
+                                                const uint8_t* body, uint32_t body_len, int32_t grpc_status, bool has_grpc_status,
+                                                uint8_t* dst, int32_t& code) {
+    code = 0;
+    if (is_grpc) {
+        if (!prefix_ok) { code = 2002; return h2c_puts(dst, 0, "Invalid gRPC response"); }                      // ERESPONSE
+        if (has_grpc_status && grpc_status != 0) {
+            code = h2c_grpc_errno(grpc_status);
+            const uint8_t* m; uint32_t ml;
+            if (h2c_get(recs, rlen, "grpc-message", m, ml)) return h2c_percent_decode(m, ml, dst);
+            return h2c_puts(dst, 0, h2c_grpc_name(grpc_status));
+        }
+    }
+    if (sc < 200 || sc >= 300) {                                 // EHTTP, "HTTP/%d.%d %d %s[: body]" then "%s" of its c_str
+        code = 1010;
+        uint32_t o = h2c_puts(dst, 0, "HTTP/2.0 ");
+        o = h2c_putd(dst, o, sc);
+        if (dst) dst[o] = ' ';
+        o++;
+        const char* rp = h2c_reason(sc);
+        if (rp) o = h2c_puts(dst, o, rp);
+        else { o = h2c_puts(dst, o, "Unknown status code ("); o = h2c_putd(dst, o, sc); o = h2c_puts(dst, o, ")"); }
+        if (body_len) {
+            o = h2c_puts(dst, o, ": ");
+            const uint32_t k = body_len < kH2ErrMax ? body_len : kH2ErrMax;
+            for (uint32_t i = 0; i < k && body[i]; i++) { if (dst) dst[o] = body[i]; o++; }
+        }
+        return o;
+    }
+    if (is_grpc && compressed) {
+        const uint8_t* e; uint32_t el;
+        if (!h2c_get(recs, rlen, "grpc-encoding", e, el)) { code = 2002; return h2c_puts(dst, 0, "Fail to find header `grpc-encoding' in compressed gRPC response"); }
+    }
+    return 0;
+}
+
+// One thread per client connection run, like k_h2_consume.  Every stream that leaves the connection becomes one b2_h2_call.
+__global__ void k_h2_client_consume(const uint8_t* bytes, const b2_run* runs, uint32_t n_runs, H2Conn* conns, HpackState* hps,
+                                    b2_h2_run_status* rs, b2_h2_call* calls, uint32_t call_cap_per_run, uint8_t* out, uint32_t region, H2Pool pool) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_runs) return;
+    const uint32_t conn = (uint32_t)runs[r].socket_id;
+    const uint32_t P = pool.pending, kH2StreamBytes = pool.stream_bytes;
+    H2Stream* const S = pool.streams + (size_t)conn * P;
+    uint8_t* const slots = pool.slots + (size_t)conn * P * kH2StreamBytes;
+    const uint32_t run_off = runs[r].offset;
+    const uint8_t* in = bytes + run_off; const uint32_t n = runs[r].length;
+    H2Conn& c = conns[conn];
+    HpackState& hp = hps[conn];
+    H2Out o; o.base = out + (size_t)r * region; o.ctrl_cap = region / 4; o.ctrl_len = 0; o.blob_off = region / 4; o.blob_end = region; o.overflow = false;
+    b2_h2_call* cout = calls + (size_t)r * call_cap_per_run;
+    const uint32_t gbase = r * region;
+    uint32_t n_calls = 0, pos = 0, last_ok = 0, perr = B2_PARSE_ERROR_NOT_ENOUGH_DATA;
+    bool no_room = false;
+    if (!(c.pad0 & kH2ClientMode)) {                             // not a client connection: nothing is read, nothing changes
+        b2_h2_run_status st; st.consumed = 0; st.parse_error = B2_PARSE_ERROR_TRY_OTHERS; st.n_msgs = 0; st.first_msg = 0;
+        st.ctrl_off = r * region; st.ctrl_len = 0; st.remote_max_frame_size = 0; st.remote_stream_window_size = 0;
+        rs[r] = st;
+        return;
+    }
+    // the stream in slot k leaves the connection as a call (it is already out of the pending map; its bytes are still in the slot)
+    auto emit = [&](int k, int32_t sid, uint32_t how, int32_t status_override) -> bool {
+        const H2Stream& st = S[k];
+        const uint8_t* slot = slots + (size_t)k * kH2StreamBytes;
+        const bool in_input = st.body_input_off != 0;
+        const uint32_t need1 = ((st.hdr_len + 15u) & ~15u) + (in_input ? 0u : ((st.body_len + 15u) & ~15u));
+        if (n_calls >= call_cap_per_run || o.blob_off + need1 > o.blob_end) return false;
+        const uint32_t ho = o.blob_off, bo = ho + ((st.hdr_len + 15u) & ~15u), eo = o.blob_off + need1;
+        b2_h2_call m;
+        m.run_idx = r; m.stream_id = (uint32_t)sid; m.how = how; m.flags = 0;
+        int32_t sc = 200;                                        // HttpHeader() (http_header.cpp:30)
+        uint32_t nh = 0;
+        const uint32_t ml = h2c_merge(slot, st.hdr_len, o.base + ho, nh, sc);
+        if (status_override >= 0) sc = status_override;
+        if (!in_input) thread_copy(o.base + bo, slot + kH2HdrBytes, st.body_len);
+        m.headers_off = gbase + ho; m.headers_len = ml; m.n_headers = nh;
+        m.body_off = in_input ? st.body_input_off : gbase + bo; m.body_len = st.body_len;
+        if (in_input) m.flags |= B2_H2_FLAG_BODY_IN_INPUT;
+        const uint8_t* body_p = in_input ? bytes + st.body_input_off : o.base + bo;
+        m.status_code = sc;
+        const uint8_t* recs = o.base + ho;
+        const uint8_t* v; uint32_t vl;
+        bool is_grpc = false;
+        if (h2c_get(recs, ml, "content-type", v, vl)) (void)h2_content_type(v, cstr_len(v, vl), is_grpc);
+        bool prefix_ok = false, compressed = false;
+        const uint8_t* msg_p = body_p; uint32_t msg_len = st.body_len;
+        m.msg_off = 0; m.msg_len = 0;
+        if (is_grpc) {                                           // RemoveGrpcPrefix (policy/http_rpc_protocol.cpp:264-277)
+            m.flags |= B2_H2_FLAG_GRPC;
+            if (st.body_len == 0) { prefix_ok = true; m.msg_off = m.body_off; }
+            else if (st.body_len >= 5) {
+                compressed = body_p[0] != 0;
+                if ((unsigned long long)load_be32(body_p + 1) + 5ull == st.body_len) { prefix_ok = true; m.msg_off = m.body_off + 5; m.msg_len = st.body_len - 5; }
+            }
+            if (prefix_ok) { m.flags |= B2_H2_FLAG_GRPC_PREFIX_OK; msg_p = body_p + (st.body_len ? 5 : 0); msg_len = m.msg_len; }
+            if (compressed) m.flags |= B2_H2_FLAG_GRPC_COMPRESSED;
+        }
+        const bool has_gs = h2c_get(recs, ml, "grpc-status", v, vl);
+        m.grpc_status = has_gs ? h2c_strtol(v, vl) : -1;
+        if (has_gs) m.flags |= B2_H2_CALL_HAS_GRPC_STATUS;
+        int32_t code = 0;
+        const uint32_t el = h2c_verdict(recs, ml, sc, is_grpc, prefix_ok, compressed, msg_p, msg_len, m.grpc_status, has_gs, nullptr, code);
+        if (eo + ((el + 15u) & ~15u) > o.blob_end) return false;
+        (void)h2c_verdict(recs, ml, sc, is_grpc, prefix_ok, compressed, msg_p, msg_len, m.grpc_status, has_gs, o.base + eo, code);
+        m.error_code = code; m.error_off = el ? gbase + eo : 0; m.error_len = el;
+        o.blob_off = eo + ((el + 15u) & ~15u);
+        cout[n_calls++] = m;
+        return true;
+    };
+    // ClearAbandonedStreams (:1145-1157): ParseH2Message runs it each time it returns, i.e. after every frame that produced a message and
+    // when the input ends; RemoveStreamAndDeferWU of each, here in ascending id order (brpc pops the most recent first)
+    auto clear_abandoned = [&]() {
+        for (;;) {
+            int best = -1;
+            for (uint32_t i = 0; i < P; i++) if (S[i].id >= 0 && (S[i].stream_ended & kH2Abandoned) && (best < 0 || S[i].id < S[best].id)) best = (int)i;
+            if (best < 0) break;
+            (void)h2_remove_stream(c, S, P, o, S[best].id);
+        }
+    };
+    uint32_t n_cleared = 0;                                      // n_calls when abandoned streams were last cleared
+    for (;;) {
+        if (n_calls != n_cleared) { clear_abandoned(); n_cleared = n_calls; }   // the previous frame returned a message
+        if (o.overflow || no_room) { perr = B2_PARSE_ERROR_NO_RESOURCE; break; }
+        if (c.conn_state == 0) { c.conn_state = 1; last_ok = pos; continue; }   // client side: READY without reading a preface (:489-491)
+        // ---- ConsumeFrameHead (:438-465)
+        const uint32_t left = n - pos;
+        if (left < 3) break;
+        const uint32_t length = ((uint32_t)in[pos] << 16) | ((uint32_t)in[pos + 1] << 8) | in[pos + 2];
+        if (length > c.l_max_frame_size) { perr = B2_PARSE_ERROR_ABSOLUTELY_WRONG; break; }
+        if ((unsigned long long)(left - 3) < 6ull + length) break;
+        const uint32_t type = in[pos + 3], flags = in[pos + 4], sid_raw = load_be32(in + pos + 5);
+        if (sid_raw & 0x80000000u) { perr = B2_PARSE_ERROR_ABSOLUTELY_WRONG; break; }
+        const int32_t sid = (int32_t)sid_raw;
+        pos += 9;
+        if (type > 9) { perr = B2_PARSE_ERROR_ABSOLUTELY_WRONG; break; }
+        const uint8_t* pl = in + pos;
+        uint32_t used = 0;
+        H2Res res = h2_ok();
+        uint32_t how = B2_H2_CALL_ENDED; int32_t sc_over = -1;
+        bool goaway = false; int32_t goaway_last = 0;
+        switch (type) {
+        case 0: {                                                    // ---- OnData (:699-779), as on the server side
+            uint32_t frag = length, padl = 0;
+            if ((flags & 0x8) && length == 0) { res = h2_err(6); break; }
+            if (flags & 0x8) { frag--; padl = pl[used++]; }
+            if (frag < padl) { res = h2_err(6); break; }
+            frag -= padl;
+            const int k = h2_find(S, P, sid);
+            if (k < 0) {
+                used += frag + padl;
+                const long long acc = (long long)frag;
+                const long long quota = (long long)(c.l_stream_window_size / (c.n_pending + 1));
+                long long tmp_deferred = (long long)frag;
+                if (acc >= quota) {
+                    if (acc > (long long)c.l_stream_window_size) { h2_defer_wu(c, o, tmp_deferred); res = h2_err(5, sid); break; }
+                    const long long swu = tmp_deferred; tmp_deferred = 0;
+                    if (swu > 0) { h2_write_wu(o, (uint32_t)sid, swu); const long long cw = swu + c.deferred_window_update; c.deferred_window_update = 0; h2_write_wu(o, 0, cw); }
+                }
+                h2_defer_wu(c, o, tmp_deferred);
+                res = h2_err(5, sid);
+                break;
+            }
+            H2Stream& st = S[k];
+            if (st.body_len == 0 && (flags & 0x1) && frag) { st.body_input_off = run_off + pos + used; st.body_len = frag; }
+            else {
+                if (kH2HdrBytes + st.body_len + frag > kH2StreamBytes) { no_room = true; break; }
+                thread_copy(slots + (size_t)k * kH2StreamBytes + kH2HdrBytes + st.body_len, pl + used, frag);
+                st.body_len += frag;
+            }
+            used += frag + padl;
+            const long long acc = (long long)frag + st.deferred_wu; st.deferred_wu += frag;
+            const long long quota = (long long)(c.l_stream_window_size / (c.n_pending + 1));
+            if (acc >= quota) {
+                if (acc > (long long)c.l_stream_window_size) { res = h2_err(3, sid); break; }
+                const long long swu = st.deferred_wu; st.deferred_wu = 0;
+                if (swu > 0) { h2_write_wu(o, (uint32_t)sid, swu); const long long cw = swu + c.deferred_window_update; c.deferred_window_update = 0; h2_write_wu(o, 0, cw); }
+            }
+            if (flags & 0x1) res = h2_end_stream(c, S, P, o, sid);
+            break; }
+        case 1: {                                                    // ---- OnHeaders (:545-653), client side
+            if (sid == 0) { res = h2_err(1); break; }
+            const bool has_padding = flags & 0x8, has_priority = flags & 0x20;
+            if (length < (has_priority ? 5u : 0u) + (has_padding ? 1u : 0u)) { res = h2_err(6); break; }
+            uint32_t frag = length, padl = 0;
+            if (has_padding) { padl = pl[used++]; frag--; }
+            if (has_priority) { used += 5; frag -= 5; }
+            if (frag < padl) { res = h2_err(6); break; }
+            frag -= padl;
+            const int k = h2_find(S, P, sid);
+            if (k < 0) {
+                // unknown stream (:600-606): decoded into a throw-away stream so that the HPACK table advances, then dropped; a failed
+                // decode leaves the rest of the payload unread, as the throw-away OnHeaders returns before moving the iterator
+                if (o.blob_off + kH2HdrBytes > o.blob_end) { no_room = true; break; }
+                H2Stream tmp; tmp.hdr_len = 0; tmp.n_headers = 0;
+                if (h2_consume_headers(c, hp, tmp, o.base + o.blob_end - kH2HdrBytes, pl + used, frag, no_room) == 0) used += frag + padl;
+                break;
+            }
+            H2Stream& st = S[k];
+            if (h2_consume_headers(c, hp, st, slots + (size_t)k * kH2StreamBytes, pl + used, frag, no_room) < 0) { if (!no_room) res = h2_err(1); break; }
+            used += frag + padl;
+            if (flags & 0x4) { if (flags & 0x1) res = h2_end_stream(c, S, P, o, sid); }
+            else if (flags & 0x1) st.stream_ended |= 1u;
+            break; }
+        case 2: res = h2_err(1); break;                              // OnPriority (:918-922)
+        case 3: {                                                    // ---- OnResetStream (:781-823), client side: the stream leaves as a call
+            if (length != 4) { res = h2_err(6); break; }
+            const uint32_t e = load_be32(pl); used += 4;
+            const int k = h2_remove_stream(c, S, P, o, sid);
+            if (k >= 0) { res.kind = 1; res.slot = k; res.err_stream = sid; how = B2_H2_CALL_RESET_BY_PEER; sc_over = h2c_status_of_error(e); }
+            break; }
+        case 4: {                                                    // ---- OnSettings (:848-916)
+            if (sid != 0) { res = h2_err(1); break; }
+            if (flags & 0x1) {                                       // ACK: _local_settings = _unack_local_settings
+                if (length != 0) { res = h2_err(1); break; }
+                c.l_stream_window_size = 256 * 1024; c.l_max_frame_size = 16384;
+                break;
+            }
+            const long long old_sw = (long long)c.r_stream_window_size;
+            uint32_t t_hts, t_push, t_mcs, t_sws, t_mfs, t_mhl;
+            if (!c.remote_settings_received) { t_hts = 4096; t_push = 0; t_mcs = 0xffffffffu; t_sws = 256 * 1024; t_mfs = 16384; t_mhl = 0xffffffffu; }
+            else { t_hts = c.r_header_table_size; t_push = c.r_enable_push; t_mcs = c.r_max_concurrent_streams; t_sws = c.r_stream_window_size; t_mfs = c.r_max_frame_size; t_mhl = c.r_max_header_list_size; }
+            bool okp = (length / 6) * 6 == length;
+            if (okp) for (uint32_t i = 0; i < length / 6; i++) {
+                const uint32_t id = ((uint32_t)pl[used] << 8) | pl[used + 1], value = load_be32(pl + used + 2);
+                used += 6;
+                if (id == 1) t_hts = value;
+                else if (id == 2) { if (value > 1) { okp = false; break; } t_push = value; }
+                else if (id == 3) t_mcs = value;
+                else if (id == 4) { if (value > (uint32_t)kH2MaxWindow) { okp = false; break; } t_sws = value; }
+                else if (id == 5) { if (value > 16777215u || value < 16384u) { okp = false; break; } t_mfs = value; }
+                else if (id == 6) t_mhl = value;
+            }
+            if (!c.remote_settings_received) {
+                if (!okp) { res = h2_err(1); break; }
+                c.remote_window_left -= (kH2MaxWindow - 65535);
+                c.remote_settings_received = 1;
+            }
+            c.r_header_table_size = t_hts; c.r_enable_push = t_push; c.r_max_concurrent_streams = t_mcs;
+            c.r_stream_window_size = t_sws; c.r_max_frame_size = t_mfs; c.r_max_header_list_size = t_mhl;
+            if (!okp) { res = h2_err(1); break; }
+            const long long diff = (long long)c.r_stream_window_size - old_sw;
+            bool flow_ok = true;
+            if (diff) for (uint32_t i = 0; i < P; i++) if (S[i].id >= 0) { if (!h2_add_window(S[i].remote_window_left, diff)) { flow_ok = false; break; } }
+            if (!flow_ok) { res = h2_err(3); break; }
+            uint8_t* p = h2_ack_room(o, 9); if (p) h2_put_head(p, 0, 4, 1, 0);
+            break; }
+        case 5: res = h2_err(1); break;                              // OnPushPromise (:924-928)
+        case 6: {                                                    // ---- OnPing (:930-952)
+            if (length != 8) { res = h2_err(6); break; }
+            if (sid != 0) { res = h2_err(1); break; }
+            if (flags & 0x1) break;
+            uint8_t* p = h2_ack_room(o, 17);
+            if (p) { h2_put_head(p, 8, 6, 1, 0); for (uint32_t i = 0; i < 8; i++) p[9 + i] = pl[i]; }
+            used += 8;
+            break; }
+        case 7: {                                                    // ---- OnGoAway (:959-1006), client side: RemoveGoAwayStreams (:388-414)
+            if (length < 8) { res = h2_err(6); break; }
+            if (sid != 0) { res = h2_err(1); break; }
+            if (flags) { res = h2_err(1); break; }
+            goaway_last = (int32_t)load_be32(pl + length - 8);       // after the debug data
+            used += length;
+            goaway = true;
+            break; }
+        case 8: {                                                    // ---- OnWindowUpdate (:1008-1038)
+            if (length != 4) { res = h2_err(6); break; }
+            const uint32_t inc = load_be32(pl); used += 4;
+            if ((inc & 0x80000000u) || inc == 0) { res = h2_err(1); break; }
+            if (sid == 0) { if (!h2_add_window(c.remote_window_left, (long long)inc)) res = h2_err(3); break; }
+            const int k = h2_find(S, P, sid);
+            if (k < 0) break;
+            if (!h2_add_window(S[k].remote_window_left, (long long)inc)) res = h2_err(3);
+            break; }
+        case 9: {                                                    // ---- OnContinuation (:655-697)
+            const int k = h2_find(S, P, sid);
+            used += length;
+            if (k < 0) {                                             // unknown stream: decoded and dropped (:659-665)
+                if (o.blob_off + kH2HdrBytes > o.blob_end) { no_room = true; break; }
+                H2Stream tmp; tmp.hdr_len = 0; tmp.n_headers = 0;
+                (void)h2_consume_headers(c, hp, tmp, o.base + o.blob_end - kH2HdrBytes, pl, length, no_room);
+                break;
+            }
+            H2Stream& st = S[k];
+            if (h2_consume_headers(c, hp, st, slots + (size_t)k * kH2StreamBytes, pl, length, no_room) < 0) { if (!no_room) res = h2_err(1); break; }
+            if ((flags & 0x4) && (st.stream_ended & 1u)) res = h2_end_stream(c, S, P, o, sid);
+            break; }
+        }
+        if (no_room) continue;
+        pos += used;
+        if (res.kind == 2) {
+            if (res.err_stream) {                                    // RST_STREAM; a stream of ours leaves as a call (:508-528)
+                uint8_t* p = h2_ack_room(o, 13);
+                if (p) { h2_put_head(p, 4, 3, 0, (uint32_t)res.err_stream); put_be32(p + 9, res.err); }
+                const int k = h2_remove_stream(c, S, P, o, res.err_stream);
+                last_ok = pos;
+                if (k >= 0 && !emit(k, res.err_stream, B2_H2_CALL_RESET_BY_US, h2c_status_of_error(res.err))) no_room = true;
+            } else {                                                 // GOAWAY with the client's _last_received_stream_id, always -1
+                uint8_t* p = h2_ack_room(o, 17);
+                if (p) { h2_put_head(p, 8, 7, 0, 0); put_be32(p + 9, 0xffffffffu); put_be32(p + 13, res.err); }
+                last_ok = pos;
+            }
+            continue;
+        }
+        last_ok = pos;
+        if (goaway) {
+            // SetLogOff + RemoveGoAwayStreams: _goaway_stream_id = last; the streams above it (all of them for 0) leave with status 503,
+            // without moving their deferred WINDOW_UPDATE (erase, not RemoveStreamAndDeferWU).  brpc walks its map in hash order; the
+            // calls here come in ascending stream id order.
+            c.last_received_stream_id = goaway_last;
+            for (;;) {
+                int best = -1;
+                for (uint32_t i = 0; i < P; i++)                     // (free records have id -1: a last_stream_id >= 2^31 is negative here)
+                    if (S[i].id >= 0 && S[i].id > goaway_last && (best < 0 || S[i].id < S[best].id)) best = (int)i;
+                if (best < 0) break;
+                const int32_t gid = S[best].id;
+                S[best].id = -1; c.n_pending--;
+                if (!emit(best, gid, B2_H2_CALL_GOAWAY, 503)) { no_room = true; break; }
+            }
+            continue;
+        }
+        if (res.kind == 1 && !emit(res.slot, res.err_stream, how, sc_over)) no_room = true;
+    }
+    clear_abandoned();
+    if (o.overflow) perr = B2_PARSE_ERROR_NO_RESOURCE;
+    b2_h2_run_status st; st.consumed = last_ok; st.parse_error = perr; st.n_msgs = n_calls; st.first_msg = o.blob_off - region / 4;
+    st.ctrl_off = r * region; st.ctrl_len = o.ctrl_len; st.remote_max_frame_size = c.r_max_frame_size; st.remote_stream_window_size = c.r_stream_window_size;
+    rs[r] = st;
+}
 #endif
 }  // namespace b2

@@ -21,8 +21,9 @@
  * (b2_set_protocols: hulu_pbrpc / sofa_pbrpc / nshead framing; rpc_dump files as a source), leaf codecs with the reference's signatures
  * (CRC32C, snappy), the client mirror (b2_pack_requests), replies the host produced (b2_pack_responses = SendRpcResponse), and the
  * h2/gRPC server path (b2_h2_process_batch = ParseH2Message, b2_h2_pack_responses = H2UnsentResponse + PackH2Message) whose
- * per-connection state lives on the device between calls, and the sending half of h2 client connections (b2_h2_pack_requests =
- * H2UnsentRequest::New + AppendAndDestroySelf; b2_h2_conn_peer_update mirrors the peer's SETTINGS / WINDOW_UPDATE).
+ * per-connection state lives on the device between calls, and both halves of h2 client connections (b2_h2_pack_requests =
+ * H2UnsentRequest::New + AppendAndDestroySelf; b2_h2_client_process_batch = ParseH2Message on a connected socket + what
+ * ProcessHttpResponse decides; or the host parses and b2_h2_conn_peer_update mirrors the peer's SETTINGS / WINDOW_UPDATE).
  */
 #ifndef B2RPC_H_
 #define B2RPC_H_
@@ -603,11 +604,17 @@ int  b2_h2_pack_responses(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const
  *   - HEADERS (+CONTINUATION) and the body as DATA frames split at the peer's max_frame_size, END_STREAM on the last frame, the
  *     deferred connection WINDOW_UPDATE; B2_H2_REQ_GRPC prepends AddGrpcPrefix's 5 bytes (policy/http_rpc_protocol.cpp:254-262).
  * `extra` headers: records {u16 name_len, u16 value_len (little endian), name, value} back to back at extra_off, extra_len bytes.
- * The pending-stream count against max_concurrent_streams (:1529) and GOAWAY (TryToInsertStream :425-436) belong to the
- * caller's correlation map, not to this call.  NOT built: the receiving half of a client connection (ParseH2Message on a socket
- * created by connect -> H2StreamContext::OnEndStream :823-846 -> ProcessHttpResponse) — the host's H2Context keeps parsing the
- * server's frames and mirrors what they change into the device's connection with b2_h2_conn_peer_update.  Requests of one
- * connection must be adjacent and in write order. */
+ * On a connection opened with b2_h2_conn_reset the pending-stream count against max_concurrent_streams (:1529) and GOAWAY
+ * (TryToInsertStream :425-436) belong to the caller's correlation map, and the host parses the server's frames and mirrors what they
+ * change with b2_h2_conn_peer_update.  On a connection opened with b2_h2_client_conn_reset the device parses them
+ * (b2_h2_client_process_batch) and this call also does what AppendAndDestroySelf does around TryToInsertStream, in its order:
+ *   - pending streams > the peer's max_concurrent_streams -> B2_H2_REQ_ELIMIT, no stream id consumed (:1529-1531);
+ *   - no free stream record in the connection's pool (b2_h2_configure's max_pending) -> B2_H2_REQ_NO_ROOM, no stream id consumed.
+ *     This is a device capacity, not a reference error: the caller may retry after calls complete, or use another connection;
+ *   - after the server's GOAWAY, a stream id above its last_stream_id -> B2_H2_REQ_LOGOFF (brpc ELOGOFF, :1559-1564), after the
+ *     window was charged, as in the reference;
+ *   - otherwise the stream enters the connection's pending map with the peer's stream window minus the body.
+ * Requests of one connection must be adjacent and in write order. */
 #define B2_H2_REQ_GRPC       1u
 #define B2_H2_REQ_GET        2u     /* :method GET instead of POST */
 #define B2_H2_REQ_HTTPS      4u     /* :scheme https */
@@ -616,6 +623,8 @@ int  b2_h2_pack_responses(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const
 #define B2_H2_REQ_OK     0
 #define B2_H2_REQ_ELIMIT 1          /* brpc ELIMIT: remote_window_left is not enough */
 #define B2_H2_REQ_RUNOUT 2          /* brpc EH2RUNOUTSTREAMS */
+#define B2_H2_REQ_LOGOFF 3          /* brpc ELOGOFF: the server sent GOAWAY (device-parsed client connections only) */
+#define B2_H2_REQ_NO_ROOM 4         /* device capacity: the connection's stream pool is full (device-parsed client connections only) */
 typedef struct b2_h2_request {
     uint32_t conn, flags;
     uint32_t path_off, path_len;                     /* inside bytes: URI::GenerateH2Path's result */
@@ -642,6 +651,63 @@ typedef struct b2_h2_peer_update {
 int  b2_h2_conn_peer_update(b2_ctx* ctx, uint32_t conn, const b2_h2_peer_update* u);
 /* the reference's own unit-test hook (:348-352: its tests start 10 000 ids before the end of the id space): the next client stream id */
 int  b2_h2_conn_set_next_stream_id(b2_ctx* ctx, uint32_t conn, uint32_t next_id);
+
+/* ---- the receiving half of an h2 / gRPC client connection, on the device --------------------------------------------------------
+ * b2_h2_client_conn_reset: a new client connection whose server frames the device parses — the H2Context(socket, NULL) constructor and
+ * Init (src/brpc/policy/http2_rpc_protocol.cpp:324-371): client _unack_local_settings (the flags of the preface SETTINGS that
+ * b2_h2_pack_requests writes first), _local_settings until the server's ACK (equal to them at brpc's default flags), _goaway_stream_id
+ * -1, fresh encoder and decoder HPACK tables.  Its stream records live in the h2 pool (b2_h2_configure).
+ * b2_h2_client_process_batch: ParseH2Message on a socket created by connect, with the same arguments as b2_h2_process_batch
+ * (runs = the bytes read from each client socket, runs[i].socket_id = connection, one run per connection): H2Context::Consume
+ * (:467-543) looped over the run — client side: no preface is read, HEADERS / CONTINUATION for an unknown stream are still decoded
+ * through the HPACK table and then dropped (:600-606, :659-665), the peer's SETTINGS / WINDOW_UPDATE update the state that
+ * b2_h2_pack_requests reads (nothing to mirror).  rs[i] as there; rs[i].ctrl_off/len hold what the reference WriteAck()s, in order
+ * (SETTINGS ACK, PING ACK, WINDOW_UPDATEs, RST_STREAM, GOAWAY).  A run on a connection not opened by b2_h2_client_conn_reset reads
+ * nothing: B2_PARSE_ERROR_TRY_OTHERS.
+ * Every stream that leaves the connection becomes one b2_h2_call, in parse order: END_STREAM (OnEndStream :825-846), the server's
+ * RST_STREAM (OnResetStream :781-823, status H2ErrorToStatusCode, http2.cpp:88), a stream error of our own that sent RST_STREAM
+ * (:508-528, the same status), or the server's GOAWAY (OnGoAway :959-1006 + RemoveGoAwayStreams :388-414: every pending stream above
+ * last_stream_id, status 503, in ascending stream id order here — brpc's map has no order).  A GOAWAY also makes later
+ * b2_h2_pack_requests on the connection refuse new streams (B2_H2_REQ_LOGOFF).
+ * Each call carries what ProcessHttpResponse (policy/http_rpc_protocol.cpp:349-564) decides before it parses the response body, for
+ * a call with a protobuf response type: gRPC content-type -> RemoveGrpcPrefix (ERESPONSE "Invalid gRPC response"), then a non-zero
+ * grpc-status -> GrpcStatusToErrorCode (grpc.cpp:83) with the percent-decoded grpc-message or GrpcStatusToString; then :status outside
+ * [200, 300) -> EHTTP "HTTP/2.0 <code> <reason>[: <first 2048 bytes of the body>]"; last, a compressed gRPC message without
+ * grpc-encoding -> ERESPONSE.  error_code is the brpc errno (0: none), the text SetFailed receives is in out.  A compressed gRPC
+ * message (B2_H2_FLAG_GRPC_COMPRESSED) is handed over as it is: inflating it is the caller's (the gzip path), not done here.
+ * Header records: {u16 name_len, u16 value_len, name, value} as in b2_h2_msg, merged the way HttpHeader is filled (ConsumeHeaders
+ * :1233-1288, HttpHeader::AppendHeader http_header.cpp:100-117): trailers included, pseudo-headers left out (":status" is status_code),
+ * a name seen again (case-insensitive) joins the first record with "," ("; " for cookie) unless that value is empty, "content-type"
+ * keeps its last value, every "set-cookie" is a record of its own; records in the order names first appear.
+ * Device capacities as for the server side (b2_h2_configure), and B2_PARSE_ERROR_NO_RESOURCE ends a run whose calls or bytes do not
+ * fit msg_cap / out_cap (the connection must then be closed).
+ * b2_h2_client_abandon_streams: AddAbandonedStream (:1140-1143) for calls the caller gave up on (timeouts): the streams are dropped
+ * where ParseH2Message runs ClearAbandonedStreams (:1103-1157) — after each frame of the next b2_h2_client_process_batch on the connection
+ * that completes a call, and at the end of that run — in ascending id order here (brpc pops the most recently added first, which only
+ * changes how their deferred WINDOW_UPDATE bytes are split).  So an abandoned call is still reported only if it is the first call to
+ * complete in that run.  Without it their pool records stay taken. */
+#define B2_H2_CALL_ENDED         0u   /* END_STREAM */
+#define B2_H2_CALL_RESET_BY_PEER 1u   /* the server's RST_STREAM */
+#define B2_H2_CALL_RESET_BY_US   2u   /* a stream error of ours: we sent RST_STREAM */
+#define B2_H2_CALL_GOAWAY        3u   /* removed by the server's GOAWAY */
+#define B2_H2_CALL_HAS_GRPC_STATUS 32u  /* flag: a grpc-status header was present */
+typedef struct b2_h2_call {
+    uint32_t run_idx, stream_id;
+    uint32_t how;                                /* B2_H2_CALL_* */
+    int32_t  status_code;                        /* :status, H2ErrorToStatusCode of a reset, 503 for GOAWAY; 200 without :status */
+    int32_t  error_code;                         /* brpc errno ProcessHttpResponse sets, 0 = none */
+    int32_t  grpc_status;                        /* strtol of grpc-status, -1 when absent */
+    uint32_t headers_off, headers_len, n_headers;/* merged header records inside out */
+    uint32_t body_off, body_len;                 /* inside out, or inside the input with B2_H2_FLAG_BODY_IN_INPUT */
+    uint32_t msg_off, msg_len;                   /* gRPC message without its 5-byte prefix (B2_H2_FLAG_GRPC_PREFIX_OK), same buffer as body */
+    uint32_t error_off, error_len;               /* the error text inside out */
+    uint32_t flags;                              /* B2_H2_FLAG_GRPC / GRPC_PREFIX_OK / GRPC_COMPRESSED / BODY_IN_INPUT, B2_H2_CALL_HAS_GRPC_STATUS */
+} b2_h2_call;                                    /* 64 bytes */
+int  b2_h2_client_conn_reset(b2_ctx* ctx, uint32_t conn);
+int  b2_h2_client_process_batch(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
+                                b2_h2_run_status* rs, b2_h2_call* calls, uint32_t call_cap, uint32_t* n_calls,
+                                void* out, uint32_t out_cap);
+int  b2_h2_client_abandon_streams(b2_ctx* ctx, uint32_t conn, const uint32_t* stream_ids, uint32_t n);
 
 /* ---- counters (bvar::Adder-like, SURVEY §8e): per-GPU totals accumulated by
  * the kernels: [0] in_bytes [1] in_msgs [2] out_bytes [3] out_msgs [4] errors
