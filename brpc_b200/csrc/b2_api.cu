@@ -43,6 +43,7 @@ struct b2_ctx {
     uint32_t* d_frame_off = nullptr; uint32_t* d_frame_run = nullptr; b2_msg_desc* d_msgs = nullptr; MsgAux* d_aux = nullptr; PackJob* d_jobs = nullptr; uint32_t* d_slow_idx = nullptr; uint8_t* d_heads = nullptr;
     uint32_t* d_slot = nullptr; uint32_t* d_scan_tmp = nullptr; uint8_t* d_resp = nullptr; uint8_t* d_unz = nullptr; uint16_t* d_snappy_tab = nullptr; HpackState* d_hpack = nullptr; H2Conn* d_h2 = nullptr; H2Stream* d_h2_streams = nullptr; uint8_t* d_h2_slots = nullptr; uint32_t h2_max_conns = B2_H2_MAX_CONNS, h2_pending = B2_H2_MAX_PENDING, h2_stream_bytes = B2_H2_STREAM_BYTES; uint64_t h2_last_in = 0, h2_last_out = 0;   // sizes of the last h2 batch still on the device
     uint32_t* d_frame_row = nullptr; uint4* d_rows = nullptr;
+    std::vector<uint8_t> h2_gunzip; uint8_t* d_h2_gz_merge = nullptr;     // host mirror of the kH2Gunzip bits; merge scratch, B2_H2_HEADER_BYTES per run
     // persistent latency kernel (b2_ring_*): pinned + mapped submit ring, its own stream
     uint8_t* ring_slots = nullptr; volatile uint32_t* ring_ctl = nullptr; uint32_t* d_ring_ticket = nullptr; cudaStream_t ring_stream = nullptr;
     uint32_t ring_next = 1, ring_stride = 0, ring_off_runs = 0, ring_off_in = 0, ring_off_out = 0; bool ring_collected[8] = { true, true, true, true, true, true, true, true };
@@ -144,7 +145,7 @@ extern "C" void b2_ctx_destroy(b2_ctx* c) {
     cudaFree(c->d_ring_ticket);
     cudaFree(c->d_bytes); cudaFree(c->d_runs); cudaFree(c->d_run_tile_base); cudaFree(c->d_tiles); cudaFree(c->d_tile_base); cudaFree(c->d_tile_scratch); cudaFree(c->d_tile_spec);
     cudaFree(c->d_run_status); cudaFree(c->d_frame_off); cudaFree(c->d_frame_run); cudaFree(c->d_msgs); cudaFree(c->d_aux); cudaFree(c->d_jobs); cudaFree(c->d_slow_idx); cudaFree(c->d_heads); cudaFree(c->d_slot);
-    cudaFree(c->d_scan_tmp); cudaFree(c->d_resp); cudaFree(c->d_unz); cudaFree(c->d_snappy_tab); cudaFree(c->d_refs); cudaFree(c->d_iov); cudaFreeHost(c->h_iov); cudaFree(c->d_frame_row); cudaFree(c->d_rows); cudaFreeHost(c->h_refs); cudaFree(c->d_hpack); cudaFree(c->d_h2); cudaFree(c->d_h2_streams); cudaFree(c->d_h2_slots); cudaFree(c->d_counters); cudaFree(c->d_totals); cudaFree(c->d_methods); cudaFree(c->d_crc_adv); cudaFree(c->d_meta); cudaFree(c->d_small); cudaFreeHost(c->h_meta); cudaFreeHost(c->h_small);
+    cudaFree(c->d_scan_tmp); cudaFree(c->d_resp); cudaFree(c->d_unz); cudaFree(c->d_snappy_tab); cudaFree(c->d_refs); cudaFree(c->d_iov); cudaFreeHost(c->h_iov); cudaFree(c->d_frame_row); cudaFree(c->d_rows); cudaFreeHost(c->h_refs); cudaFree(c->d_hpack); cudaFree(c->d_h2); cudaFree(c->d_h2_streams); cudaFree(c->d_h2_slots); cudaFree(c->d_h2_gz_merge); cudaFree(c->d_counters); cudaFree(c->d_totals); cudaFree(c->d_methods); cudaFree(c->d_crc_adv); cudaFree(c->d_meta); cudaFree(c->d_small); cudaFreeHost(c->h_meta); cudaFreeHost(c->h_small);
     cudaFreeHost(c->h_run_status); cudaFreeHost(c->h_msgs); cudaFreeHost(c->h_resp); cudaFreeHost(c->h_totals);
     cudaFreeHost(c->h_run_tile_base);
     for (int i = 0; i <= kMaxStages; i++) if (c->ev[i]) cudaEventDestroy(c->ev[i]);
@@ -1140,7 +1141,37 @@ extern "C" int b2_h2_conn_reset(b2_ctx* c, uint32_t conn) {
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     k_h2_conn_reset<<<1, 1, 0, c->stream>>>(c->d_h2, c->d_hpack, conn, h2_pool(c));
     CU(cudaStreamSynchronize(c->stream));
+    if (conn < c->h2_gunzip.size()) c->h2_gunzip[conn] = 0;        // (the kernel cleared the device bit with the rest of H2Conn)
     return B2_OK;
+}
+extern "C" int b2_h2_conn_set_gunzip(b2_ctx* c, uint32_t conn, int enable) {
+    if (!c || conn >= c->h2_max_conns) { set_err("bad connection index"); return B2_E_INVAL; }
+    int rc = h2_ensure(c); if (rc != B2_OK) return rc;
+    CU(cudaSetDevice(c->opt.device));
+    if (enable && !c->d_h2_gz_merge) {                            // once per context: the merge scratch of the select pass
+        if (cudaMalloc(&c->d_h2_gz_merge, (size_t)c->opt.max_runs * B2_H2_HEADER_BYTES) != cudaSuccess) { c->d_h2_gz_merge = nullptr; set_err("cudaMalloc gunzip scratch failed"); return B2_E_NOMEM; }
+    }
+    if (c->h2_gunzip.size() < c->h2_max_conns) c->h2_gunzip.resize(c->h2_max_conns, 0);
+    k_h2_set_gunzip<<<1, 1, 0, c->stream>>>(c->d_h2, conn, enable ? 1 : 0);
+    CU(cudaStreamSynchronize(c->stream));
+    c->h2_gunzip[conn] = enable ? 1 : 0;
+    return B2_OK;
+}
+// the gunzip passes over a parsed batch (b2_h2_conn_set_gunzip), enqueued after the consume kernel and before the run statuses are fetched;
+// nothing is launched unless a run is on an opted-in connection
+static bool h2_gz_wanted(const b2_ctx* c, const b2_run* runs, uint32_t n_runs) {
+    if (c->h2_gunzip.empty()) return false;
+    for (uint32_t r = 0; r < n_runs; r++) if (c->h2_gunzip[runs[r].socket_id]) return true;
+    return false;
+}
+template <class M>
+static void h2_gz_launch(b2_ctx* c, uint32_t n_runs, b2_h2_run_status* d_rs, M* d_msgs, uint32_t per_run, uint32_t region) {
+    uint32_t* d_gz = c->d_frame_off;                              // one word per descriptor slot (n_runs * per_run <= max_msgs)
+    const uint32_t n_slots = n_runs * per_run;
+    k_h2_gz_select<M><<<(n_runs + 31) / 32, 32, 0, c->stream>>>(c->d_bytes, (const b2_run*)c->d_meta, n_runs, c->d_h2, d_rs, d_msgs, per_run, c->d_unz, c->d_h2_gz_merge, d_gz);
+    k_h2_gz_size<M><<<(n_slots + 63) / 64, 64, 0, c->stream>>>(c->d_bytes, n_runs, d_rs, d_msgs, per_run, c->d_unz, d_gz);
+    k_h2_gz_place<M><<<(n_runs + 31) / 32, 32, 0, c->stream>>>(n_runs, d_rs, d_msgs, per_run, region, d_gz);
+    k_h2_gz_inflate<M><<<(n_slots + 63) / 64, 64, 0, c->stream>>>(c->d_bytes, n_runs, d_rs, d_msgs, per_run, c->d_unz, d_gz);
 }
 extern "C" int b2_h2_process_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
                                    b2_h2_run_status* rs, b2_h2_msg* msgs, uint32_t msg_cap, uint32_t* n_msgs,
@@ -1166,6 +1197,7 @@ extern "C" int b2_h2_process_batch(b2_ctx* c, const void* bytes, uint32_t nbytes
     CU(cudaMemcpyAsync(c->d_meta, runs, sizeof(b2_run) * (size_t)n_runs, cudaMemcpyHostToDevice, c->stream));
     k_h2_consume<<<(n_runs + 31) / 32, 32, 0, c->stream>>>(c->d_bytes, (const b2_run*)c->d_meta, n_runs, c->d_h2, c->d_hpack, c->d_methods, c->cfg.n_methods,
                                                             d_rs, d_msgs, per_run_msgs, c->d_unz, region, h2_pool(c));
+    if (h2_gz_wanted(c, runs, n_runs)) h2_gz_launch(c, n_runs, d_rs, d_msgs, per_run_msgs, region);
     CU(cudaMemcpyAsync(rs, d_rs, sizeof(b2_h2_run_status) * (size_t)n_runs, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     // fetch only what was produced: every run owns `region` bytes (acks from its start, records/bodies from region/4) and
@@ -1322,6 +1354,7 @@ extern "C" int b2_h2_client_conn_reset(b2_ctx* c, uint32_t conn) {
     CU(cudaSetDevice(c->opt.device));
     k_h2_client_conn_reset<<<1, 1, 0, c->stream>>>(c->d_h2, c->d_hpack, conn, h2_pool(c));
     CU(cudaStreamSynchronize(c->stream));
+    if (conn < c->h2_gunzip.size()) c->h2_gunzip[conn] = 0;
     return B2_OK;
 }
 extern "C" int b2_h2_client_abandon_streams(b2_ctx* c, uint32_t conn, const uint32_t* stream_ids, uint32_t n) {
@@ -1361,6 +1394,7 @@ extern "C" int b2_h2_client_process_batch(b2_ctx* c, const void* bytes, uint32_t
     CU(cudaMemcpyAsync(c->d_meta, runs, sizeof(b2_run) * (size_t)n_runs, cudaMemcpyHostToDevice, c->stream));
     k_h2_client_consume<<<(n_runs + 31) / 32, 32, 0, c->stream>>>(c->d_bytes, (const b2_run*)c->d_meta, n_runs, c->d_h2, c->d_hpack,
                                                                    d_rs, d_calls, per_run_calls, c->d_unz, region, h2_pool(c));
+    if (h2_gz_wanted(c, runs, n_runs)) h2_gz_launch(c, n_runs, d_rs, d_calls, per_run_calls, region);
     CU(cudaMemcpyAsync(rs, d_rs, sizeof(b2_h2_run_status) * (size_t)n_runs, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     // as b2_h2_process_batch: three strided copies of what was produced, then the calls are compacted into one list (run order)

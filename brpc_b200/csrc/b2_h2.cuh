@@ -9,6 +9,7 @@
 #include <cuda_runtime.h>
 #include "b2_core.cuh"
 #include "b2_hpack_tables.cuh"
+#include "b2_inflate.cuh"
 
 namespace b2 {
 
@@ -1503,6 +1504,104 @@ __global__ void k_h2_client_consume(const uint8_t* bytes, const b2_run* runs, ui
     b2_h2_run_status st; st.consumed = last_ok; st.parse_error = perr; st.n_msgs = n_calls; st.first_msg = o.blob_off - region / 4;
     st.ctrl_off = r * region; st.ctrl_len = o.ctrl_len; st.remote_max_frame_size = c.r_max_frame_size; st.remote_stream_window_size = c.r_stream_window_size;
     rs[r] = st;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// gzip-compressed messages on connections opted in with b2_h2_conn_set_gunzip: the step of ProcessHttpRequest (policy/http_rpc_protocol.cpp
+// :1645-1683) / ProcessHttpResponse (:507-529) between RemoveGrpcPrefix and the protobuf parse, over what k_h2_consume / k_h2_client_consume
+// left on the device.  Four passes, launched only when a run of the batch is on such a connection:
+//   select (one thread per run: the server's raw records are merged like the client's) -> size (one thread per candidate,
+//   gz_input_stream<false>) -> place (one thread per run, message order, 16-byte aligned after the parse's own bytes in the run's region)
+//   -> inflate (one thread per placed candidate, gz_input_stream<true>).  gz[slot] carries a candidate from one pass to the next.
+constexpr uint32_t kH2Gunzip = 2u;                                // H2Conn::pad0 bit: b2_h2_conn_set_gunzip
+constexpr uint32_t kGzSkip = 0xffffffffu, kGzToHost = 0xfffffffeu, kGzToSize = 0xfffffffdu;
+__global__ void k_h2_set_gunzip(H2Conn* conns, uint32_t conn, int enable) {
+    if (enable) conns[conn].pad0 |= kH2Gunzip; else conns[conn].pad0 &= ~kH2Gunzip;
+}
+__device__ __forceinline__ bool h2gz_failed(const b2_h2_msg&) { return false; }
+__device__ __forceinline__ bool h2gz_failed(const b2_h2_call& m) { return m.error_code != 0; }   // ProcessHttpResponse stopped before
+// ... before its grpc-encoding check: with a valid prefix, ERESPONSE (2002) comes from that check itself
+__device__ __forceinline__ bool h2gz_stopped_earlier(const b2_h2_msg&) { return false; }
+__device__ __forceinline__ bool h2gz_stopped_earlier(const b2_h2_call& m) { return m.error_code != 0 && m.error_code != 2002; }
+__device__ __forceinline__ bool h2gz_client(const b2_h2_msg&) { return false; }
+__device__ __forceinline__ bool h2gz_client(const b2_h2_call&) { return true; }
+// the compressed bytes: the gRPC message after its prefix, or the whole body
+template <class M>
+__device__ __forceinline__ const uint8_t* h2gz_src(const M& m, const uint8_t* bytes, const uint8_t* out, uint32_t& n) {
+    const bool grpc = m.flags & B2_H2_FLAG_GRPC;
+    n = grpc ? m.body_len - 5 : m.body_len;
+    return ((m.flags & B2_H2_FLAG_BODY_IN_INPUT) ? bytes : out) + m.body_off + (grpc ? 5 : 0);
+}
+template <class M>
+__global__ void k_h2_gz_select(const uint8_t* bytes, const b2_run* runs, uint32_t n_runs, const H2Conn* conns, const b2_h2_run_status* rs,
+                               M* msgs, uint32_t per_run, const uint8_t* out, uint8_t* merge_scratch, uint32_t* gz) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_runs) return;
+    const bool on = conns[(uint32_t)runs[r].socket_id].pad0 & kH2Gunzip;
+    uint8_t* const scratch = merge_scratch + (size_t)r * kH2HdrBytes;
+    for (uint32_t i = 0; i < rs[r].n_msgs; i++) {
+        const uint32_t slot = r * per_run + i;
+        gz[slot] = kGzSkip;
+        if (!on) continue;
+        M& m = msgs[slot];
+        const uint8_t* recs = out + m.headers_off; uint32_t rl = m.headers_len;
+        if (!h2gz_client(m)) {                                      // server records are raw: merge them as HttpHeader holds them
+            uint32_t nh; int32_t sc = 200;
+            rl = h2c_merge(recs, rl, scratch, nh, sc); recs = scratch;
+        }
+        const bool grpc = m.flags & B2_H2_FLAG_GRPC;
+        const uint8_t* e; uint32_t el;
+        bool has;
+        if (grpc) {
+            if (!(m.flags & B2_H2_FLAG_GRPC_PREFIX_OK) || !(m.flags & B2_H2_FLAG_GRPC_COMPRESSED)) continue;   // encoding stays NULL
+            has = h2c_get(recs, rl, "grpc-encoding", e, el);
+            if (!has) { if (!h2gz_stopped_earlier(m)) m.flags |= B2_H2_FLAG_NO_GRPC_ENCODING; continue; }
+        } else {
+            if (!h2gz_client(m) && m.body_len == 0) continue;      // ProcessHttpRequest: an empty body is not decoded
+            has = h2c_get(recs, rl, "content-encoding", e, el);
+        }
+        if (!has || h2gz_failed(m) || !lit_eq(e, el, "gzip")) continue;   // *encoding == "gzip": the whole std::string
+        uint32_t n;
+        (void)h2gz_src(m, bytes, out, n);
+        gz[slot] = n > kGzMaxIn ? kGzToHost : kGzToSize;
+    }
+}
+template <class M>
+__global__ void k_h2_gz_size(const uint8_t* bytes, uint32_t n_runs, const b2_h2_run_status* rs, const M* msgs, uint32_t per_run,
+                             const uint8_t* out, uint32_t* gz) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n_runs * per_run || t % per_run >= rs[t / per_run].n_msgs || gz[t] != kGzToSize) return;
+    uint32_t n;
+    const uint8_t* src = h2gz_src(msgs[t], bytes, out, n);
+    bool big = false;
+    const uint32_t bound = gz_input_stream<false>(src, n, B2_COMPRESS_TYPE_GZIP, nullptr, kGzMaxOut, &big);
+    gz[t] = big ? kGzToHost : bound;
+}
+template <class M>
+__global__ void k_h2_gz_place(uint32_t n_runs, b2_h2_run_status* rs, M* msgs, uint32_t per_run, uint32_t region, uint32_t* gz) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_runs) return;
+    uint32_t cur = region / 4 + rs[r].first_msg;                    // (the consume kernel reports its blob bytes there, a multiple of 16)
+    for (uint32_t i = 0; i < rs[r].n_msgs; i++) {
+        const uint32_t slot = r * per_run + i, g = gz[slot];
+        if (g == kGzSkip) continue;
+        if (g == kGzToHost || (unsigned long long)cur + g > region) { msgs[slot].flags |= B2_H2_FLAG_GUNZIP_HOST; gz[slot] = kGzSkip; continue; }
+        msgs[slot].msg_off = r * region + cur;
+        cur += (g + 15u) & ~15u;
+    }
+    rs[r].first_msg = cur - region / 4;                            // the strided copy-back brings the inflated bytes home
+}
+template <class M>
+__global__ void k_h2_gz_inflate(const uint8_t* bytes, uint32_t n_runs, const b2_h2_run_status* rs, M* msgs, uint32_t per_run,
+                                uint8_t* out, const uint32_t* gz) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n_runs * per_run || t % per_run >= rs[t / per_run].n_msgs || gz[t] == kGzSkip) return;
+    M& m = msgs[t];
+    uint32_t n;
+    const uint8_t* src = h2gz_src(m, bytes, out, n);
+    bool big = false;
+    m.msg_len = gz_input_stream<true>(src, n, B2_COMPRESS_TYPE_GZIP, out + m.msg_off, gz[t], &big);   // <= the bound: a failed check hands over less
+    m.flags |= B2_H2_FLAG_GUNZIPPED;
 }
 #endif
 }  // namespace b2

@@ -37,6 +37,9 @@ public:
 
     int AddMethod(const b2_method& m) { const int i = b2_register_method(_ctx, &m); if (i >= 0) { _handlers.resize(i + 1); _handlers[i] = m.handler; } return i; }
     void SetHostProcess(Process p) { _process = p; }
+    // Connections added from now on inflate gzip-compressed requests on the device (b2_h2_conn_set_gunzip): an echo request that arrives
+    // compressed is answered from the inflated bytes, uncompressed (brpc's echo sets no response_compress_type).  Off by default.
+    void SetGunzip(bool on) { _gunzip = on; }
     // a new server-side connection: H2Context is created when the first bytes arrive (:1108-1120)
     // Device connection slots are a free list: RemoveConnection gives the slot back.  nullptr = no slot left (the caller keeps such a
     // connection on the host parser) or the device refused the reset.
@@ -46,6 +49,7 @@ public:
         if (_free_conns.empty()) return nullptr;
         const uint32_t slot = _free_conns.back();
         if (b2_h2_conn_reset(_ctx, slot) != B2_OK) return nullptr;
+        if (_gunzip && b2_h2_conn_set_gunzip(_ctx, slot, 1) != B2_OK) return nullptr;
         _free_conns.pop_back();
         _conn_of[id] = slot;
         return (_sockets[id] = std::unique_ptr<Socket>(new Socket(id))).get();
@@ -83,7 +87,9 @@ public:
             if (st.ctrl_len) { IOBuf ack; ack.append(_out + st.ctrl_off, st.ctrl_len); s->Write(&ack); }      // WriteAck (:144-150)
             for (uint32_t m = st.first_msg; m < st.first_msg + st.n_msgs; m++) {
                 const b2_h2_msg& d = msgs[m];
-                const bool device_echo = (d.flags & B2_H2_FLAG_GRPC) && (d.flags & B2_H2_FLAG_GRPC_PREFIX_OK) && !(d.flags & B2_H2_FLAG_GRPC_COMPRESSED) &&
+                // a compressed request is echoed only once the device inflated it (msg_off/len then index out)
+                const bool gunzipped = d.flags & B2_H2_FLAG_GUNZIPPED;
+                const bool device_echo = (d.flags & B2_H2_FLAG_GRPC) && (d.flags & B2_H2_FLAG_GRPC_PREFIX_OK) && (!(d.flags & B2_H2_FLAG_GRPC_COMPRESSED) || gunzipped) &&
                                          d.method_idx >= 0 && d.method_idx < (int)_handlers.size() && _handlers[d.method_idx] == B2_HANDLER_ECHO;
                 uint32_t ct_off = 0, ct_len = 0;
                 if (device_echo) FindHeader(d, "content-type", &ct_off, &ct_len);
@@ -91,7 +97,7 @@ public:
                     // SendHttpResponse for gRPC: status 200, the request's content-type, the echoed message, grpc-status 0
                     b2_h2_response r; memset(&r, 0, sizeof r);
                     r.conn = (uint32_t)runs[i].socket_id; r.stream_id = d.stream_id; r.status_code = 200;
-                    r.flags = B2_H2_RESP_GRPC | B2_H2_RESP_CT_IN_OUT | ((d.flags & B2_H2_FLAG_BODY_IN_INPUT) ? B2_H2_RESP_BODY_IN_INPUT : B2_H2_RESP_BODY_IN_OUT);
+                    r.flags = B2_H2_RESP_GRPC | B2_H2_RESP_CT_IN_OUT | ((d.flags & B2_H2_FLAG_BODY_IN_INPUT) && !gunzipped ? B2_H2_RESP_BODY_IN_INPUT : B2_H2_RESP_BODY_IN_OUT);
                     r.content_type_off = ct_off; r.content_type_len = ct_len; r.body_off = d.msg_off; r.body_len = d.msg_len;
                     resps.push_back(r); resp_sock.push_back(s);
                 } else if (_process) {
@@ -130,7 +136,7 @@ private:
     }
     b2_ctx* _ctx = nullptr; uint8_t* _batch = nullptr; uint8_t* _out = nullptr; uint8_t* _pack = nullptr; size_t _cap; uint32_t _out_cap, _max_conns; size_t _msg_cap;
     std::vector<uint32_t> _free_conns;
-    Process _process = nullptr; std::vector<int> _handlers;
+    Process _process = nullptr; std::vector<int> _handlers; bool _gunzip = false;
     std::unordered_map<uint64_t, std::unique_ptr<Socket>> _sockets;
     std::unordered_map<uint64_t, uint32_t> _conn_of;
 };

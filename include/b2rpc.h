@@ -674,7 +674,7 @@ int  b2_h2_conn_set_next_stream_id(b2_ctx* ctx, uint32_t conn, uint32_t next_id)
  * grpc-status -> GrpcStatusToErrorCode (grpc.cpp:83) with the percent-decoded grpc-message or GrpcStatusToString; then :status outside
  * [200, 300) -> EHTTP "HTTP/2.0 <code> <reason>[: <first 2048 bytes of the body>]"; last, a compressed gRPC message without
  * grpc-encoding -> ERESPONSE.  error_code is the brpc errno (0: none), the text SetFailed receives is in out.  A compressed gRPC
- * message (B2_H2_FLAG_GRPC_COMPRESSED) is handed over as it is: inflating it is the caller's (the gzip path), not done here.
+ * message (B2_H2_FLAG_GRPC_COMPRESSED) is handed over as it is unless the connection opted in to b2_h2_conn_set_gunzip (below).
  * Header records: {u16 name_len, u16 value_len, name, value} as in b2_h2_msg, merged the way HttpHeader is filled (ConsumeHeaders
  * :1233-1288, HttpHeader::AppendHeader http_header.cpp:100-117): trailers included, pseudo-headers left out (":status" is status_code),
  * a name seen again (case-insensitive) joins the first record with "," ("; " for cookie) unless that value is empty, "content-type"
@@ -708,6 +708,28 @@ int  b2_h2_client_process_batch(b2_ctx* ctx, const void* bytes, uint32_t nbytes,
                                 b2_h2_run_status* rs, b2_h2_call* calls, uint32_t call_cap, uint32_t* n_calls,
                                 void* out, uint32_t out_cap);
 int  b2_h2_client_abandon_streams(b2_ctx* ctx, uint32_t conn, const uint32_t* stream_ids, uint32_t n);
+
+/* ---- gzip-compressed h2 / gRPC messages, inflated on the device (opt-in per connection) ------------------------------------------
+ * b2_h2_conn_set_gunzip: the connection's messages are protobuf-typed, so the next b2_h2_process_batch (server connections) or
+ * b2_h2_client_process_batch (device-parsed client connections) also does what ProcessHttpRequest (policy/http_rpc_protocol.cpp:
+ * 1645-1683) / ProcessHttpResponse (:507-529) do before the protobuf parse:
+ *   - the encoding: gRPC content-type -> the merged "grpc-encoding" value, only when the prefix's compressed flag is set (a message
+ *     sent uncompressed with "grpc-encoding: gzip", as grpc clients and servers send small ones, is left alone); other messages ->
+ *     the merged "content-encoding" value.  It must be exactly "gzip" (case and all; "gzip" sent twice merges into "gzip,gzip");
+ *   - candidates: server messages with a valid gRPC prefix or, not gRPC, a non-empty body; client calls with error_code 0 (so a call
+ *     with an invalid prefix, a non-zero grpc-status or a non-2xx status is never inflated);
+ *   - policy::GzipDecompress: GzipInputStream(GZIP) over the message as ONE block (as the baidu_std gzip bodies), which cannot fail;
+ *     a damaged stream yields what zlib handed over before the error.  brpc reads a body of several IOBuf blocks and can then answer
+ *     "Fail to un-gzip ..." depending on where the blocks end; the device never does.
+ * The inflated bytes land in out, 16-byte aligned after what the parse itself wrote in the run's region, in message order; a
+ * message whose size bound does not fit there is skipped (B2_H2_FLAG_GUNZIP_HOST) and later ones are still tried.  A server message
+ * echoed from there needs no copy: b2_h2_pack_responses with B2_H2_RESP_BODY_IN_OUT.  b2_h2_conn_reset and b2_h2_client_conn_reset
+ * clear the setting; batches without such a connection run exactly as before. */
+#define B2_H2_FLAG_GUNZIPPED        64u   /* inflated: msg_off/msg_len index the inflated bytes in out (body_* still the received body) */
+#define B2_H2_FLAG_GUNZIP_HOST     128u   /* would be inflated, left as received: > 1 MiB compressed or inflated, or no room in out */
+#define B2_H2_FLAG_NO_GRPC_ENCODING 256u  /* compressed gRPC message without grpc-encoding (brpc: EREQUEST / ERESPONSE "Fail to find header");
+                                             not set on a client call an earlier verdict already failed */
+int  b2_h2_conn_set_gunzip(b2_ctx* ctx, uint32_t conn, int enable);
 
 /* ---- counters (bvar::Adder-like, SURVEY §8e): per-GPU totals accumulated by
  * the kernels: [0] in_bytes [1] in_msgs [2] out_bytes [3] out_msgs [4] errors
