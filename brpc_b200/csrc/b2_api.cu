@@ -1173,57 +1173,67 @@ static void h2_gz_launch(b2_ctx* c, uint32_t n_runs, b2_h2_run_status* d_rs, M* 
     k_h2_gz_place<M><<<(n_runs + 31) / 32, 32, 0, c->stream>>>(n_runs, d_rs, d_msgs, per_run, region, d_gz);
     k_h2_gz_inflate<M><<<(n_slots + 63) / 64, 64, 0, c->stream>>>(c->d_bytes, n_runs, d_rs, d_msgs, per_run, c->d_unz, d_gz);
 }
-extern "C" int b2_h2_process_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
-                                   b2_h2_run_status* rs, b2_h2_msg* msgs, uint32_t msg_cap, uint32_t* n_msgs,
-                                   void* out, uint32_t out_cap) {
-    if (!c || !bytes || !runs || !rs || !msgs || !n_msgs || !out) { set_err("null argument"); return B2_E_INVAL; }
-    static_assert(sizeof(b2_h2_msg) == 64 && sizeof(b2_h2_run_status) == 32, "h2 ABI layout");
-    if (nbytes > c->opt.max_batch_bytes || n_runs > c->opt.max_runs || out_cap > 2ull * c->opt.max_resp_bytes || msg_cap > c->opt.max_msgs) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
-    *n_msgs = 0;
+// ParseH2Message over a batch, server (b2_h2_msg) or client (b2_h2_call) connections: upload, the side's consume kernel (then the
+// gunzip passes), and a fetch of only what was produced.  Every run owns `region` bytes (acks from its start, records/bodies from
+// region/4) and per_run descriptors: three strided copies, then the descriptors are compacted into one list (run order).
+template <class M>
+static int h2_parse_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
+                          b2_h2_run_status* rs, M* descs, uint32_t cap, uint32_t* n_descs, void* out, uint32_t out_cap) {
+    constexpr bool kClient = std::is_same<M, b2_h2_call>::value;
+    if (!c || !bytes || !runs || !rs || !descs || !n_descs || !out) { set_err("null argument"); return B2_E_INVAL; }
+    static_assert(sizeof(M) == 64 && sizeof(b2_h2_run_status) == 32, "h2 ABI layout");
+    if (nbytes > c->opt.max_batch_bytes || n_runs > c->opt.max_runs || out_cap > 2ull * c->opt.max_resp_bytes || cap > c->opt.max_msgs) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    *n_descs = 0;
     if (n_runs == 0) return B2_OK;
     for (uint32_t r = 0; r < n_runs; r++) {
         if ((uint64_t)runs[r].offset + runs[r].length > nbytes) { set_err("run outside buffer"); return B2_E_INVAL; }
         if (runs[r].socket_id >= c->h2_max_conns) { set_err("connection index out of range"); return B2_E_INVAL; }
         for (uint32_t q = 0; q < r; q++) if (runs[q].socket_id == runs[r].socket_id) { set_err("one run per connection and batch"); return B2_E_INVAL; }
     }
-    const uint32_t region = (out_cap / n_runs) & ~63u, per_run_msgs = msg_cap / n_runs;
-    if (region < 256 || per_run_msgs == 0) { set_err("out_cap / msg_cap too small for the number of runs"); return B2_E_CAPACITY; }
+    const uint32_t region = (out_cap / n_runs) & ~63u, per_run = cap / n_runs;
+    if (region < 256 || per_run == 0) { set_err(kClient ? "out_cap / call_cap too small for the number of runs" : "out_cap / msg_cap too small for the number of runs"); return B2_E_CAPACITY; }
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     CU(cudaSetDevice(c->opt.device));
     b2_h2_run_status* d_rs = reinterpret_cast<b2_h2_run_status*>(c->d_run_status);      // 32 B each, like b2_run_status
-    b2_h2_msg* d_msgs = reinterpret_cast<b2_h2_msg*>(c->d_msgs);                         // 64 B each, like b2_msg_desc
+    M* d_descs = reinterpret_cast<M*>(c->d_msgs);                                        // 64 B each, like b2_msg_desc
     c->h2_last_in = 0; c->h2_last_out = 0;       // the device copies of the last h2 batch are about to be overwritten
     CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(c->d_meta, runs, sizeof(b2_run) * (size_t)n_runs, cudaMemcpyHostToDevice, c->stream));
-    k_h2_consume<<<(n_runs + 31) / 32, 32, 0, c->stream>>>(c->d_bytes, (const b2_run*)c->d_meta, n_runs, c->d_h2, c->d_hpack, c->d_methods, c->cfg.n_methods,
-                                                            d_rs, d_msgs, per_run_msgs, c->d_unz, region, h2_pool(c));
-    if (h2_gz_wanted(c, runs, n_runs)) h2_gz_launch(c, n_runs, d_rs, d_msgs, per_run_msgs, region);
+    if constexpr (kClient) k_h2_client_consume<<<(n_runs + 31) / 32, 32, 0, c->stream>>>(c->d_bytes, (const b2_run*)c->d_meta, n_runs, c->d_h2, c->d_hpack,
+                                                                                          d_rs, d_descs, per_run, c->d_unz, region, h2_pool(c));
+    else k_h2_consume<<<(n_runs + 31) / 32, 32, 0, c->stream>>>(c->d_bytes, (const b2_run*)c->d_meta, n_runs, c->d_h2, c->d_hpack, c->d_methods, c->cfg.n_methods,
+                                                                 d_rs, d_descs, per_run, c->d_unz, region, h2_pool(c));
+    if (h2_gz_wanted(c, runs, n_runs)) h2_gz_launch(c, n_runs, d_rs, d_descs, per_run, region);
     CU(cudaMemcpyAsync(rs, d_rs, sizeof(b2_h2_run_status) * (size_t)n_runs, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
-    // fetch only what was produced: every run owns `region` bytes (acks from its start, records/bodies from region/4) and
-    // per_run_msgs descriptors — three strided copies, then the descriptors are compacted into one list (run order)
-    uint32_t total = 0, max_msgs = 0, max_ctrl = 0, max_blob = 0;
+    uint32_t total = 0, max_descs = 0, max_ctrl = 0, max_blob = 0;
     for (uint32_t r = 0; r < n_runs; r++) {
-        total += rs[r].n_msgs; if (rs[r].n_msgs > max_msgs) max_msgs = rs[r].n_msgs;
+        total += rs[r].n_msgs; if (rs[r].n_msgs > max_descs) max_descs = rs[r].n_msgs;
         if (rs[r].ctrl_len > max_ctrl) max_ctrl = rs[r].ctrl_len;
         if (rs[r].first_msg > max_blob) max_blob = rs[r].first_msg;             // (the kernel reports the blob bytes it used here)
     }
-    if (total > msg_cap) { set_err("msg_cap too small"); return B2_E_CAPACITY; }
-    std::vector<b2_h2_msg> tmp((size_t)n_runs * (max_msgs ? max_msgs : 1));
-    if (max_msgs) CU(cudaMemcpy2DAsync(tmp.data(), sizeof(b2_h2_msg) * (size_t)max_msgs, d_msgs, sizeof(b2_h2_msg) * (size_t)per_run_msgs,
-                                       sizeof(b2_h2_msg) * (size_t)max_msgs, n_runs, cudaMemcpyDeviceToHost, c->stream));
+    if constexpr (!kClient) { if (total > cap) { set_err("msg_cap too small"); return B2_E_CAPACITY; } }
+    std::vector<M> tmp((size_t)n_runs * (max_descs ? max_descs : 1));
+    if (max_descs) CU(cudaMemcpy2DAsync(tmp.data(), sizeof(M) * (size_t)max_descs, d_descs, sizeof(M) * (size_t)per_run,
+                                        sizeof(M) * (size_t)max_descs, n_runs, cudaMemcpyDeviceToHost, c->stream));
     if (max_ctrl) CU(cudaMemcpy2DAsync(out, region, c->d_unz, region, max_ctrl, n_runs, cudaMemcpyDeviceToHost, c->stream));
     if (max_blob) CU(cudaMemcpy2DAsync((uint8_t*)out + region / 4, region, c->d_unz + region / 4, region, max_blob, n_runs, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     total = 0;
     for (uint32_t r = 0; r < n_runs; r++) {
-        if (rs[r].n_msgs) memcpy(msgs + total, tmp.data() + (size_t)r * max_msgs, sizeof(b2_h2_msg) * (size_t)rs[r].n_msgs);
+        if (rs[r].n_msgs) memcpy(descs + total, tmp.data() + (size_t)r * max_descs, sizeof(M) * (size_t)rs[r].n_msgs);
         rs[r].first_msg = total; total += rs[r].n_msgs;
     }
-    c->h2_last_in = nbytes; c->h2_last_out = (uint64_t)region * n_runs;
-    *n_msgs = total;
+    // a server batch stays readable by b2_h2_pack_responses; a client batch leaves h2_last_in / h2_last_out at 0, so that it may not
+    if constexpr (!kClient) { c->h2_last_in = nbytes; c->h2_last_out = (uint64_t)region * n_runs; }
+    *n_descs = total;
     c->uploaded = false; c->executed = false;
     return B2_OK;
+}
+extern "C" int b2_h2_process_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
+                                   b2_h2_run_status* rs, b2_h2_msg* msgs, uint32_t msg_cap, uint32_t* n_msgs,
+                                   void* out, uint32_t out_cap) {
+    return h2_parse_batch(c, bytes, nbytes, runs, n_runs, rs, msgs, msg_cap, n_msgs, out, out_cap);
 }
 
 extern "C" int b2_h2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_h2_response* resps, uint32_t n,
@@ -1373,51 +1383,7 @@ extern "C" int b2_h2_client_abandon_streams(b2_ctx* c, uint32_t conn, const uint
 extern "C" int b2_h2_client_process_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
                                           b2_h2_run_status* rs, b2_h2_call* calls, uint32_t call_cap, uint32_t* n_calls,
                                           void* out, uint32_t out_cap) {
-    if (!c || !bytes || !runs || !rs || !calls || !n_calls || !out) { set_err("null argument"); return B2_E_INVAL; }
-    static_assert(sizeof(b2_h2_call) == 64, "h2 call ABI layout");
-    if (nbytes > c->opt.max_batch_bytes || n_runs > c->opt.max_runs || out_cap > 2ull * c->opt.max_resp_bytes || call_cap > c->opt.max_msgs) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
-    *n_calls = 0;
-    if (n_runs == 0) return B2_OK;
-    for (uint32_t r = 0; r < n_runs; r++) {
-        if ((uint64_t)runs[r].offset + runs[r].length > nbytes) { set_err("run outside buffer"); return B2_E_INVAL; }
-        if (runs[r].socket_id >= c->h2_max_conns) { set_err("connection index out of range"); return B2_E_INVAL; }
-        for (uint32_t q = 0; q < r; q++) if (runs[q].socket_id == runs[r].socket_id) { set_err("one run per connection and batch"); return B2_E_INVAL; }
-    }
-    const uint32_t region = (out_cap / n_runs) & ~63u, per_run_calls = call_cap / n_runs;
-    if (region < 256 || per_run_calls == 0) { set_err("out_cap / call_cap too small for the number of runs"); return B2_E_CAPACITY; }
-    int rc = h2_ensure(c); if (rc != B2_OK) return rc;
-    CU(cudaSetDevice(c->opt.device));
-    b2_h2_run_status* d_rs = reinterpret_cast<b2_h2_run_status*>(c->d_run_status);
-    b2_h2_call* d_calls = reinterpret_cast<b2_h2_call*>(c->d_msgs);                    // 64 B each, like b2_msg_desc
-    c->h2_last_in = 0; c->h2_last_out = 0;       // the device copies of the last h2 batch are about to be overwritten
-    CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
-    CU(cudaMemcpyAsync(c->d_meta, runs, sizeof(b2_run) * (size_t)n_runs, cudaMemcpyHostToDevice, c->stream));
-    k_h2_client_consume<<<(n_runs + 31) / 32, 32, 0, c->stream>>>(c->d_bytes, (const b2_run*)c->d_meta, n_runs, c->d_h2, c->d_hpack,
-                                                                   d_rs, d_calls, per_run_calls, c->d_unz, region, h2_pool(c));
-    if (h2_gz_wanted(c, runs, n_runs)) h2_gz_launch(c, n_runs, d_rs, d_calls, per_run_calls, region);
-    CU(cudaMemcpyAsync(rs, d_rs, sizeof(b2_h2_run_status) * (size_t)n_runs, cudaMemcpyDeviceToHost, c->stream));
-    CU(cudaStreamSynchronize(c->stream));
-    // as b2_h2_process_batch: three strided copies of what was produced, then the calls are compacted into one list (run order)
-    uint32_t total = 0, max_calls = 0, max_ctrl = 0, max_blob = 0;
-    for (uint32_t r = 0; r < n_runs; r++) {
-        total += rs[r].n_msgs; if (rs[r].n_msgs > max_calls) max_calls = rs[r].n_msgs;
-        if (rs[r].ctrl_len > max_ctrl) max_ctrl = rs[r].ctrl_len;
-        if (rs[r].first_msg > max_blob) max_blob = rs[r].first_msg;             // (the kernel reports the blob bytes it used here)
-    }
-    std::vector<b2_h2_call> tmp((size_t)n_runs * (max_calls ? max_calls : 1));
-    if (max_calls) CU(cudaMemcpy2DAsync(tmp.data(), sizeof(b2_h2_call) * (size_t)max_calls, d_calls, sizeof(b2_h2_call) * (size_t)per_run_calls,
-                                        sizeof(b2_h2_call) * (size_t)max_calls, n_runs, cudaMemcpyDeviceToHost, c->stream));
-    if (max_ctrl) CU(cudaMemcpy2DAsync(out, region, c->d_unz, region, max_ctrl, n_runs, cudaMemcpyDeviceToHost, c->stream));
-    if (max_blob) CU(cudaMemcpy2DAsync((uint8_t*)out + region / 4, region, c->d_unz + region / 4, region, max_blob, n_runs, cudaMemcpyDeviceToHost, c->stream));
-    CU(cudaStreamSynchronize(c->stream));
-    total = 0;
-    for (uint32_t r = 0; r < n_runs; r++) {
-        if (rs[r].n_msgs) memcpy(calls + total, tmp.data() + (size_t)r * max_calls, sizeof(b2_h2_call) * (size_t)rs[r].n_msgs);
-        rs[r].first_msg = total; total += rs[r].n_msgs;
-    }
-    *n_calls = total;                            // (h2_last_in / h2_last_out stay 0: b2_h2_pack_responses may not read a client batch)
-    c->uploaded = false; c->executed = false;
-    return B2_OK;
+    return h2_parse_batch(c, bytes, nbytes, runs, n_runs, rs, calls, call_cap, n_calls, out, out_cap);
 }
 
 extern "C" int b2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_request* reqs, uint32_t n,
