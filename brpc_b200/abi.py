@@ -41,6 +41,9 @@ H2_CALL_DT = np.dtype([("run_idx", "<u4"), ("stream_id", "<u4"), ("how", "<u4"),
                        ("msg_off", "<u4"), ("msg_len", "<u4"), ("error_off", "<u4"), ("error_len", "<u4"), ("flags", "<u4")])   # == b2_h2_call, 64 bytes
 # b2_h2_msg / b2_h2_call flags of connections opted in with Context.h2_conn_set_gunzip (include/b2rpc.h)
 H2_FLAG_GUNZIPPED, H2_FLAG_GUNZIP_HOST, H2_FLAG_NO_GRPC_ENCODING = 64, 128, 256
+# b2_h2_msg flag of a call Context.h2_serve_batch answered on the device (msgs["reserved"] then holds the reply's grpc-status)
+H2_FLAG_ANSWERED = 512
+H2_REPLY_SPAN_DT = np.dtype([("off", "<u4"), ("len", "<u4"), ("n_answered", "<u4"), ("reserved", "<u4")])   # == b2_h2_reply_span, 16 bytes
 MSG_DT = np.dtype([("run_idx", "<u4"), ("frame_off", "<u4"), ("body_size", "<u4"), ("meta_size", "<u4"),
                    ("correlation_id", "<i8"), ("log_id", "<i8"),
                    ("attachment_size", "<i4"), ("compress_type", "<i4"), ("checksum_type", "<i4"), ("error_code", "<i4"),
@@ -142,6 +145,8 @@ def _load():
                                              C.POINTER(C.c_uint32), C.c_void_p, C.c_uint32]
     l.b2_h2_client_abandon_streams.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
     l.b2_h2_conn_set_gunzip.argtypes = [C.c_void_p, C.c_uint32, C.c_int]
+    l.b2_h2_serve_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32,
+                                    C.POINTER(C.c_uint32), C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p]
     l.b2_h2_pack_responses.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     l.b2_pack_requests.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     l.b2_pack_responses.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
@@ -158,7 +163,8 @@ ABI_SYMBOLS = ["b2_ctx_create", "b2_ctx_destroy", "b2_last_error", "b2_version",
                "b2_batch_execute", "b2_batch_execute_many", "b2_batch_download", "b2_batch_launch", "b2_batch_wait",
                "b2_elapsed_ms", "b2_batch_info", "b2_device_pci_bus_id", "b2_stage_times", "b2_crc32c_batch", "b2_crc32c_extend", "b2_snappy_max_compressed_length", "b2_snappy_raw_compress", "b2_snappy_get_uncompressed_length", "b2_snappy_raw_uncompress", "b2_snappy_uncompress_batch", "b2_snappy_compress_batch", "b2_hpack_reset", "b2_hpack_decode_batch", "b2_pack_requests", "b2_pack_responses", "b2_h2_scan_batch", "b2_h2_conn_reset", "b2_h2_configure", "b2_h2_process_batch", "b2_h2_pack_responses", "b2_counters_read",
                "b2_counters_device_ptr", "b2_counters_allreduce", "b2_h2_pack_requests", "b2_h2_conn_set_next_stream_id", "b2_h2_conn_peer_update",
-               "b2_h2_client_conn_reset", "b2_h2_client_process_batch", "b2_h2_client_abandon_streams", "b2_h2_conn_set_gunzip"]
+               "b2_h2_client_conn_reset", "b2_h2_client_process_batch", "b2_h2_client_abandon_streams", "b2_h2_conn_set_gunzip",
+               "b2_h2_serve_batch"]
 
 ECHO_METHOD = dict(service_full_name=b"example.EchoService", service_name=b"EchoService", method_name=b"Echo",
                    request_type_name=b"example.EchoRequest", handler=1, echo_attachment=1,
@@ -506,6 +512,24 @@ class Context:
         """The connection's gzip-compressed messages are inflated on the device by the next batches (H2_FLAG_GUNZIPPED: msg_off / msg_len
         then index the inflated bytes in out; H2_FLAG_GUNZIP_HOST: left for the host).  h2_conn_reset / h2_client_conn_reset clear it."""
         _check(lib.b2_h2_conn_set_gunzip(self._h, conn, 1 if enable else 0))
+
+    def h2_serve_batch(self, data, runs, msg_cap=None, out_cap=None, replies_cap=None, out=None, replies=None):
+        """h2_process_batch that also answers the gRPC calls of device echo methods (b2_h2_serve_batch).  Returns (run_status, msgs, out,
+        replies, spans): answered calls carry H2_FLAG_ANSWERED and their grpc-status in msgs["reserved"]; run i's replies are
+        replies[spans[i]["off"]:spans[i]["off"] + spans[i]["len"]], to be written after its control bytes."""
+        data = np.ascontiguousarray(data, dtype=np.uint8); runs = np.ascontiguousarray(runs, dtype=RUN_DT)
+        n = len(runs)
+        msg_cap = msg_cap or max(64, 64 * n)
+        out_cap = out_cap or max(1 << 16, n * (1 << 17))
+        replies_cap = replies_cap or max(1 << 16, n * (1 << 17))
+        rs = np.zeros(n, H2_RUN_STATUS_DT); msgs = np.zeros(msg_cap, H2_MSG_DT); nm = C.c_uint32(0); spans = np.zeros(n, H2_REPLY_SPAN_DT)
+        if out is None:
+            out = np.empty(out_cap, np.uint8)
+        if replies is None:
+            replies = np.empty(replies_cap, np.uint8)
+        _check(lib.b2_h2_serve_batch(self._h, data.ctypes.data, data.nbytes, runs.ctypes.data, n, rs.ctypes.data, msgs.ctypes.data, msg_cap,
+                                     C.byref(nm), out.ctypes.data, out.nbytes, replies.ctypes.data, replies.nbytes, spans.ctypes.data))
+        return rs, msgs[:nm.value], out, replies, spans
 
     def pack_requests(self, data, reqs, out_cap=None):
         """reqs: REQUEST_DT array (offsets into data).  Returns the packed frame of every request (b"" = rejected)."""

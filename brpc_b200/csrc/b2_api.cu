@@ -1173,16 +1173,39 @@ static void h2_gz_launch(b2_ctx* c, uint32_t n_runs, b2_h2_run_status* d_rs, M* 
     k_h2_gz_place<M><<<(n_runs + 31) / 32, 32, 0, c->stream>>>(n_runs, d_rs, d_msgs, per_run, region, d_gz);
     k_h2_gz_inflate<M><<<(n_slots + 63) / 64, 64, 0, c->stream>>>(c->d_bytes, n_runs, d_rs, d_msgs, per_run, c->d_unz, d_gz);
 }
+// the answering passes of b2_h2_serve_batch (k_h2_serve .. k_h2_serve_gather), enqueued after the gunzip passes and before the run
+// statuses are fetched.  Device scratch: per_run-strided records in the head rows and their reply offsets in d_frame_run, the list
+// k_h2_pack reads in d_aux / d_slot, its lengths in d_frame_off (free once the gunzip passes ran), group_first in d_run_tile_base,
+// the spans in d_refs, the packed replies in d_resp.
+struct H2Serve { void* replies; uint32_t replies_cap; b2_h2_reply_span* spans; };
+static void h2_serve_launch(b2_ctx* c, uint32_t n_runs, b2_h2_run_status* d_rs, b2_h2_msg* d_msgs, uint32_t per_run, uint32_t region, uint32_t reply_region) {
+    static_assert(kHeadBytes >= sizeof(b2_h2_response) && sizeof(MsgAux) >= sizeof(b2_h2_response) && sizeof(uint4) == sizeof(b2_h2_reply_span), "serve scratch");
+    b2_h2_response* d_strided = reinterpret_cast<b2_h2_response*>(c->d_heads);
+    b2_h2_response* d_list = reinterpret_cast<b2_h2_response*>(c->d_aux);
+    b2_h2_reply_span* d_spans = reinterpret_cast<b2_h2_reply_span*>(c->d_refs);
+    uint32_t* d_first = c->d_run_tile_base;
+    static_assert(sizeof(H2ServeCfg::identity) == sizeof(DevConfig::identity), "identity buffer");
+    H2ServeCfg cfg; cfg.n_methods = c->cfg.n_methods; cfg.identity_len = c->cfg.identity_len; memcpy(cfg.identity, c->cfg.identity, sizeof cfg.identity);
+    k_h2_serve<<<(n_runs + 31) / 32, 32, 0, c->stream>>>(c->d_bytes, (const b2_run*)c->d_meta, n_runs, c->d_methods, cfg, d_rs, d_msgs, per_run, c->d_unz, region,
+                                                         d_strided, c->d_frame_run, reply_region, d_spans);
+    k_h2_serve_scan<<<1, 32, 0, c->stream>>>(n_runs, d_spans, d_first);
+    k_h2_serve_compact<<<(n_runs * per_run + 255) / 256, 256, 0, c->stream>>>(n_runs, per_run, d_spans, d_first, d_strided, c->d_frame_run, d_list, c->d_slot);
+    k_h2_pack<<<(n_runs + kH2PackWarps - 1) / kH2PackWarps, kH2PackWarps * 32, 0, c->stream>>>(c->d_unz, c->d_bytes, c->d_unz, d_list, d_first, n_runs, c->d_h2,
+                                                                                             c->d_resp, c->d_slot, c->d_frame_off);
+    k_h2_serve_gather<<<(n_runs + kH2PackWarps - 1) / kH2PackWarps, kH2PackWarps * 32, 0, c->stream>>>(n_runs, d_first, c->d_slot, c->d_frame_off, c->d_resp, d_spans);
+}
 // ParseH2Message over a batch, server (b2_h2_msg) or client (b2_h2_call) connections: upload, the side's consume kernel (then the
-// gunzip passes), and a fetch of only what was produced.  Every run owns `region` bytes (acks from its start, records/bodies from
-// region/4) and per_run descriptors: three strided copies, then the descriptors are compacted into one list (run order).
+// gunzip passes, and for b2_h2_serve_batch the answering passes), and a fetch of only what was produced.  Every run owns `region` bytes
+// (acks from its start, records/bodies from region/4) and per_run descriptors: three strided copies, then the descriptors are compacted
+// into one list (run order).
 template <class M>
 static int h2_parse_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
-                          b2_h2_run_status* rs, M* descs, uint32_t cap, uint32_t* n_descs, void* out, uint32_t out_cap) {
+                          b2_h2_run_status* rs, M* descs, uint32_t cap, uint32_t* n_descs, void* out, uint32_t out_cap, const H2Serve* serve = nullptr) {
     constexpr bool kClient = std::is_same<M, b2_h2_call>::value;
-    if (!c || !bytes || !runs || !rs || !descs || !n_descs || !out) { set_err("null argument"); return B2_E_INVAL; }
+    if (!c || !bytes || !runs || !rs || !descs || !n_descs || !out || (serve && (!serve->replies || !serve->spans))) { set_err("null argument"); return B2_E_INVAL; }
     static_assert(sizeof(M) == 64 && sizeof(b2_h2_run_status) == 32, "h2 ABI layout");
-    if (nbytes > c->opt.max_batch_bytes || n_runs > c->opt.max_runs || out_cap > 2ull * c->opt.max_resp_bytes || cap > c->opt.max_msgs) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    if (nbytes > c->opt.max_batch_bytes || n_runs > c->opt.max_runs || out_cap > 2ull * c->opt.max_resp_bytes || cap > c->opt.max_msgs ||
+        (serve && serve->replies_cap > c->opt.max_resp_bytes)) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     *n_descs = 0;
     if (n_runs == 0) return B2_OK;
     for (uint32_t r = 0; r < n_runs; r++) {
@@ -1204,13 +1227,21 @@ static int h2_parse_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b
     else k_h2_consume<<<(n_runs + 31) / 32, 32, 0, c->stream>>>(c->d_bytes, (const b2_run*)c->d_meta, n_runs, c->d_h2, c->d_hpack, c->d_methods, c->cfg.n_methods,
                                                                  d_rs, d_descs, per_run, c->d_unz, region, h2_pool(c));
     if (h2_gz_wanted(c, runs, n_runs)) h2_gz_launch(c, n_runs, d_rs, d_descs, per_run, region);
+    const uint32_t reply_region = serve ? (serve->replies_cap / n_runs) & ~63u : 0;
+    if constexpr (!kClient) {
+        if (serve) {
+            h2_serve_launch(c, n_runs, d_rs, d_descs, per_run, region, reply_region);
+            CU(cudaMemcpyAsync(serve->spans, c->d_refs, sizeof(b2_h2_reply_span) * (size_t)n_runs, cudaMemcpyDeviceToHost, c->stream));
+        }
+    }
     CU(cudaMemcpyAsync(rs, d_rs, sizeof(b2_h2_run_status) * (size_t)n_runs, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
-    uint32_t total = 0, max_descs = 0, max_ctrl = 0, max_blob = 0;
+    uint32_t total = 0, max_descs = 0, max_ctrl = 0, max_blob = 0, max_reply = 0;
     for (uint32_t r = 0; r < n_runs; r++) {
         total += rs[r].n_msgs; if (rs[r].n_msgs > max_descs) max_descs = rs[r].n_msgs;
         if (rs[r].ctrl_len > max_ctrl) max_ctrl = rs[r].ctrl_len;
         if (rs[r].first_msg > max_blob) max_blob = rs[r].first_msg;             // (the kernel reports the blob bytes it used here)
+        if (serve && serve->spans[r].len > max_reply) max_reply = serve->spans[r].len;
     }
     if constexpr (!kClient) { if (total > cap) { set_err("msg_cap too small"); return B2_E_CAPACITY; } }
     std::vector<M> tmp((size_t)n_runs * (max_descs ? max_descs : 1));
@@ -1218,6 +1249,7 @@ static int h2_parse_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b
                                         sizeof(M) * (size_t)max_descs, n_runs, cudaMemcpyDeviceToHost, c->stream));
     if (max_ctrl) CU(cudaMemcpy2DAsync(out, region, c->d_unz, region, max_ctrl, n_runs, cudaMemcpyDeviceToHost, c->stream));
     if (max_blob) CU(cudaMemcpy2DAsync((uint8_t*)out + region / 4, region, c->d_unz + region / 4, region, max_blob, n_runs, cudaMemcpyDeviceToHost, c->stream));
+    if (max_reply) CU(cudaMemcpy2DAsync(serve->replies, reply_region, c->d_resp, reply_region, max_reply, n_runs, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     total = 0;
     for (uint32_t r = 0; r < n_runs; r++) {
@@ -1234,6 +1266,13 @@ extern "C" int b2_h2_process_batch(b2_ctx* c, const void* bytes, uint32_t nbytes
                                    b2_h2_run_status* rs, b2_h2_msg* msgs, uint32_t msg_cap, uint32_t* n_msgs,
                                    void* out, uint32_t out_cap) {
     return h2_parse_batch(c, bytes, nbytes, runs, n_runs, rs, msgs, msg_cap, n_msgs, out, out_cap);
+}
+extern "C" int b2_h2_serve_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
+                                 b2_h2_run_status* rs, b2_h2_msg* msgs, uint32_t msg_cap, uint32_t* n_msgs, void* out, uint32_t out_cap,
+                                 void* replies, uint32_t replies_cap, b2_h2_reply_span* spans) {
+    static_assert(sizeof(b2_h2_reply_span) == 16, "reply span ABI layout");
+    const H2Serve serve = { replies, replies_cap, spans };
+    return h2_parse_batch(c, bytes, nbytes, runs, n_runs, rs, msgs, msg_cap, n_msgs, out, out_cap, &serve);
 }
 
 extern "C" int b2_h2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_h2_response* resps, uint32_t n,
@@ -1252,8 +1291,7 @@ extern "C" int b2_h2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbyte
             (uint64_t)r.grpc_message_off + r.grpc_message_len > nbytes || r.content_type_len > 256 || r.grpc_message_len > 512) { set_err("bad response descriptor"); return B2_E_INVAL; }
         if ((r.flags & (B2_H2_RESP_BODY_IN_OUT | B2_H2_RESP_CT_IN_OUT)) && c->h2_last_out > c->opt.max_resp_bytes) { set_err("last h2 out buffer too large to stay resident"); return B2_E_CAPACITY; }
         if (i == 0 || r.conn != resps[i - 1].conn) first.push_back(i);
-        const uint64_t data = (uint64_t)r.body_len + 5;
-        const uint64_t need = data + 9 * (data / 16384 + 4) + 2ull * (r.content_type_len + r.grpc_message_len + 64) + 13 + 16;
+        const uint64_t need = h2_reply_bound(r.body_len, r.content_type_len, r.grpc_message_len);
         out_offs[i] = (uint32_t)total;
         total = (total + need + 15) & ~15ull;
         if (total > out_cap) { set_err("out_cap too small"); return B2_E_CAPACITY; }

@@ -595,6 +595,13 @@ __device__ __forceinline__ uint32_t put_dec_i32_h2(uint8_t* p, int32_t v) {     
 }
 constexpr uint32_t kH2FragCap = 1024;      // encoded header block of one response (":status", "content-type", trailers)
 constexpr uint32_t kH2PackWarps = 4;
+// The out bytes one reply of k_h2_pack may take, reserved by b2_h2_pack_responses and b2_h2_serve_batch alike: DATA (the body + the
+// 5-byte gRPC prefix) with a frame head per max_frame_size (>= 16384) piece, HEADERS + trailers (each header at most twice its bytes
+// + 64 once encoded), the deferred WINDOW_UPDATE and 16 bytes of slack.
+B2_HD uint64_t h2_reply_bound(uint32_t body_len, uint32_t content_type_len, uint32_t grpc_message_len) {
+    const uint64_t data = (uint64_t)body_len + 5;
+    return data + 9 * (data / 16384 + 4) + 2ull * (content_type_len + grpc_message_len + 64) + 13 + 16;
+}
 // One WARP per connection: lane 0 runs the serial part (window check, HPACK encode against the connection's table,
 // deferred WINDOW_UPDATE) into shared memory, then the whole warp writes the frames — the DATA payload, which is
 // nearly all of the bytes, with coalesced 16-byte copies.
@@ -1480,6 +1487,182 @@ __global__ void k_h2_gz_inflate(const uint8_t* bytes, uint32_t n_runs, const b2_
     bool big = false;
     m.msg_len = gz_input_stream<true>(src, n, B2_COMPRESS_TYPE_GZIP, out + m.msg_off, gz[t], &big);   // <= the bound: a failed check hands over less
     m.flags |= B2_H2_FLAG_GUNZIPPED;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// b2_h2_serve_batch: for gRPC calls of B2_HANDLER_ECHO methods, what follows the parse in brpc — ProcessHttpRequest's body checks
+// (policy/http_rpc_protocol.cpp:1631-1689), EchoServiceImpl::Echo and SendHttpResponse (:852-1027) — over what h2_consume_run and
+// the gunzip passes left on the device.  k_h2_serve (one thread per run: a connection's replies are ordered) decides every call,
+// writes error texts and copied bodies into the run's out region and builds b2_h2_response records; k_h2_serve_scan and
+// k_h2_serve_compact list them connection by connection for k_h2_pack, which frames them as for b2_h2_pack_responses;
+// k_h2_serve_gather closes the gaps between a run's replies.
+constexpr uint32_t kH2ServeCtMax = 256;                           // the content-type length b2_h2_pack_responses accepts
+// The longest error text (Controller::SetFailed, controller.cpp:468-490): "[" identity "]" "[E1003]" then request_type_name and
+// " needs to be created from a non-empty json, it has required fields." (67 bytes) = 1 + 63 + 1 + 7 + 95 + 67 = 234 bytes.
+// PercentEncode makes each byte at most "%xx": 702 bytes of grpc-message, more than the 512 b2_h2_pack_responses takes from the host.
+// k_h2_pack encodes it as a literal: the trailer holds grpc-status (at most 15 bytes) and grpc-message (1 + 1 + 12 + 3 length bytes +
+// the value), its scratch name || value, and the connection's HPACK table an entry of name + value + 32 bytes.
+struct H2ServeCfg { uint32_t n_methods, identity_len; char identity[64]; };   // of DevConfig: the registered methods, b2_set_server_identity
+constexpr uint32_t kH2ServeTextMax = 1 + (sizeof(H2ServeCfg::identity) - 1) + 1 + 7 + (sizeof(DevMethod::request_type) - 1) + 67;
+constexpr uint32_t kH2ServeMsgMax = 3 * kH2ServeTextMax;
+static_assert(kH2ServeTextMax == 234 && kH2ServeMsgMax == 702, "the longest error text");
+static_assert(15 + 17 + kH2ServeMsgMax <= kH2FragCap && 12 + kH2ServeMsgMax <= kH2FragCap, "grpc-message fits k_h2_pack's trailer and scratch");
+static_assert(12 + kH2ServeMsgMax + 32 <= 4096, "grpc-message fits an HPACK table entry");
+static_assert(1 + 2 + 3 + kH2ServeCtMax <= kH2FragCap && 12 + kH2ServeCtMax <= kH2FragCap, "content-type fits k_h2_pack's header block and scratch");
+enum H2ServeWhy : uint32_t { kServeOk = 0, kServeEmpty, kServeBadPrefix, kServeNoEncoding, kServeParse };
+// PercentEncode (grpc.cpp:121-141) of n bytes: only a-z A-Z - _ . ~ stay, everything else (digits too) is "%xx" in lowercase hex.
+// Counts when p is null.
+__device__ __forceinline__ uint32_t h2_pct(uint8_t* p, const uint8_t* s, uint32_t n) {
+    uint32_t o = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        const uint8_t c = s[i];
+        if ((c >= 'a' && c <= 'z') || (c >= 'A' && c <= 'Z') || c == '-' || c == '_' || c == '.' || c == '~') { if (p) p[o] = c; o++; }
+        else { if (p) { p[o] = '%'; p[o + 1] = (uint8_t)"0123456789abcdef"[c >> 4]; p[o + 2] = (uint8_t)"0123456789abcdef"[c & 15]; } o += 3; }
+    }
+    return o;
+}
+__device__ __forceinline__ uint32_t h2_pct_lit(uint8_t* p, const char* lit) {
+    uint32_t n = 0; while (lit[n]) n++;
+    return h2_pct(p, (const uint8_t*)lit, n);
+}
+// the grpc-message of an EREQUEST reply: PercentEncode of SetFailed's text ("[ip:port]" when an identity is set, "[E1003]", the reason
+// of ProcessHttpRequest :1637-1689); its length, and its bytes at p unless p is null
+__device__ __noinline__ uint32_t h2_serve_error(uint8_t* p, const H2ServeCfg& C, const DevMethod& M, uint32_t why) {
+    uint32_t o = 0;
+    auto at = [&]() { return p ? p + o : nullptr; };
+    if (C.identity_len) { o += h2_pct_lit(at(), "["); o += h2_pct(at(), (const uint8_t*)C.identity, C.identity_len); o += h2_pct_lit(at(), "]"); }
+    o += h2_pct_lit(at(), "[E1003]");
+    const uint8_t* rt = (const uint8_t*)M.request_type;
+    switch (why) {
+    case kServeEmpty: o += h2_pct(at(), rt, M.request_type_len); o += h2_pct_lit(at(), " needs to be created from a non-empty json, it has required fields."); break;
+    case kServeBadPrefix: o += h2_pct_lit(at(), "Invalid gRPC request"); break;
+    case kServeNoEncoding: o += h2_pct_lit(at(), "Fail to find header `grpc-encoding' in compressed gRPC request"); break;
+    default: o += h2_pct_lit(at(), "Fail to parse http body as "); o += h2_pct(at(), rt, M.request_type_len); break;
+    }
+    return o;
+}
+// The records of run r go to resps / reply_offs[r * per_run ...], their count to spans[r].n_answered.  Reply i of the run gets
+// h2_reply_bound bytes at reply_offs (16-byte aligned) in the run's reply_region bytes of the packed replies.
+__global__ void k_h2_serve(const uint8_t* bytes, const b2_run* runs, uint32_t n_runs, const DevMethod* methods, const H2ServeCfg cfg,
+                           b2_h2_run_status* rs, b2_h2_msg* msgs, uint32_t per_run, uint8_t* out, uint32_t region,
+                           b2_h2_response* resps, uint32_t* reply_offs, uint32_t reply_region, b2_h2_reply_span* spans) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_runs) return;
+    const uint32_t gbase = r * region;
+    uint32_t cur = region / 4 + rs[r].first_msg;                    // behind the parse's and the gunzip passes' bytes (a multiple of 16)
+    uint32_t rep = 0, k = 0;
+    for (uint32_t i = 0; i < rs[r].n_msgs; i++) {
+        b2_h2_msg& m = msgs[r * per_run + i];
+        if (!(m.flags & B2_H2_FLAG_GRPC) || m.content_type != 2 /*HTTP_CONTENT_PROTO*/ || m.method_idx < 0 || (uint32_t)m.method_idx >= cfg.n_methods) continue;
+        const DevMethod& M = methods[m.method_idx];
+        if (M.handler != B2_HANDLER_ECHO || M.response_compress_type != B2_COMPRESS_TYPE_NONE) continue;
+        uint32_t ct_off = 0, ct_len = 0;                            // SendHttpResponse answers with the request's content-type (:857-862)
+        for (uint32_t q = 0; q < m.headers_len;) {
+            const uint8_t* rec = out + m.headers_off + q;
+            const uint32_t nl = rec[0] | ((uint32_t)rec[1] << 8), vl = rec[2] | ((uint32_t)rec[3] << 8);
+            if (lit_eq(rec + 4, cstr_len(rec + 4, nl), "content-type")) { ct_off = m.headers_off + q + 4 + nl; ct_len = vl; }
+            q += 4 + nl + vl;
+        }
+        if (ct_len > kH2ServeCtMax) continue;
+        // ProcessHttpRequest (:1631-1689), in its order
+        const uint8_t* src = (m.flags & B2_H2_FLAG_BODY_IN_INPUT) ? bytes : out;
+        uint32_t why = kServeOk;
+        Span msg; msg.off = 0; msg.len = 0;
+        if (m.body_len == 0) why = kServeEmpty;                     // EchoRequest has a required field
+        else if (!(m.flags & B2_H2_FLAG_GRPC_PREFIX_OK)) why = kServeBadPrefix;
+        else if (m.flags & B2_H2_FLAG_GRPC_COMPRESSED) {
+            if (m.flags & B2_H2_FLAG_NO_GRPC_ENCODING) why = kServeNoEncoding;
+            else if (m.flags & B2_H2_FLAG_GUNZIPPED) src = out;     // the inflated bytes
+            else continue;                                          // another encoding, or left to the host's zlib
+        }
+        if (why == kServeOk && !decode_echo_request(src + m.msg_off, m.msg_len, msg)) why = kServeParse;
+        b2_h2_response R;
+        R.conn = (uint32_t)runs[r].socket_id; R.stream_id = m.stream_id; R.status_code = 200;
+        R.flags = B2_H2_RESP_GRPC | B2_H2_RESP_CT_IN_OUT; R.content_type_off = ct_off; R.content_type_len = ct_len;
+        R.body_off = 0; R.body_len = 0; R.grpc_status = 0; R.grpc_message_off = 0; R.grpc_message_len = 0; R.reserved = 0;
+        uint32_t put = 0;                                           // bytes the reply needs in out
+        const uint32_t at = m.msg_off + msg.off, vn = varint_len(msg.len);
+        if (why != kServeOk) {                                      // an empty body, the 5-byte prefix and the trailers (:937-959, :1008-1011)
+            R.grpc_status = 3;                                      // ErrorCodeToGrpcStatus(EREQUEST), grpc.cpp:63-65
+            put = R.grpc_message_len = h2_serve_error(nullptr, cfg, M, why);
+        } else {                                                    // EchoResponse{message}: 0a varint(len) message
+            R.body_len = 1 + vn + msg.len;
+            // the request already holds that field when the tag is 0a and the length took exactly varint_len(len) bytes
+            bool same = msg.off >= 1 + vn && src[at - vn - 1] == 0x0a;
+            unsigned long long v = 0;
+            for (uint32_t j = 0; same && j < vn; j++) {
+                const uint8_t b = src[at - vn + j];
+                same = (j + 1 < vn) == ((b & 0x80) != 0); v |= (unsigned long long)(b & 0x7f) << (7 * j);
+            }
+            if (same && v == msg.len) { R.body_off = at - vn - 1; R.flags |= src == bytes ? B2_H2_RESP_BODY_IN_INPUT : B2_H2_RESP_BODY_IN_OUT; }
+            else put = R.body_len;
+        }
+        const uint64_t next = (rep + h2_reply_bound(R.body_len, ct_len, R.grpc_message_len) + 15) & ~15ull;
+        if (next > reply_region) break;                             // the run's reply region is full: the rest is the host's
+        if (put && (uint64_t)cur + put > region) continue;          // no room in out for this call's bytes
+        if (why != kServeOk) { R.grpc_message_off = gbase + cur; (void)h2_serve_error(out + gbase + cur, cfg, M, why); }
+        else if (put) {
+            uint8_t* o = out + gbase + cur;
+            *o++ = 0x0a; o = put_varint(o, msg.len);
+            thread_copy(o, src + at, msg.len);
+            R.body_off = gbase + cur; R.flags |= B2_H2_RESP_BODY_IN_OUT;
+        }
+        cur += (put + 15u) & ~15u;
+        resps[r * per_run + k] = R; reply_offs[r * per_run + k] = r * reply_region + rep; k++;
+        rep = (uint32_t)next;
+        m.flags |= B2_H2_FLAG_ANSWERED; m.reserved = (uint32_t)R.grpc_status;
+    }
+    rs[r].first_msg = cur - region / 4;                             // the strided copy-back brings the texts and bodies home
+    b2_h2_reply_span sp; sp.off = r * reply_region; sp.len = 0; sp.n_answered = k; sp.reserved = 0;
+    spans[r] = sp;
+}
+// One warp: group_first (k_h2_pack's list of connections, one per run, empty ones included) = the exclusive prefix of the answered counts
+__global__ void k_h2_serve_scan(uint32_t n_runs, const b2_h2_reply_span* spans, uint32_t* group_first) {
+    const uint32_t lane = threadIdx.x, per = (n_runs + 31) / 32;
+    const uint32_t lo = min(lane * per, n_runs), hi = min(lo + per, n_runs);
+    uint32_t sum = 0;
+    for (uint32_t r = lo; r < hi; r++) sum += spans[r].n_answered;
+    uint32_t incl = sum;
+    for (uint32_t d = 1; d < 32; d <<= 1) {
+        const uint32_t v = __shfl_sync(0xffffffffu, incl, lane >= d ? lane - d : lane);
+        if (lane >= d) incl += v;
+    }
+    uint32_t at = incl - sum;
+    for (uint32_t r = lo; r < hi; r++) { group_first[r] = at; at += spans[r].n_answered; }
+    if (lane == 31) group_first[n_runs] = incl;
+}
+// one thread per descriptor slot: the records and reply offsets move from per_run strides into that list
+__global__ void k_h2_serve_compact(uint32_t n_runs, uint32_t per_run, const b2_h2_reply_span* spans, const uint32_t* group_first,
+                                   const b2_h2_response* strided, const uint32_t* strided_offs, b2_h2_response* resps, uint32_t* reply_offs) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x, r = t / per_run, k = t % per_run;
+    if (r >= n_runs || k >= spans[r].n_answered) return;
+    resps[group_first[r] + k] = strided[t]; reply_offs[group_first[r] + k] = strided_offs[t];
+}
+// One warp per run: the replies k_h2_pack wrote at their reserved offsets move down to follow each other.  The move is forward inside
+// the run's region: every 512-byte step is loaded whole before any of it is stored, and a step never stores past what it loaded.
+__global__ void __launch_bounds__(kH2PackWarps * 32) k_h2_serve_gather(uint32_t n_runs, const uint32_t* group_first, const uint32_t* reply_offs,
+                                                                       const uint32_t* reply_lens, uint8_t* replies, b2_h2_reply_span* spans) {
+    const uint32_t lane = threadIdx.x & 31, r = blockIdx.x * kH2PackWarps + (threadIdx.x >> 5);
+    if (r >= n_runs) return;
+    const uint32_t start = spans[r].off;
+    uint32_t dst = start;
+    for (uint32_t i = group_first[r]; i < group_first[r + 1]; i++) {
+        const uint32_t src = reply_offs[i], n = reply_lens[i];
+        if (src != dst) {
+            for (uint32_t s = 0; s < n; s += 512) {
+                const uint32_t o = s + 16 * lane;
+                uint4 v = make_uint4(0, 0, 0, 0);
+                if (o < n) v = *reinterpret_cast<const uint4*>(replies + src + o);     // (src is 16-byte aligned)
+                __syncwarp();
+#pragma unroll
+                for (uint32_t j = 0; j < 16; j++)
+                    if (o + j < n) replies[dst + o + j] = (uint8_t)((j < 4 ? v.x : j < 8 ? v.y : j < 12 ? v.z : v.w) >> (8 * (j & 3)));
+                __syncwarp();
+            }
+        }
+        dst += n;
+    }
+    if (lane == 0) spans[r].len = dst - start;
 }
 #endif
 }  // namespace b2

@@ -731,6 +731,39 @@ int  b2_h2_client_abandon_streams(b2_ctx* ctx, uint32_t conn, const uint32_t* st
                                              not set on a client call an earlier verdict already failed */
 int  b2_h2_conn_set_gunzip(b2_ctx* ctx, uint32_t conn, int enable);
 
+/* ---- gRPC calls to device echo methods answered on the device, in the parse call ------------------------------------------------
+ * b2_h2_serve_batch: b2_h2_process_batch, then for the calls it can answer what brpc does next — ProcessHttpRequest's body checks
+ * (policy/http_rpc_protocol.cpp:1631-1689), EchoServiceImpl::Echo, SendHttpResponse (:852-1027) — framed like b2_h2_pack_responses.
+ * rs, msgs and out are what b2_h2_process_batch returns for the same input (gunzip included), except that answered calls carry
+ * B2_H2_FLAG_ANSWERED and their reply's grpc-status in msgs[i].reserved.
+ * A call is answered when it is gRPC, its content type is HTTP_CONTENT_PROTO, method_idx names a B2_HANDLER_ECHO method whose
+ * response_compress_type is NONE, and its content-type value is at most 256 bytes; everything else (unknown paths included) is left to
+ * the host unchanged.  The verdicts, in the reference's order, each an EREQUEST reply unless the call is OK:
+ *   - an empty body: "<request_type_name> needs to be created from a non-empty json, it has required fields." (:1637-1643);
+ *   - RemoveGrpcPrefix fails: "Invalid gRPC request";
+ *   - a compressed message with B2_H2_FLAG_NO_GRPC_ENCODING: "Fail to find header `grpc-encoding' in compressed gRPC request";
+ *     with B2_H2_FLAG_GUNZIPPED the inflated bytes go on; any other compressed message is not answered;
+ *   - the message is not an EchoRequest (proto2, required `message`): "Fail to parse http body as <request_type_name>";
+ *   - OK: :status 200, the request's content-type, the body EchoResponse{message} (0a varint(len) message: referenced in the input or
+ *     the inflated bytes when the request holds exactly those bytes, else written into the run's out region), grpc-status 0.
+ * An error reply is :status 200, the request's content-type, an empty message (5-byte prefix), grpc-status 3 (ErrorCodeToGrpcStatus,
+ * grpc.cpp:54-81) and grpc-message = PercentEncode (grpc.cpp:121-141: a-z A-Z - _ . ~ kept, every other byte "%xx") of the text
+ * Controller::SetFailed builds (controller.cpp:468-490): "[ip:port]" (b2_set_server_identity, when set), "[E1003]", the reason.  Up to 702
+ * bytes; the text is written into the run's out region.  A call whose bytes do not fit behind the parse's and the gunzip's bytes in the
+ * run's out region is not answered; later calls still may be.
+ * Replies: run i's region of `replies` is replies_cap / n_runs bytes (rounded down to 64).  Each answered call reserves the bound of
+ * b2_h2_pack_responses there; when the next does not fit, the run's remaining calls are not answered.  Run i's replies are
+ * replies[spans[i].off, + spans[i].len), in message order, spans[i].n_answered of them: write them after rs[i].ctrl_*.  The encoder
+ * HPACK table, the remote windows and the deferred WINDOW_UPDATE end as after b2_h2_process_batch + b2_h2_pack_responses on the same
+ * records, and the call leaves the batch readable by b2_h2_pack_responses: the host answers the rest, zero-copy as before.
+ * replies_cap <= the context's max_resp_bytes.  Not modelled: concurrency limiters (EOVERCROWDED), auth, grpc-timeout; a request
+ * attachment is always empty here, so echo_attachment changes nothing. */
+#define B2_H2_FLAG_ANSWERED 512u   /* b2_h2_msg.flags: the device wrote this call's reply (b2_h2_serve_batch) */
+typedef struct b2_h2_reply_span { uint32_t off, len, n_answered, reserved; } b2_h2_reply_span;   /* 16 bytes */
+int  b2_h2_serve_batch(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
+                       b2_h2_run_status* rs, b2_h2_msg* msgs, uint32_t msg_cap, uint32_t* n_msgs, void* out, uint32_t out_cap,
+                       void* replies, uint32_t replies_cap, b2_h2_reply_span* spans);
+
 /* ---- counters (bvar::Adder-like, SURVEY §8e): per-GPU totals accumulated by
  * the kernels: [0] in_bytes [1] in_msgs [2] out_bytes [3] out_msgs [4] errors
  * [5] batches [6..7] reserved.  The cross-GPU reduce is an NCCL all-reduce on
