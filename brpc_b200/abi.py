@@ -50,6 +50,16 @@ MSG_DT = np.dtype([("run_idx", "<u4"), ("frame_off", "<u4"), ("body_size", "<u4"
                    ("has_bits", "<u2"), ("protocol", "u1"), ("content_type", "u1"),
                    ("method_idx", "<i2"), ("status", "<u2"), ("resp_off", "<u4"), ("resp_len", "<u4")])
 assert RUN_DT.itemsize == 24 and RUN_STATUS_DT.itemsize == 32 and MSG_DT.itemsize == 64
+# the stream table (b2_stream_*)
+STREAM_DESC_DT = np.dtype([("stream_id", "<i8"), ("remote_stream_id", "<i8"), ("host_socket_id", "<u8"), ("flags", "<u4"), ("reserved", "<u4")])
+STREAM_MSG_DT = np.dtype([("stream_id", "<i8"), ("first_frame", "<u4"), ("n_frames", "<u4"), ("off", "<u4"), ("len", "<u4"), ("flags", "<u4"), ("reserved", "<u4")])
+STREAM_EVENT_DT = np.dtype([("stream_id", "<i8"), ("host_socket_id", "<u8"), ("local_consumed", "<u8"), ("remote_consumed", "<u8"), ("n_msgs", "<u4"),
+                            ("first_msg", "<u4"), ("consumed_bytes", "<u4"), ("flags", "<u4"), ("fb_off", "<u4"), ("fb_len", "<u4"), ("close_off", "<u4"),
+                            ("close_len", "<u4"), ("handover_msg", "<u4"), ("pending_bytes", "<u4"), ("reserved", "<u4", (2,))])
+assert STREAM_DESC_DT.itemsize == 32 and STREAM_MSG_DT.itemsize == 32 and STREAM_EVENT_DT.itemsize == 80
+STREAM_CONNECTED, STREAM_NEED_FEEDBACK, STREAM_CLOSED, STREAM_HANDED_OVER = 1, 2, 4, 8
+STREAM_MSG_IN_INPUT = 1
+STREAM_EV_REMOTE_CONSUMED_MOVED, STREAM_EV_CLOSED_BY_RST, STREAM_EV_CLOSED_BY_CLOSE, STREAM_EV_HANDED_OVER = 1, 2, 4, 8
 
 
 class Method(C.Structure):
@@ -69,6 +79,17 @@ class BatchResult(C.Structure):
                 ("msgs", C.c_void_p), ("n_msgs", C.c_uint32),
                 ("resp", C.c_void_p), ("resp_bytes", C.c_uint32),
                 ("kernel_ms", C.c_float), ("n_launches", C.c_uint32), ("refs", C.c_void_p), ("iov", C.c_void_p)]
+
+
+class StreamState(C.Structure):
+    _fields_ = [("local_consumed", C.c_uint64), ("remote_consumed", C.c_uint64), ("pending_bytes", C.c_uint32), ("flags", C.c_uint32),
+                ("error_code", C.c_int32), ("reserved", C.c_uint32)]
+
+
+class StreamBatchResult(C.Structure):
+    _fields_ = [("msgs", C.c_void_p), ("n_msgs", C.c_uint32), ("events", C.c_void_p), ("n_events", C.c_uint32),
+                ("out", C.c_void_p), ("out_bytes", C.c_uint32), ("ctrl", C.c_void_p), ("ctrl_bytes", C.c_uint32),
+                ("run_ctrl", C.c_void_p), ("n_runs", C.c_uint32)]
 
 
 REF_DT = np.dtype([("prefix_len", "<u4"), ("src_off", "<u4"), ("src_len", "<u4"), ("reserved", "<u4")])
@@ -150,6 +171,13 @@ def _load():
     l.b2_h2_pack_responses.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     l.b2_pack_requests.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     l.b2_pack_responses.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
+    l.b2_stream_configure.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]
+    l.b2_stream_open.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+    l.b2_stream_set_connected.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
+    l.b2_stream_close.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
+    l.b2_stream_query.argtypes = [C.c_void_p, C.c_int64, C.POINTER(StreamState)]
+    l.b2_stream_take_pending.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
+    l.b2_stream_results.argtypes = [C.c_void_p, C.POINTER(StreamBatchResult)]
     l.b2_counters_read.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
     l.b2_counters_device_ptr.restype = C.c_void_p; l.b2_counters_device_ptr.argtypes = [C.c_void_p]
     return l
@@ -164,7 +192,8 @@ ABI_SYMBOLS = ["b2_ctx_create", "b2_ctx_destroy", "b2_last_error", "b2_version",
                "b2_elapsed_ms", "b2_batch_info", "b2_device_pci_bus_id", "b2_stage_times", "b2_crc32c_batch", "b2_crc32c_extend", "b2_snappy_max_compressed_length", "b2_snappy_raw_compress", "b2_snappy_get_uncompressed_length", "b2_snappy_raw_uncompress", "b2_snappy_uncompress_batch", "b2_snappy_compress_batch", "b2_hpack_reset", "b2_hpack_decode_batch", "b2_pack_requests", "b2_pack_responses", "b2_h2_scan_batch", "b2_h2_conn_reset", "b2_h2_configure", "b2_h2_process_batch", "b2_h2_pack_responses", "b2_counters_read",
                "b2_counters_device_ptr", "b2_counters_allreduce", "b2_h2_pack_requests", "b2_h2_conn_set_next_stream_id", "b2_h2_conn_peer_update",
                "b2_h2_client_conn_reset", "b2_h2_client_process_batch", "b2_h2_client_abandon_streams", "b2_h2_conn_set_gunzip",
-               "b2_h2_serve_batch"]
+               "b2_h2_serve_batch", "b2_stream_configure", "b2_stream_open", "b2_stream_set_connected", "b2_stream_close", "b2_stream_query",
+               "b2_stream_take_pending", "b2_stream_results"]
 
 ECHO_METHOD = dict(service_full_name=b"example.EchoService", service_name=b"EchoService", method_name=b"Echo",
                    request_type_name=b"example.EchoRequest", handler=1, echo_attachment=1,
@@ -356,6 +385,53 @@ class Context:
         _check(lib.b2_batch_collect(self._h, C.byref(res)))
         rs, msgs, resp = self._views(res)
         return rs, msgs, resp, self._info(res)
+
+    # ---- the stream table: the receiving side of brpc's Stream on the device (b2_stream_*) ----
+    def stream_configure(self, max_streams, pending_bytes, out_bytes=0):
+        _check(lib.b2_stream_configure(self._h, max_streams, pending_bytes, out_bytes))
+
+    def stream_open(self, streams):
+        """streams: STREAM_DESC_DT array or a list of (stream_id, remote_stream_id, host_socket_id, flags)."""
+        if not isinstance(streams, np.ndarray):
+            a = np.zeros(len(streams), STREAM_DESC_DT)
+            for i, t in enumerate(streams):
+                a[i] = tuple(t) + (0,)
+            streams = a
+        streams = np.ascontiguousarray(streams, dtype=STREAM_DESC_DT)
+        _check(lib.b2_stream_open(self._h, streams.ctypes.data, len(streams)))
+
+    def stream_set_connected(self, stream_id, remote_stream_id, flags=0):
+        """Returns the FEEDBACK frame SetConnected writes (b"" = none)."""
+        buf = C.create_string_buffer(64); n = C.c_uint32(0)
+        _check(lib.b2_stream_set_connected(self._h, stream_id, remote_stream_id, flags, buf, 64, C.byref(n)))
+        return buf.raw[:n.value]
+
+    def stream_close(self, stream_id):
+        """Returns the CLOSE frame to write (b"" = none)."""
+        buf = C.create_string_buffer(64); n = C.c_uint32(0)
+        _check(lib.b2_stream_close(self._h, stream_id, buf, 64, C.byref(n)))
+        return buf.raw[:n.value]
+
+    def stream_query(self, stream_id):
+        st = StreamState()
+        _check(lib.b2_stream_query(self._h, stream_id, C.byref(st)))
+        return {"local_consumed": st.local_consumed, "remote_consumed": st.remote_consumed, "pending_bytes": st.pending_bytes,
+                "flags": st.flags, "error_code": st.error_code}
+
+    def stream_take_pending(self, stream_id, cap):
+        buf = np.zeros(max(1, cap), np.uint8); n = C.c_uint32(0)
+        _check(lib.b2_stream_take_pending(self._h, stream_id, buf.ctypes.data, cap, C.byref(n)))
+        return buf[:n.value].tobytes()
+
+    def stream_results(self):
+        """(msgs, events, out, ctrl, run_ctrl) of the last collected batch: views of context-owned memory, valid until the next batch call."""
+        r = StreamBatchResult()
+        _check(lib.b2_stream_results(self._h, C.byref(r)))
+
+        def view(ptr, nbytes, dt):
+            return np.ctypeslib.as_array((C.c_uint8 * nbytes).from_address(ptr)).view(dt) if nbytes else np.zeros(0, dt)
+        return (view(r.msgs, 32 * r.n_msgs, STREAM_MSG_DT), view(r.events, 80 * r.n_events, STREAM_EVENT_DT), view(r.out, r.out_bytes, np.uint8),
+                view(r.ctrl, r.ctrl_bytes, np.uint8), view(r.run_ctrl, 8 * r.n_runs, np.uint32).reshape(-1, 2))
 
     def batch_info(self):
         out = (C.c_uint32 * 4)()

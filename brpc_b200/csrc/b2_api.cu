@@ -7,6 +7,7 @@
 #include <time.h>
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
 #include <mutex>
 #include <string>
 #include <unordered_map>
@@ -52,6 +53,12 @@ struct b2_ctx {
     uint4* d_refs = nullptr; b2_resp_ref* h_refs = nullptr; int input_mode = B2_INPUT_COPY, resp_mode = B2_RESP_COPY; const uint8_t* pull_bytes = nullptr; uint32_t small_off_refs = 0;
     uint32_t* d_crc_adv = nullptr; unsigned long long* d_counters = nullptr; uint32_t* d_totals = nullptr; DevMethod* d_methods = nullptr;
     size_t meta_tile_off = 0; uint32_t max_tiles = 0; uint32_t n_sms = 132; bool use_tma_pack = true; uint32_t stage_mask = 7;  // debug: 1 front stages, 2 k_pack_tma, 4 k_pack_slow
+    // stream table (b2_stream_*): the device side in `sp`; the host keeps the keys (it picks the table slots) and the free pool slots
+    StreamPass sp = {}; bool has_streams = false, stream_armed = false, stream_ran = false, stream_valid = false;
+    uint32_t st_max = 0, st_open = 0; std::vector<long long> st_keys; std::vector<uint8_t> st_state; std::vector<uint32_t> st_pool, st_pool_free;
+    void* d_st_block[10] = {}; void* h_st_mapped[5] = {}; uint32_t* h_st_cnts = nullptr; uint8_t* h_st_out = nullptr; uint8_t* h_st_ctl = nullptr; uint8_t* d_st_ctl = nullptr;
+    b2_stream_msg* h_st_msgs = nullptr; b2_stream_event* h_st_events = nullptr; uint8_t* h_st_ctrl = nullptr; uint32_t* h_st_run_ctrl = nullptr;
+    cudaEvent_t st_ev[6] = {};
     // pinned host mirrors
     b2_run_status* h_run_status = nullptr; b2_msg_desc* h_msgs = nullptr; uint8_t* h_resp = nullptr;
     uint32_t* h_totals = nullptr; uint32_t* h_run_tile_base = nullptr;
@@ -135,6 +142,7 @@ extern "C" void b2_block_free(void* p) { if (p) block_pool().free(p); }
 extern "C" uint64_t b2_block_pool_host_allocs(void) { std::lock_guard<std::mutex> g(block_pool().mu); return block_pool().n_host_alloc; }
 
 static void ring_halt(b2_ctx* c);
+static void stream_free(b2_ctx* c);
 extern "C" void b2_ctx_destroy(b2_ctx* c) {
     if (!c) return;
     cudaSetDevice(c->opt.device);
@@ -148,6 +156,7 @@ extern "C" void b2_ctx_destroy(b2_ctx* c) {
     cudaFree(c->d_scan_tmp); cudaFree(c->d_resp); cudaFree(c->d_unz); cudaFree(c->d_snappy_tab); cudaFree(c->d_refs); cudaFree(c->d_iov); cudaFreeHost(c->h_iov); cudaFree(c->d_frame_row); cudaFree(c->d_rows); cudaFreeHost(c->h_refs); cudaFree(c->d_hpack); cudaFree(c->d_h2); cudaFree(c->d_h2_streams); cudaFree(c->d_h2_slots); cudaFree(c->d_h2_gz_merge); cudaFree(c->d_counters); cudaFree(c->d_totals); cudaFree(c->d_methods); cudaFree(c->d_crc_adv); cudaFree(c->d_meta); cudaFree(c->d_small); cudaFreeHost(c->h_meta); cudaFreeHost(c->h_small);
     cudaFreeHost(c->h_run_status); cudaFreeHost(c->h_msgs); cudaFreeHost(c->h_resp); cudaFreeHost(c->h_totals);
     cudaFreeHost(c->h_run_tile_base);
+    stream_free(c);
     for (int i = 0; i <= kMaxStages; i++) if (c->ev[i]) cudaEventDestroy(c->ev[i]);
     if (c->stream) cudaStreamDestroy(c->stream);
     delete c;
@@ -357,6 +366,7 @@ extern "C" int b2_batch_upload(b2_ctx* c, const void* bytes, uint32_t nbytes, co
     if ((c->input_mode != B2_INPUT_PULL && nbytes > c->opt.max_batch_bytes) || nbytes >= (1u << 31) || n_runs > c->opt.max_runs) { set_err("batch exceeds ctx capacity"); return B2_E_CAPACITY; }
     uint64_t covered = 0; for (uint32_t r = 0; r < n_runs; r++) covered += runs[r].length;
     if (c->input_mode == B2_INPUT_PULL && covered > c->opt.max_batch_bytes) { set_err("runs exceed ctx capacity"); return B2_E_CAPACITY; }
+    c->stream_valid = false;
     c->covered = covered;                           // (what the runs hold: with B2_INPUT_PULL nbytes spans the caller's whole arena)
     CU(cudaSetDevice(c->opt.device));
     if (c->adaptive_tile) {
@@ -422,6 +432,24 @@ extern "C" int b2_batch_upload(b2_ctx* c, const void* bytes, uint32_t nbytes, co
     return B2_OK;
 }
 
+// The stream pass of a batch call (k_stream_*): behind the stage that wrote msgs[], on the same stream, inside the call's synchronisation.
+static const char* const kStreamStages[5] = { "stream_route", "stream_alloc", "stream_group", "stream_run", "stream_rst" };
+static int launch_stream_pass(b2_ctx* c, const BatchPtrs& B, cudaStream_t s, uint32_t& launches) {
+    const StreamPass& S = c->sp;
+    const uint32_t msg_bound = c->small ? c->small_msgs : c->opt.max_msgs, sms = c->n_sms;
+    auto grid = [&](uint32_t items, uint32_t per_block, uint32_t most) { const uint32_t g = (items + per_block - 1) / per_block; return g < 1 ? 1u : g < most ? g : most; };
+    CU(cudaMemsetAsync(S.cnts, 0, 4 * (16 + 2 * (size_t)S.cap), s));          // counters | cnt | fill
+    CU(cudaEventRecord(c->st_ev[0], s));
+    k_stream_route<<<grid(msg_bound, 256, sms * 4), 256, 0, s>>>(B, S); CU(cudaEventRecord(c->st_ev[1], s));
+    k_stream_alloc<<<grid(c->st_max, 256, sms), 256, 0, s>>>(B, S); CU(cudaEventRecord(c->st_ev[2], s));
+    k_stream_group<<<grid(msg_bound, 256, sms * 4), 256, 0, s>>>(B, S); CU(cudaEventRecord(c->st_ev[3], s));
+    k_stream_run<<<grid(c->st_max, 4, sms * 8), 128, 0, s>>>(B, S); CU(cudaEventRecord(c->st_ev[4], s));
+    k_stream_rst<<<grid(c->n_runs, 4, sms * 4), 128, 0, s>>>(B, S); CU(cudaEventRecord(c->st_ev[5], s));
+    CU(cudaMemcpyAsync(c->h_st_cnts, S.cnts, 64, cudaMemcpyDeviceToHost, s));
+    launches += 5; c->stream_ran = true;
+    return B2_OK;
+}
+
 static int launch_pipeline(b2_ctx* c) {
     const BatchPtrs B = make_ptrs(c);
     DevConfig C = c->cfg;
@@ -436,12 +464,15 @@ static int launch_pipeline(b2_ctx* c) {
     const uint32_t mask = c->stage_mask;
     if (mask & 1) CU(cudaMemsetAsync(B.totals, 0, 48, s));
     CU(cudaEventRecord(c->ev[0], s));
+    c->stream_ran = false;
     if (c->n_runs == 0) { c->n_stages = 0; c->last_launches = 0; return B2_OK; }
     if (c->small && c->use_fused_small && !prof) {
         // latency path: the whole pipeline in one launch, one CTA
         k_small<<<1, kSmallThreads, sizeof(SmallSmem), s>>>(B, C);
+        launches = 1;
+        if (c->stream_armed) { int rc = launch_stream_pass(c, B, s, launches); if (rc != B2_OK) return rc; }
         c->stage_names[0] = "fused_small"; cudaEventRecord(c->ev[1], s);
-        c->n_stages = 1; c->last_launches = 1;
+        c->n_stages = 1; c->last_launches = launches;
         CU(cudaGetLastError());
         return B2_OK;
     }
@@ -491,6 +522,7 @@ static int launch_pipeline(b2_ctx* c) {
         k_emit_iov<<<sms * 4, 256, 0, s>>>(B, c->d_iov, (unsigned long long)(uintptr_t)c->h_resp, (unsigned long long)(uintptr_t)c->host_bytes);
         launches++; mark("emit_iov");
     }
+    if (c->stream_armed) { int rc = launch_stream_pass(c, B, s, launches); if (rc != B2_OK) return rc; }
     if (!prof) { c->stage_names[0] = "pipeline"; cudaEventRecord(c->ev[1], s); st = 1; }
     c->n_stages = st; c->last_launches = launches;
     CU(cudaGetLastError());
@@ -500,6 +532,7 @@ static int launch_pipeline(b2_ctx* c) {
 extern "C" int b2_batch_execute(b2_ctx* c, float* kernel_ms, uint32_t* n_launches) {
     if (!c || !c->uploaded) { set_err("no batch uploaded"); return B2_E_INVAL; }
     CU(cudaSetDevice(c->opt.device));
+    if (c->stream_armed) { set_err("a submitted batch of a context with a stream table must be collected first: this entry point replays a batch and does not run the stream pass"); return B2_E_INVAL; }
     c->profile_stages = true;
     int rc = launch_pipeline(c);
     c->profile_stages = false;
@@ -519,6 +552,7 @@ extern "C" int b2_batch_execute_many(b2_ctx* c, uint32_t steps, float* total_ms,
     cudaEvent_t e0, e1;
     CU(cudaEventCreate(&e0)); CU(cudaEventCreate(&e1));
     CU(cudaEventRecord(e0, c->stream));
+    if (c->stream_armed) { set_err("a submitted batch of a context with a stream table must be collected first: this entry point replays a batch and does not run the stream pass"); return B2_E_INVAL; }
     uint32_t launches = 0;
     for (uint32_t i = 0; i < steps; i++) {
         int rc = launch_pipeline(c);
@@ -541,6 +575,7 @@ extern "C" int b2_batch_launch(b2_ctx* c) {
     if (!c || !c->uploaded) { set_err("no batch uploaded"); return B2_E_INVAL; }
     CU(cudaSetDevice(c->opt.device));
     if (c->first_pending) { CU(cudaEventRecord(c->ev_first, c->stream)); c->first_pending = false; }
+    if (c->stream_armed) { set_err("a submitted batch of a context with a stream table must be collected first: this entry point replays a batch and does not run the stream pass"); return B2_E_INVAL; }
     int rc = launch_pipeline(c);
     if (rc != B2_OK) return rc;
     CU(cudaEventRecord(c->ev_last, c->stream));
@@ -607,6 +642,7 @@ static int download_normal(b2_ctx* c, b2_batch_result* out) {
     const bool iovec = c->resp_mode == B2_RESP_IOVEC;
     if (n_msgs && c->cfg.by_ref && !iovec) CU(cudaMemcpyAsync(c->h_refs, c->d_refs, sizeof(b2_resp_ref) * (size_t)n_msgs, cudaMemcpyDeviceToHost, c->stream));
     if (n_msgs && iovec) CU(cudaMemcpyAsync(c->h_iov, c->d_iov, 32 * (size_t)n_msgs, cudaMemcpyDeviceToHost, c->stream));
+    if (c->stream_ran && c->h_st_cnts[2]) CU(cudaMemcpyAsync(c->h_st_out, c->sp.out, c->h_st_cnts[2], cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     out->refs = c->cfg.by_ref && !iovec ? c->h_refs : nullptr;
     out->iov = iovec ? c->h_iov : nullptr;
@@ -638,6 +674,10 @@ extern "C" int b2_batch_download(b2_ctx* c, b2_batch_result* out) {
             out->resp = c->h_small + c->small_off_resp; out->resp_bytes = tot[1];
             out->refs = c->cfg.by_ref ? reinterpret_cast<const b2_resp_ref*>(c->h_small + c->small_off_refs) : nullptr;
             if (c->resp_mode == B2_RESP_IOVEC) refs_to_iov(c, out, c->host_bytes);
+            if (c->stream_ran && c->h_st_cnts[2]) {          // multi-frame messages completed: their bytes follow
+                CU(cudaMemcpyAsync(c->h_st_out, c->sp.out, c->h_st_cnts[2], cudaMemcpyDeviceToHost, c->stream));
+                CU(cudaStreamSynchronize(c->stream));
+            }
         }
     } else {
         int rc = download_normal(c, out);
@@ -645,12 +685,14 @@ extern "C" int b2_batch_download(b2_ctx* c, b2_batch_result* out) {
     }
     if (out->n_msgs) { const uint32_t now = (uint32_t)(c->covered / out->n_msgs); c->avg_frame = c->avg_frame ? (uint32_t)(((uint64_t)c->avg_frame * 3 + now) / 4) : now; }
     out->kernel_ms = c->last_kernel_ms; out->n_launches = c->last_launches;
+    c->stream_valid = c->stream_armed; c->stream_armed = false;
     return B2_OK;
 }
 
 extern "C" int b2_batch_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs) {
     int rc = b2_batch_upload(c, bytes, nbytes, runs, n_runs);
     if (rc != B2_OK) return rc;
+    c->stream_armed = c->has_streams;
     rc = launch_pipeline(c);
     if (rc != B2_OK) return rc;
     c->executed = true;
@@ -674,6 +716,173 @@ extern "C" int b2_process_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, c
     return b2_batch_collect(c, out);
 }
 
+
+// ---- the stream table (b2_stream_*) -------------------------------------------------------------------------------------------------
+static void stream_free(b2_ctx* c) {
+    for (void*& p : c->d_st_block) { cudaFree(p); p = nullptr; }
+    for (void*& p : c->h_st_mapped) { cudaFreeHost(p); p = nullptr; }
+    cudaFreeHost(c->h_st_cnts); c->h_st_cnts = nullptr; cudaFreeHost(c->h_st_out); c->h_st_out = nullptr;
+    for (cudaEvent_t& e : c->st_ev) if (e) { cudaEventDestroy(e); e = nullptr; }
+    cudaGetLastError();
+}
+static int stream_configure(b2_ctx* c, uint32_t max_streams, uint32_t pending_bytes, uint32_t out_bytes);
+extern "C" int b2_stream_configure(b2_ctx* c, uint32_t max_streams, uint32_t pending_bytes, uint32_t out_bytes) {
+    const int rc = stream_configure(c, max_streams, pending_bytes, out_bytes);
+    if (rc != B2_OK && c && !c->has_streams) stream_free(c);          // nothing of a failed attempt stays behind
+    return rc;
+}
+static int stream_configure(b2_ctx* c, uint32_t max_streams, uint32_t pending_bytes, uint32_t out_bytes) {
+    if (!c || max_streams == 0 || max_streams > (1u << 24) || pending_bytes == 0 || (pending_bytes & 15u)) { set_err("max_streams in 1 .. 2^24, pending_bytes a non-zero multiple of 16"); return B2_E_INVAL; }
+    if (c->has_streams) { set_err("the stream table is already configured"); return B2_E_INVAL; }
+    static_assert(sizeof(StreamEnt) == 64 && sizeof(b2_stream_msg) == 32 && sizeof(b2_stream_event) == 80 && sizeof(b2_stream_desc) == 32 && sizeof(b2_stream_state) == 32, "stream ABI layout");
+    CU(cudaSetDevice(c->opt.device));
+    CU(cudaStreamSynchronize(c->stream));
+    ring_halt(c);
+    StreamPass& S = c->sp;
+    uint32_t cap = 16; while (cap < 2 * max_streams) cap <<= 1;
+    const size_t mm = c->opt.max_msgs;
+    S.cap = cap; S.pending_bytes = pending_bytes; S.out_cap = out_bytes ? out_bytes : c->opt.max_batch_bytes;
+    const size_t dev_bytes[9] = { sizeof(StreamEnt) * (size_t)cap, (size_t)max_streams * pending_bytes, 4 * (16 + 2 * (size_t)cap), 4 * (size_t)cap, 4 * (size_t)cap,
+                                  4 * mm, mm, 8 * mm, 64 * mm };
+    for (int i = 0; i < 9; i++) if (cudaMalloc(&c->d_st_block[i], dev_bytes[i] + (i == 1 ? 16 : 0)) != cudaSuccess) { cudaGetLastError(); set_err("cudaMalloc of the stream table failed"); return B2_E_NOMEM; }
+    S.tab = (StreamEnt*)c->d_st_block[0]; S.pool = (uint8_t*)c->d_st_block[1]; S.cnts = (uint32_t*)c->d_st_block[2]; S.cnt = S.cnts + 16; S.fill = S.cnt + cap;
+    S.base = (uint32_t*)c->d_st_block[3]; S.touched = (uint32_t*)c->d_st_block[4]; S.frame_slot = (uint32_t*)c->d_st_block[5]; S.rst = (uint8_t*)c->d_st_block[6];
+    S.group = (uint32_t*)c->d_st_block[7]; S.tmp_msgs = (b2_stream_msg*)c->d_st_block[8];
+    CU(cudaMemset(S.tab, 0, dev_bytes[0]));
+    // results the kernels write in place: mapped host memory (msgs, events, control frames, per-run RST spans, the frame of close / set_connected)
+    const size_t map_bytes[5] = { sizeof(b2_stream_msg) * mm, sizeof(b2_stream_event) * (size_t)max_streams, (size_t)kStreamCtrlMax * (mm + 2 * (size_t)max_streams), 8 * (size_t)c->opt.max_runs, 256 };
+    void* dev[5];
+    for (int i = 0; i < 5; i++) {
+        if (cudaHostAlloc(&c->h_st_mapped[i], map_bytes[i], cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) { cudaGetLastError(); set_err("cudaHostAlloc of the stream results failed"); return B2_E_NOMEM; }
+        CU(cudaHostGetDevicePointer(&dev[i], c->h_st_mapped[i], 0));
+    }
+    c->h_st_msgs = (b2_stream_msg*)c->h_st_mapped[0]; c->h_st_events = (b2_stream_event*)c->h_st_mapped[1]; c->h_st_ctrl = (uint8_t*)c->h_st_mapped[2];
+    c->h_st_run_ctrl = (uint32_t*)c->h_st_mapped[3]; c->h_st_ctl = (uint8_t*)c->h_st_mapped[4]; c->d_st_ctl = (uint8_t*)dev[4];
+    S.msgs = (b2_stream_msg*)dev[0]; S.events = (b2_stream_event*)dev[1]; S.ctrl = (uint8_t*)dev[2]; S.run_ctrl = (uint32_t*)dev[3];
+    if (cudaMalloc(&c->d_st_block[9], (size_t)S.out_cap + 16) != cudaSuccess) { cudaGetLastError(); set_err("cudaMalloc of the stream out region failed"); return B2_E_NOMEM; }
+    S.out = (uint8_t*)c->d_st_block[9];
+    if (cudaHostAlloc((void**)&c->h_st_cnts, 64, cudaHostAllocDefault) != cudaSuccess || cudaHostAlloc((void**)&c->h_st_out, (size_t)S.out_cap + 16, cudaHostAllocDefault) != cudaSuccess) {
+        cudaGetLastError(); set_err("cudaHostAlloc of the stream out mirror failed"); return B2_E_NOMEM;
+    }
+    memset(c->h_st_cnts, 0, 64);
+    for (cudaEvent_t& e : c->st_ev) CU(cudaEventCreate(&e));
+    c->st_max = max_streams; c->st_open = 0;
+    c->st_keys.assign(cap, 0); c->st_state.assign(cap, 0); c->st_pool.assign(cap, 0);
+    c->st_pool_free.clear(); for (uint32_t i = max_streams; i > 0; i--) c->st_pool_free.push_back(i - 1);
+    c->has_streams = true;
+    return B2_OK;
+}
+
+static uint32_t stream_find(const b2_ctx* c, int64_t id) {
+    const uint32_t cap = c->sp.cap;
+    uint32_t h = stream_hash((long long)id, cap);
+    for (uint32_t k = 0; k < cap; k++, h = (h + 1) & (cap - 1)) {
+        if (c->st_state[h] == 0) return kNone;
+        if (c->st_state[h] == 1 && c->st_keys[h] == (long long)id) return h;
+    }
+    return kNone;
+}
+
+extern "C" int b2_stream_open(b2_ctx* c, const b2_stream_desc* streams, uint32_t n) {
+    if (!c || !c->has_streams || (!streams && n)) { set_err("no stream table (b2_stream_configure) or null argument"); return B2_E_INVAL; }
+    if (c->st_open + (uint64_t)n > c->st_max) { set_err("stream table full"); return B2_E_CAPACITY; }
+    CU(cudaSetDevice(c->opt.device));
+    CU(cudaStreamSynchronize(c->stream));
+    // the slots are picked on the host mirror; the entries travel staged, contiguous slots in one copy each, one synchronisation for all
+    const uint32_t cap = c->sp.cap;
+    std::vector<std::pair<uint32_t, StreamEnt>> staged; staged.reserve(n);
+    int rc = B2_OK;
+    for (uint32_t i = 0; i < n && rc == B2_OK; i++) {
+        const b2_stream_desc& d = streams[i];
+        if (stream_find(c, d.stream_id) != kNone) { set_err("stream id is already open"); rc = B2_E_INVAL; break; }
+        uint32_t h = stream_hash((long long)d.stream_id, cap);
+        while (c->st_state[h] == 1) h = (h + 1) & (cap - 1);
+        StreamEnt e; memset(&e, 0, sizeof e);
+        e.id = d.stream_id; e.remote_id = d.remote_stream_id; e.host_socket = d.host_socket_id;
+        e.flags = kStUsed | ((d.flags & B2_STREAM_CONNECTED) ? kStConnected : 0u) | ((d.flags & B2_STREAM_NEED_FEEDBACK) ? kStNeedFeedback : 0u);
+        e.pool_idx = c->st_pool_free.back(); c->st_pool_free.pop_back();
+        c->st_state[h] = 1; c->st_keys[h] = (long long)d.stream_id; c->st_pool[h] = e.pool_idx; c->st_open++;
+        staged.push_back({ h, e });
+    }
+    std::sort(staged.begin(), staged.end(), [](const std::pair<uint32_t, StreamEnt>& a, const std::pair<uint32_t, StreamEnt>& b) { return a.first < b.first; });
+    std::vector<StreamEnt> flat(staged.size());
+    for (size_t i = 0; i < staged.size(); i++) flat[i] = staged[i].second;
+    for (size_t i = 0; i < staged.size();) {
+        size_t j = i + 1;
+        while (j < staged.size() && staged[j].first == staged[j - 1].first + 1) j++;
+        CU(cudaMemcpyAsync(c->sp.tab + staged[i].first, flat.data() + i, sizeof(StreamEnt) * (j - i), cudaMemcpyHostToDevice, c->stream));
+        i = j;
+    }
+    CU(cudaStreamSynchronize(c->stream));
+    return rc;
+}
+
+static int stream_ctl(b2_ctx* c, int64_t id, int op, int64_t remote, uint32_t flags, void* frame, uint32_t frame_cap, uint32_t* frame_len, uint32_t* slot_out) {
+    if (!c || !c->has_streams || !frame_len || (!frame && frame_cap)) { set_err("no stream table (b2_stream_configure) or null argument"); return B2_E_INVAL; }
+    if (frame_cap < kStreamCtrlMax) { set_err("frame_cap must be at least 64"); return B2_E_INVAL; }
+    const uint32_t slot = stream_find(c, id);
+    if (slot == kNone) { set_err("stream id is not open"); return B2_E_INVAL; }
+    CU(cudaSetDevice(c->opt.device));
+    uint32_t* d_len = reinterpret_cast<uint32_t*>(c->d_st_ctl + 128);
+    k_stream_ctl<<<1, 1, 0, c->stream>>>(c->sp.tab, slot, op, (long long)remote, (flags & B2_STREAM_NEED_FEEDBACK) ? kStNeedFeedback : 0u, c->d_st_ctl, d_len);
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(c->stream));
+    *frame_len = *reinterpret_cast<const uint32_t*>(c->h_st_ctl + 128);
+    memcpy(frame, c->h_st_ctl, *frame_len);
+    *slot_out = slot;
+    return B2_OK;
+}
+extern "C" int b2_stream_set_connected(b2_ctx* c, int64_t stream_id, int64_t remote_stream_id, uint32_t flags, void* frame, uint32_t frame_cap, uint32_t* frame_len) {
+    uint32_t slot;
+    return stream_ctl(c, stream_id, 1, remote_stream_id, flags, frame, frame_cap, frame_len, &slot);
+}
+extern "C" int b2_stream_close(b2_ctx* c, int64_t stream_id, void* frame, uint32_t frame_cap, uint32_t* frame_len) {
+    uint32_t slot;
+    int rc = stream_ctl(c, stream_id, 0, 0, 0, frame, frame_cap, frame_len, &slot);
+    if (rc != B2_OK) return rc;
+    c->st_pool_free.push_back(c->st_pool[slot]); c->st_state[slot] = 2; c->st_open--;      // (a tombstone: probes for other ids walk over it)
+    return B2_OK;
+}
+static int stream_read(b2_ctx* c, int64_t id, StreamEnt* e, uint32_t* slot) {
+    if (!c || !c->has_streams) { set_err("no stream table (b2_stream_configure)"); return B2_E_INVAL; }
+    *slot = stream_find(c, id);
+    if (*slot == kNone) { set_err("stream id is not open"); return B2_E_INVAL; }
+    CU(cudaSetDevice(c->opt.device));
+    CU(cudaStreamSynchronize(c->stream));
+    CU(cudaMemcpy(e, c->sp.tab + *slot, sizeof *e, cudaMemcpyDeviceToHost));
+    return B2_OK;
+}
+extern "C" int b2_stream_query(b2_ctx* c, int64_t stream_id, b2_stream_state* out) {
+    if (!out) { set_err("null argument"); return B2_E_INVAL; }
+    StreamEnt e; uint32_t slot;
+    int rc = stream_read(c, stream_id, &e, &slot); if (rc != B2_OK) return rc;
+    out->local_consumed = e.local_consumed; out->remote_consumed = e.remote_consumed; out->pending_bytes = e.pending_len; out->error_code = e.error; out->reserved = 0;
+    out->flags = ((e.flags & kStConnected) ? B2_STREAM_CONNECTED : 0u) | ((e.flags & kStNeedFeedback) ? B2_STREAM_NEED_FEEDBACK : 0u) |
+                 ((e.flags & kStClosed) ? B2_STREAM_CLOSED : 0u) | ((e.flags & kStHandedOver) ? B2_STREAM_HANDED_OVER : 0u);
+    return B2_OK;
+}
+extern "C" int b2_stream_take_pending(b2_ctx* c, int64_t stream_id, void* out, uint32_t cap, uint32_t* len) {
+    if (!len || (!out && cap)) { set_err("null argument"); return B2_E_INVAL; }
+    StreamEnt e; uint32_t slot;
+    int rc = stream_read(c, stream_id, &e, &slot); if (rc != B2_OK) return rc;
+    if (e.pending_len > cap) { set_err("the pending bytes do not fit"); return B2_E_CAPACITY; }
+    if (e.pending_len) CU(cudaMemcpy(out, c->sp.pool + (size_t)e.pool_idx * c->sp.pending_bytes, e.pending_len, cudaMemcpyDeviceToHost));
+    *len = e.pending_len;
+    e.pending_len = 0; e.pending_frames = 0;
+    CU(cudaMemcpy(c->sp.tab + slot, &e, sizeof e, cudaMemcpyHostToDevice));
+    return B2_OK;
+}
+extern "C" int b2_stream_results(b2_ctx* c, b2_stream_batch_result* out) {
+    if (!c || !out || !c->has_streams) { set_err("no stream table (b2_stream_configure) or null argument"); return B2_E_INVAL; }
+    if (!c->stream_valid) { set_err("no collected batch of b2_process_batch / b2_batch_collect"); return B2_E_INVAL; }
+    memset(out, 0, sizeof *out);
+    if (!c->stream_ran) return B2_OK;                      // (a batch without runs)
+    const uint32_t* n = c->h_st_cnts;
+    out->msgs = c->h_st_msgs; out->n_msgs = n[0]; out->events = c->h_st_events; out->n_events = n[1];
+    out->out = c->h_st_out; out->out_bytes = n[2]; out->ctrl = c->h_st_ctrl; out->ctrl_bytes = n[3];
+    out->run_ctrl = c->h_st_run_ctrl; out->n_runs = c->n_runs;
+    return B2_OK;
+}
 
 // ---- the persistent latency path: submit ring + resident kernel (k_ring) ---------------------------------------------------------
 static void ring_halt(b2_ctx* c) {
@@ -723,6 +932,7 @@ extern "C" int b2_ring_stop(b2_ctx* c) { if (!c) return B2_E_INVAL; cudaSetDevic
 
 extern "C" int b2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs, uint32_t* ticket) {
     if (!c || !bytes || !runs || !ticket || n_runs == 0) { set_err("null argument"); return B2_E_INVAL; }
+    if (c->has_streams) { set_err("the ring path does not run the stream pass: use b2_batch_submit on a context with a stream table"); return B2_E_INVAL; }
     if (nbytes > kSmallBytes || n_runs > kSmallRuns) { set_err("b2_ring_submit serves batches up to 128 KiB / 512 runs: use b2_batch_submit"); return B2_E_CAPACITY; }
     if (!c->ring_slots) { int rc = b2_ring_start(c); if (rc != B2_OK) return rc; }
     const uint32_t t = c->ring_next, si = t % kRingSlots;
@@ -832,7 +1042,11 @@ extern "C" int b2_stage_times(b2_ctx* c, const char** names, float* ms, int cap)
         cudaEventElapsedTime(&t, c->ev[i], c->ev[i + 1]);
         ms[i] = t;
     }
-    return c->n_stages;
+    int total = c->n_stages;
+    if (c->stream_valid && c->stream_ran) {          // the stream pass of the last collected batch, kernel by kernel
+        for (int i = 0; i < 5; i++, total++) if (total < cap) { names[total] = kStreamStages[i]; float t = 0.f; cudaEventElapsedTime(&t, c->st_ev[i], c->st_ev[i + 1]); ms[total] = t; }
+    }
+    return total;
 }
 
 // what the last upload / launch decided: [0] tile bytes [1] tiles [2] frame offsets kept per tile [3] 1 = the fused kernel served it

@@ -2851,5 +2851,292 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_ring(RingDev R, BatchPtrs 
     if (tid == 0) *R.next_ticket = ticket;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------------
+// streaming_rpc: the receiving side of a Stream on the device (b2_stream_*).  What brpc does with a STRM frame after the meta parse:
+//   ParseStreamingMessage (policy/streaming_rpc_protocol.cpp:99-129): Socket::Address(stream_id); unknown id -> SendStreamRst (:139-149)
+//     unless the frame is a FEEDBACK or carries no source_stream_id
+//   Stream::OnReceived (stream.cpp:499-543): DATA appended to _pending_buf until a frame without has_continuation completes the message;
+//     FEEDBACK -> SetRemoteConsumed (:362-401); RST / CLOSE -> Close (:710-732)
+//   Stream::Consume (:582-651) + SendFeedback (:653-662): _local_consumed += bytes, one FEEDBACK frame with the cumulative count;
+//     BeforeRecycle (:129-146): the CLOSE frame of a connected stream
+// Streams are independent of each other and sequential inside: one warp walks one stream's frames of the batch in msgs[] order.
+//   k_stream_route  thread/descriptor  table probe, frames per stream, list of the streams this batch touches, RST marks for unknown ids
+//   k_stream_alloc  thread/stream      a slice of the group array for each touched stream
+//   k_stream_group  thread/descriptor  every stream's frame indices into its slice
+//   k_stream_run    warp/stream        sorts the slice, walks the state machine, copies multi-frame messages, writes FEEDBACK / CLOSE
+//   k_stream_rst    warp/run           the RST frames of a run, in message order
+// The table is written by the host between batch calls (open / close) and by the one warp that owns the stream inside a batch.
+constexpr uint32_t kStUsed = 1, kStConnected = 2, kStNeedFeedback = 4, kStClosed = 8, kStHandedOver = 16, kStTomb = 32;
+constexpr int32_t kFrameRst = 1, kFrameClose = 2, kFrameData = 3, kFrameFeedback = 4;     // brpc::FrameType (streaming_rpc_meta.proto:32-38)
+constexpr uint32_t kStreamCtrlMax = 64;     // bytes of one control frame: 12 + stream_id, source_stream_id, frame_type, feedback{consumed_size} <= 49
+struct __align__(16) StreamEnt {            // 64 bytes
+    long long id, remote_id;
+    unsigned long long host_socket, local_consumed, remote_consumed;
+    uint32_t flags; int32_t error;
+    uint32_t pending_len, pending_frames;   // the partial message in this stream's pool slot
+    uint32_t pool_idx;                      // its slot of the pending pool (handed out by the host)
+    uint32_t pad;
+};
+struct StreamPass {
+    StreamEnt* tab; uint32_t cap;           // open addressing on the id, cap a power of two; the host picks the slots (b2_stream_open)
+    uint8_t* pool; uint32_t pending_bytes;  // [max_streams][pending_bytes] partial messages that wait for their next frame
+    uint32_t* cnts;                         // [16] [0] completed messages [1] touched streams [2] out bytes [3] ctrl bytes [4] group words
+    uint32_t* cnt;                          // [cap] frames of the stream in this batch
+    uint32_t* fill;                         // [cap] k_stream_group's cursor
+    uint32_t* base;                         // [cap] the stream's slice of group / tmp_msgs
+    uint32_t* touched;                      // [cap] table slots with frames in this batch
+    uint32_t* frame_slot;                   // [max_msgs] table slot of every descriptor (kNone: not a frame of an open stream)
+    uint8_t* rst;                           // [max_msgs] 1 = answer this frame with RST
+    uint32_t* group;                        // [2 * max_msgs] slices padded to a power of two (the bitonic sort)
+    b2_stream_msg* tmp_msgs;                // [2 * max_msgs] a stream's messages before they are compacted
+    uint8_t* out; uint32_t out_cap;         // reassembled multi-frame messages (HBM)
+    b2_stream_msg* msgs; b2_stream_event* events; uint8_t* ctrl; uint32_t* run_ctrl;   // results, mapped host memory
+};
+
+B2_HD uint32_t stream_hash(long long id, uint32_t cap) {
+    unsigned long long x = (unsigned long long)id * 0x9e3779b97f4a7c15ull;
+    return (uint32_t)(x >> 32) & (cap - 1);
+}
+__device__ __forceinline__ uint32_t stream_probe(const StreamPass& S, long long id) {
+    uint32_t h = stream_hash(id, S.cap);
+    for (uint32_t k = 0; k < S.cap; k++, h = (h + 1) & (S.cap - 1)) {
+        const uint32_t f = S.tab[h].flags;
+        if (f == 0) return kNone;
+        if ((f & kStUsed) && S.tab[h].id == id) return h;
+    }
+    return kNone;
+}
+// PackStreamMessage (policy/streaming_rpc_protocol.cpp:42-58) of a frame without payload; returns its length (<= kStreamCtrlMax)
+__device__ __forceinline__ uint32_t stream_ctrl_frame(uint8_t* o, long long stream_id, bool has_source, long long source, int32_t type, bool has_fb, unsigned long long consumed) {
+    uint8_t* m = o + 12;
+    *m++ = 0x08; m = put_varint(m, (uint64_t)stream_id);
+    if (has_source) { *m++ = 0x10; m = put_varint(m, (uint64_t)source); }
+    *m++ = 0x18; *m++ = (uint8_t)type;
+    if (has_fb) { *m++ = 0x2a; *m++ = (uint8_t)(1 + varint_len(consumed)); *m++ = 0x08; m = put_varint(m, consumed); }
+    const uint32_t ml = (uint32_t)(m - o) - 12;
+    o[0] = 'S'; o[1] = 'T'; o[2] = 'R'; o[3] = 'M'; put_be32(o + 4, ml); put_be32(o + 8, ml);
+    return 12 + ml;
+}
+__device__ __forceinline__ bool stream_wants_rst(const b2_msg_desc& d) {
+    return (d.has_bits & B2_SHAS_SOURCE_STREAM_ID) && !((d.has_bits & B2_SHAS_FRAME_TYPE) && d.compress_type == kFrameFeedback);
+}
+// (the pool and the out region are written in this pass: plain loads, not the read-only path of warp_copy)
+__device__ __forceinline__ void stream_copy(uint8_t* dst, const uint8_t* src, uint32_t n, uint32_t lane) {
+    if (((((uintptr_t)dst) | ((uintptr_t)src)) & 15u) == 0) {
+        const uint32_t nv = n >> 4;
+        const uint4* s4 = reinterpret_cast<const uint4*>(src); uint4* d4 = reinterpret_cast<uint4*>(dst);
+        for (uint32_t i = lane; i < nv; i += 32) d4[i] = s4[i];
+        for (uint32_t i = (nv << 4) + lane; i < n; i += 32) dst[i] = src[i];
+    } else for (uint32_t i = lane; i < n; i += 32) dst[i] = src[i];
+}
+
+__global__ void __launch_bounds__(256) k_stream_route(BatchPtrs B, StreamPass S) {
+    if (B.totals[2] & 3u) return;                     // the batch is about to be redone (or to fail): the table must not see it twice
+    const uint32_t n = B.totals[0];
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const b2_msg_desc& d = B.msgs[i];
+        uint32_t slot = kNone; uint8_t rst = 0;
+        if (d.status == B2_MSG_STREAM_FRAME) {
+            const uint32_t s = stream_probe(S, d.correlation_id);
+            const uint32_t f = s == kNone ? (uint32_t)kStClosed : S.tab[s].flags;
+            if (f & kStClosed) rst = stream_wants_rst(d) ? 1 : 0;
+            else if (!(f & kStHandedOver)) {
+                slot = s;
+                if (atomicAdd(&S.cnt[s], 1u) == 0) S.touched[atomicAdd(&S.cnts[1], 1u)] = s;
+            }
+        }
+        S.frame_slot[i] = slot; S.rst[i] = rst;
+    }
+}
+__global__ void __launch_bounds__(256) k_stream_alloc(BatchPtrs B, StreamPass S) {
+    if (B.totals[2] & 3u) return;
+    const uint32_t n = S.cnts[1];
+    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
+        const uint32_t s = S.touched[t], c = S.cnt[s];
+        uint32_t p = 1; while (p < c) p <<= 1;
+        S.base[s] = atomicAdd(&S.cnts[4], p);
+    }
+}
+__global__ void __launch_bounds__(256) k_stream_group(BatchPtrs B, StreamPass S) {
+    if (B.totals[2] & 3u) return;
+    const uint32_t n = B.totals[0];
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const uint32_t s = S.frame_slot[i];
+        if (s != kNone) S.group[S.base[s] + atomicAdd(&S.fill[s], 1u)] = i;
+    }
+}
+
+__global__ void __launch_bounds__(128) k_stream_run(BatchPtrs B, StreamPass S) {
+    if (B.totals[2] & 3u) return;
+    const uint32_t lane = threadIdx.x & 31, n_warps = (gridDim.x * blockDim.x) >> 5, n_touched = S.cnts[1];
+    for (uint32_t t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; t < n_touched; t += n_warps) {
+        const uint32_t s = S.touched[t], n = S.cnt[s];
+        uint32_t* g = S.group + S.base[s];
+        b2_stream_msg* tm = S.tmp_msgs + S.base[s];
+        {   // the slice in msgs[] order: bitonic sort over the padded slice
+            uint32_t P = 1; while (P < n) P <<= 1;
+            for (uint32_t i = n + lane; i < P; i += 32) g[i] = kNone;
+            __syncwarp();
+            for (uint32_t k = 2; k <= P; k <<= 1)
+                for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+                    for (uint32_t i = lane; i < P; i += 32) {
+                        const uint32_t l = i ^ j;
+                        if (l > i) {
+                            const uint32_t a = g[i], b = g[l];
+                            if (((i & k) == 0) ? a > b : a < b) { g[i] = b; g[l] = a; }
+                        }
+                    }
+                    __syncwarp();
+                }
+        }
+        StreamEnt e = S.tab[s];
+        __syncwarp();                                        // every lane holds the entry before lane 0 may publish the walk's result
+        uint8_t* pend = S.pool + (size_t)e.pool_idx * S.pending_bytes;
+        uint32_t nm = 0, ev = 0, handover = kNone;
+        unsigned long long consumed = 0;
+        uint32_t k = 0;
+        while (k < n && !(ev & (B2_STREAM_EV_CLOSED_BY_RST | B2_STREAM_EV_CLOSED_BY_CLOSE | B2_STREAM_EV_HANDED_OVER))) {
+            const b2_msg_desc& d = B.msgs[g[k]];
+            const int32_t ft = (d.has_bits & B2_SHAS_FRAME_TYPE) ? d.compress_type : 0;
+            if (ft == kFrameFeedback) {
+                const unsigned long long c = ((unsigned long long)(uint32_t)d.checksum_type << 32) | (uint32_t)d.attachment_size;
+                if (c > e.remote_consumed) { e.remote_consumed = c; ev |= B2_STREAM_EV_REMOTE_CONSUMED_MOVED; }
+                k++;
+            } else if (ft == kFrameRst || ft == kFrameClose) {
+                ev |= ft == kFrameRst ? B2_STREAM_EV_CLOSED_BY_RST : B2_STREAM_EV_CLOSED_BY_CLOSE;
+                e.error = ft == kFrameRst ? 104 /*ECONNRESET*/ : 0;
+                e.pending_len = 0; e.pending_frames = 0;
+                k++;
+            } else if (ft == kFrameData) {
+                // look ahead for the frame that completes the message: [k, end] then holds every part that is in this batch
+                unsigned long long total = e.pending_len; uint32_t nfr = e.pending_frames, end = kNone, j = k;
+                for (; j < n; j++) {
+                    const b2_msg_desc& dj = B.msgs[g[j]];
+                    const int32_t fj = (dj.has_bits & B2_SHAS_FRAME_TYPE) ? dj.compress_type : 0;
+                    if (fj == kFrameRst || fj == kFrameClose) break;
+                    if (fj == kFrameFeedback) {
+                        const unsigned long long c = ((unsigned long long)(uint32_t)dj.checksum_type << 32) | (uint32_t)dj.attachment_size;
+                        if (c > e.remote_consumed) { e.remote_consumed = c; ev |= B2_STREAM_EV_REMOTE_CONSUMED_MOVED; }
+                    }
+                    if (fj != kFrameData) continue;
+                    total += dj.body_size - dj.meta_size; nfr++;
+                    if (!(dj.has_bits & B2_SVAL_HAS_CONTINUATION)) { end = j; break; }
+                }
+                if (end != kNone) {
+                    b2_stream_msg m; m.stream_id = e.id; m.first_frame = g[k]; m.n_frames = nfr; m.len = (uint32_t)total; m.flags = 0; m.reserved = 0;
+                    if (nfr == 1) { m.off = d.frame_off + 12 + d.meta_size; m.flags = B2_STREAM_MSG_IN_INPUT; }
+                    else {
+                        const uint32_t need = ((uint32_t)total + 15u) & ~15u;
+                        uint32_t off = 0;
+                        if (lane == 0) {
+                            off = total > S.out_cap ? kNone : atomicAdd(&S.cnts[2], need);
+                            if (off != kNone && (unsigned long long)off + need > S.out_cap) { atomicAdd(&S.cnts[2], 0u - need); off = kNone; }
+                        }
+                        off = __shfl_sync(0xffffffffu, off, 0);
+                        if (off == kNone) { ev |= B2_STREAM_EV_HANDED_OVER; handover = g[k]; break; }
+                        uint8_t* o = S.out + off;
+                        stream_copy(o, pend, e.pending_len, lane); o += e.pending_len;
+                        for (uint32_t q = k; q <= end; q++) {
+                            const b2_msg_desc& dq = B.msgs[g[q]];
+                            if (!((dq.has_bits & B2_SHAS_FRAME_TYPE) && dq.compress_type == kFrameData)) continue;
+                            const uint32_t len = dq.body_size - dq.meta_size;
+                            stream_copy(o, B.bytes + dq.frame_off + 12 + dq.meta_size, len, lane); o += len;
+                        }
+                        __syncwarp();                        // the pool slot is read out before a later partial message may be written into it
+                        m.off = off; e.pending_len = 0; e.pending_frames = 0;
+                    }
+                    if (lane == 0) tm[nm] = m;
+                    nm++; consumed += total; k = end + 1;
+                } else if (j < n) {
+                    k = j;                                   // RST / CLOSE before the message completed: its parts are dropped with the stream
+                } else {
+                    // the batch ends inside the message: its parts wait in the pool
+                    if (total > S.pending_bytes) { ev |= B2_STREAM_EV_HANDED_OVER; handover = g[k]; break; }
+                    for (uint32_t q = k; q < n; q++) {
+                        const b2_msg_desc& dq = B.msgs[g[q]];
+                        if (!((dq.has_bits & B2_SHAS_FRAME_TYPE) && dq.compress_type == kFrameData)) continue;
+                        const uint32_t len = dq.body_size - dq.meta_size;
+                        stream_copy(pend + e.pending_len, B.bytes + dq.frame_off + 12 + dq.meta_size, len, lane); e.pending_len += len;
+                    }
+                    __syncwarp();
+                    e.pending_frames = nfr; k = n;
+                }
+            } else k++;                                      // FRAME_TYPE_UNKNOWN, absent, or an enum value proto2 does not know: ignored (stream.cpp:538-540)
+        }
+        const bool closed = ev & (B2_STREAM_EV_CLOSED_BY_RST | B2_STREAM_EV_CLOSED_BY_CLOSE);
+        // frames behind the close meet an id that no longer resolves
+        if (closed) for (uint32_t q = k + lane; q < n; q += 32) if (stream_wants_rst(B.msgs[g[q]])) S.rst[g[q]] = 1;
+        // one Consume for the batch, then the control frames: FEEDBACK before CLOSE
+        e.local_consumed += consumed;
+        uint32_t first = 0;
+        if (lane == 0) {
+            b2_stream_event E;
+            E.stream_id = e.id; E.host_socket_id = e.host_socket; E.local_consumed = e.local_consumed; E.remote_consumed = e.remote_consumed;
+            E.n_msgs = nm; E.consumed_bytes = (uint32_t)consumed; E.flags = ev; E.handover_msg = handover; E.pending_bytes = e.pending_len;
+            E.fb_off = E.fb_len = E.close_off = E.close_len = 0; E.reserved[0] = E.reserved[1] = 0;
+            uint8_t fr[2 * kStreamCtrlMax]; uint32_t fl = 0, cl = 0;
+            if (consumed > 0 && (e.flags & kStConnected) && (e.flags & kStNeedFeedback)) fl = stream_ctrl_frame(fr, e.remote_id, true, e.id, kFrameFeedback, true, e.local_consumed);
+            if (closed && (e.flags & kStConnected)) cl = stream_ctrl_frame(fr + fl, e.remote_id, true, e.id, kFrameClose, false, 0);
+            if (fl + cl) {
+                const uint32_t co = atomicAdd(&S.cnts[3], fl + cl);
+                for (uint32_t q = 0; q < fl + cl; q++) S.ctrl[co + q] = fr[q];
+                E.fb_off = co; E.fb_len = fl; E.close_off = co + fl; E.close_len = cl;
+            }
+            first = nm ? atomicAdd(&S.cnts[0], nm) : 0;
+            E.first_msg = first;
+            S.events[t] = E;
+            if (closed) e.flags |= kStClosed;
+            if (ev & B2_STREAM_EV_HANDED_OVER) e.flags |= kStHandedOver;
+            S.tab[s] = e;
+        }
+        first = __shfl_sync(0xffffffffu, first, 0);
+        __syncwarp();
+        for (uint32_t q = lane; q < nm; q += 32) S.msgs[first + q] = tm[q];
+    }
+}
+
+__global__ void __launch_bounds__(128) k_stream_rst(BatchPtrs B, StreamPass S) {
+    if (B.totals[2] & 3u) return;
+    const uint32_t lane = threadIdx.x & 31, n_warps = (gridDim.x * blockDim.x) >> 5;
+    for (uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < B.n_runs; r += n_warps) {
+        const uint32_t first = B.run_status[r].first_msg, n = B.run_status[r].n_msgs;
+        uint32_t total = 0;
+        for (int pass = 0; pass < 2; pass++) {               // sizes, then bytes
+            uint32_t base = 0, run = 0;
+            if (pass == 1) {
+                if (lane == 0 && total) base = atomicAdd(&S.cnts[3], total);
+                base = __shfl_sync(0xffffffffu, base, 0);
+                if (lane == 0) { S.run_ctrl[2 * r] = total ? base : 0; S.run_ctrl[2 * r + 1] = total; }
+                if (!total) break;
+            }
+            for (uint32_t i0 = 0; i0 < n; i0 += 32) {
+                const uint32_t i = first + i0 + lane;
+                const bool on = i0 + lane < n && S.rst[i];
+                const long long src = on ? B.msgs[i].log_id : 0;
+                const uint32_t len = on ? 12 + 1 + varint_len((uint64_t)src) + 2 : 0;
+                uint32_t inc = len;
+                for (uint32_t o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += v; }
+                if (pass == 1 && on) stream_ctrl_frame(S.ctrl + base + run + inc - len, src, false, 0, kFrameRst, false, 0);
+                run += __shfl_sync(0xffffffffu, inc, 31);
+            }
+            total = run;
+        }
+    }
+}
+
+// b2_stream_close / b2_stream_set_connected: one stream between batch calls.  frame[0..] = the frame to write, *frame_len its length (0 = none).
+__global__ void k_stream_ctl(StreamEnt* tab, uint32_t slot, int op, long long remote_id, uint32_t flags, uint8_t* frame, uint32_t* frame_len) {
+    StreamEnt& e = tab[slot];
+    uint32_t len = 0;
+    if (op == 0) {            // local close (BeforeRecycle, stream.cpp:129-146): a connected stream that the peer has not closed says CLOSE
+        if ((e.flags & kStConnected) && !(e.flags & kStClosed)) len = stream_ctrl_frame(frame, e.remote_id, true, e.id, kFrameClose, false, 0);
+        e.flags = kStTomb;
+    } else if (!(e.flags & (kStClosed | kStConnected))) {      // SetConnected with the peer's settings (stream.cpp:270-307)
+        e.remote_id = remote_id; e.flags |= kStConnected | (flags & kStNeedFeedback);
+        if ((e.flags & kStNeedFeedback) && e.local_consumed > 0) len = stream_ctrl_frame(frame, e.remote_id, true, e.id, kFrameFeedback, true, e.local_consumed);
+    }
+    *frame_len = len;
+}
+
 #endif  // __CUDACC__
 }  // namespace b2

@@ -764,6 +764,100 @@ int  b2_h2_serve_batch(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2
                        b2_h2_run_status* rs, b2_h2_msg* msgs, uint32_t msg_cap, uint32_t* n_msgs, void* out, uint32_t out_cap,
                        void* replies, uint32_t replies_cap, b2_h2_reply_span* spans);
 
+/* ---- streaming_rpc, the receiving side of a Stream on the device ------------------------------------------------------------------
+ * Without a stream table a STRM frame ends as a B2_MSG_STREAM_FRAME descriptor and the host rebuilds brpc's Stream from the list.  With
+ * one (b2_stream_configure) every batch call also runs, behind the stage that writes msgs[] and inside the same synchronisation, what
+ * brpc does per frame after the meta parse:
+ *   ParseStreamingMessage (src/brpc/policy/streaming_rpc_protocol.cpp:99-129): the id is looked up; a frame for an id that is not open
+ *     (never opened, closed in an earlier batch or earlier in this one) is answered with SendStreamRst (:139-149) when it carries a
+ *     source_stream_id and is not a FEEDBACK, and does nothing else;
+ *   Stream::OnReceived (src/brpc/stream.cpp:499-543): DATA payloads are appended until a frame whose has_continuation VALUE is false
+ *     completes the message; FEEDBACK -> remote_consumed = max(remote_consumed, consumed_size) (SetRemoteConsumed :362-401, with
+ *     -socket_max_streams_unconsumed_bytes at its default 0); RST -> closed with ECONNRESET, CLOSE -> closed with 0 (Close :710-732),
+ *     the partial message is dropped; any other frame_type is ignored;
+ *   Stream::Consume (:582-651) + SendFeedback (:653-662), ONCE per stream per batch: local_consumed += the bytes of the messages the
+ *     batch completed, and when that is > 0 on a CONNECTED stream whose peer set need_feedback one FEEDBACK frame with the cumulative
+ *     count; BeforeRecycle (:129-146): the CLOSE frame of a connected stream that was closed.
+ * Decisions brpc leaves to bthread scheduling: one Consume per stream per batch; a stream closed in a batch still delivers the messages
+ * completed before the close and writes FEEDBACK before CLOSE; frames of one stream are ordered by their msgs[] index, whichever
+ * socket they came in on.  The per-frame b2_msg_desc records stay exactly as without a table (B2_STREAM_SNAPPY_UNCOMPRESS included).
+ * Capacity (the reference has none): a partial message that outgrows pending_bytes, or a multi-frame message that no longer fits the
+ * out region of the batch, puts the stream into HANDED_OVER — the event names the first descriptor the device did not absorb
+ * (handover_msg), the parts gathered in earlier batches are fetched once with b2_stream_take_pending, and from then on the stream's
+ * frames are described per frame only (no routing, no RST) until b2_stream_close.
+ * Not modelled: _parse_rpc_response (open a client stream after the host took the RPC response), idle timers, messages_in_batch.
+ * The ring path does not run the pass: b2_ring_submit fails with B2_E_INVAL on a context that has a table.  The measurement entry
+ * points (b2_batch_execute, b2_batch_execute_many, b2_batch_launch) do not run it either: they replay one batch, and fail with
+ * B2_E_INVAL between b2_batch_submit and b2_batch_collect on a context with a table.  When one batch completes more multi-frame bytes
+ * than the out region holds, WHICH of the competing streams is handed over is unspecified (room is handed out as the warps ask). */
+#define B2_STREAM_CONNECTED      1u   /* b2_stream_desc.flags: Stream::_connected, remote_stream_id is valid */
+#define B2_STREAM_NEED_FEEDBACK  2u   /* _remote_settings.need_feedback */
+#define B2_STREAM_CLOSED         4u   /* b2_stream_state.flags */
+#define B2_STREAM_HANDED_OVER    8u
+typedef struct b2_stream_desc {
+    int64_t  stream_id;               /* what peers put in StreamFrameMeta.stream_id */
+    int64_t  remote_stream_id;        /* _remote_settings.stream_id (CONNECTED) */
+    uint64_t host_socket_id;          /* opaque; echoed in the events: where FEEDBACK / CLOSE go */
+    uint32_t flags, reserved;
+} b2_stream_desc;                     /* 32 bytes */
+typedef struct b2_stream_state {
+    uint64_t local_consumed, remote_consumed;
+    uint32_t pending_bytes;           /* bytes of the partial message that waits on the device */
+    uint32_t flags;                   /* B2_STREAM_* */
+    int32_t  error_code;              /* of the close: ECONNRESET (104) after RST, 0 after CLOSE */
+    uint32_t reserved;
+} b2_stream_state;                    /* 32 bytes */
+#define B2_STREAM_MSG_IN_INPUT 1u     /* off indexes the request bytes (one frame carried the message: zero copy), else the out region */
+typedef struct b2_stream_msg {
+    int64_t  stream_id;
+    uint32_t first_frame;             /* b2_msg_desc index of the message's first frame in THIS batch */
+    uint32_t n_frames;                /* DATA frames of the message, earlier batches included */
+    uint32_t off, len;
+    uint32_t flags, reserved;
+} b2_stream_msg;                      /* 32 bytes */
+#define B2_STREAM_EV_REMOTE_CONSUMED_MOVED 1u
+#define B2_STREAM_EV_CLOSED_BY_RST         2u   /* error ECONNRESET */
+#define B2_STREAM_EV_CLOSED_BY_CLOSE       4u   /* error 0 */
+#define B2_STREAM_EV_HANDED_OVER           8u
+typedef struct b2_stream_event {
+    int64_t  stream_id;
+    uint64_t host_socket_id;
+    uint64_t local_consumed, remote_consumed;   /* after the batch */
+    uint32_t n_msgs, first_msg;       /* the stream's completed messages: b2_stream_batch_result.msgs[first_msg, +n_msgs), arrival order */
+    uint32_t consumed_bytes;          /* of this batch */
+    uint32_t flags;                   /* B2_STREAM_EV_* */
+    uint32_t fb_off, fb_len;          /* FEEDBACK frame inside ctrl (len 0 = none) */
+    uint32_t close_off, close_len;    /* CLOSE frame inside ctrl, to be written after the FEEDBACK */
+    uint32_t handover_msg;            /* HANDED_OVER: first b2_msg_desc of the stream the device did not absorb */
+    uint32_t pending_bytes;           /* bytes of the partial message kept on the device after the batch */
+    uint32_t reserved[2];
+} b2_stream_event;                    /* 80 bytes */
+/* Pointers into ctx-owned pinned memory, valid after b2_process_batch / b2_batch_collect until the next batch call on the context.
+ * msgs are grouped by stream; the order of streams (and of the spans inside out / ctrl) is not specified. */
+typedef struct b2_stream_batch_result {
+    const b2_stream_msg*   msgs;    uint32_t n_msgs;
+    const b2_stream_event* events;  uint32_t n_events;     /* one per stream the batch touched */
+    const uint8_t*         out;     uint32_t out_bytes;    /* reassembled multi-frame messages */
+    const uint8_t*         ctrl;    uint32_t ctrl_bytes;   /* wire-ready frames to write */
+    const uint32_t*        run_ctrl; uint32_t n_runs;      /* [2 * n_runs] {off, len} inside ctrl: run i's RST frames, in message order,
+                                                              to be written to the socket the run came from */
+} b2_stream_batch_result;
+/* Before the first batch call.  max_streams open streams; pending_bytes (multiple of 16) per stream for a message that spans batches;
+ * out_bytes for the multi-frame messages one batch completes (0 = the context's max_batch_bytes). */
+int  b2_stream_configure(b2_ctx* ctx, uint32_t max_streams, uint32_t pending_bytes, uint32_t out_bytes);
+/* StreamAccept / StreamCreate: the ids start resolving.  Between batch calls. */
+int  b2_stream_open(b2_ctx* ctx, const b2_stream_desc* streams, uint32_t n);
+/* Stream::SetConnected(remote_settings) of a client-side stream whose settings arrive with the RPC response (stream.cpp:270-307):
+ * flags = B2_STREAM_NEED_FEEDBACK or 0.  frame / frame_len: its first FEEDBACK when bytes were consumed before (frame_cap >= 64). */
+int  b2_stream_set_connected(b2_ctx* ctx, int64_t stream_id, int64_t remote_stream_id, uint32_t flags, void* frame, uint32_t frame_cap, uint32_t* frame_len);
+/* Local close: the id stops resolving and its table slot is free again.  frame / frame_len: the CLOSE frame when the stream was
+ * connected and the peer had not closed it (frame_cap >= 64). */
+int  b2_stream_close(b2_ctx* ctx, int64_t stream_id, void* frame, uint32_t frame_cap, uint32_t* frame_len);
+int  b2_stream_query(b2_ctx* ctx, int64_t stream_id, b2_stream_state* out);
+/* The partial message of a stream (a HANDED_OVER one hands it out this way), at most cap bytes; it is gone from the device afterwards. */
+int  b2_stream_take_pending(b2_ctx* ctx, int64_t stream_id, void* out, uint32_t cap, uint32_t* len);
+int  b2_stream_results(b2_ctx* ctx, b2_stream_batch_result* out);
+
 /* ---- counters (bvar::Adder-like, SURVEY §8e): per-GPU totals accumulated by
  * the kernels: [0] in_bytes [1] in_msgs [2] out_bytes [3] out_msgs [4] errors
  * [5] batches [6..7] reserved.  The cross-GPU reduce is an NCCL all-reduce on
