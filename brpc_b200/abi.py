@@ -51,7 +51,7 @@ MSG_DT = np.dtype([("run_idx", "<u4"), ("frame_off", "<u4"), ("body_size", "<u4"
                    ("method_idx", "<i2"), ("status", "<u2"), ("resp_off", "<u4"), ("resp_len", "<u4")])
 assert RUN_DT.itemsize == 24 and RUN_STATUS_DT.itemsize == 32 and MSG_DT.itemsize == 64
 # the stream table (b2_stream_*)
-STREAM_DESC_DT = np.dtype([("stream_id", "<i8"), ("remote_stream_id", "<i8"), ("host_socket_id", "<u8"), ("flags", "<u4"), ("reserved", "<u4")])
+STREAM_DESC_DT = np.dtype([("stream_id", "<i8"), ("remote_stream_id", "<i8"), ("host_socket_id", "<u8"), ("flags", "<u4"), ("max_buf_size", "<u4")])
 STREAM_MSG_DT = np.dtype([("stream_id", "<i8"), ("first_frame", "<u4"), ("n_frames", "<u4"), ("off", "<u4"), ("len", "<u4"), ("flags", "<u4"), ("reserved", "<u4")])
 STREAM_EVENT_DT = np.dtype([("stream_id", "<i8"), ("host_socket_id", "<u8"), ("local_consumed", "<u8"), ("remote_consumed", "<u8"), ("n_msgs", "<u4"),
                             ("first_msg", "<u4"), ("consumed_bytes", "<u4"), ("flags", "<u4"), ("fb_off", "<u4"), ("fb_len", "<u4"), ("close_off", "<u4"),
@@ -59,7 +59,15 @@ STREAM_EVENT_DT = np.dtype([("stream_id", "<i8"), ("host_socket_id", "<u8"), ("l
 assert STREAM_DESC_DT.itemsize == 32 and STREAM_MSG_DT.itemsize == 32 and STREAM_EVENT_DT.itemsize == 80
 STREAM_CONNECTED, STREAM_NEED_FEEDBACK, STREAM_CLOSED, STREAM_HANDED_OVER = 1, 2, 4, 8
 STREAM_MSG_IN_INPUT = 1
-STREAM_EV_REMOTE_CONSUMED_MOVED, STREAM_EV_CLOSED_BY_RST, STREAM_EV_CLOSED_BY_CLOSE, STREAM_EV_HANDED_OVER = 1, 2, 4, 8
+STREAM_EV_REMOTE_CONSUMED_MOVED, STREAM_EV_CLOSED_BY_RST, STREAM_EV_CLOSED_BY_CLOSE, STREAM_EV_HANDED_OVER, STREAM_EV_WRITABLE = 1, 2, 4, 8, 16
+# the sending side (b2_stream_write)
+STREAM_WRITE_DT = np.dtype([("stream_id", "<i8"), ("flags", "<u4"), ("src_off", "<u4"), ("src_len", "<u4"), ("reserved", "<u4")])      # == b2_stream_write_desc
+STREAM_WRITE_RESULT_DT = np.dtype([("status", "<i4"), ("n_frames", "<u4"), ("out_off", "<u4"), ("out_len", "<u4"), ("produced", "<u8"),
+                                   ("host_socket_id", "<u8")])
+assert STREAM_WRITE_DT.itemsize == 24 and STREAM_WRITE_RESULT_DT.itemsize == 32
+STREAM_W_FROM_MSG = 1
+STREAM_W_NOT_CONNECTED, STREAM_W_HANDED_OVER = -1, -2
+STREAM_W_DEFAULT_SEGMENT = 512 << 20          # -stream_write_max_segment_size's default (max_segment_size 0)
 
 
 class Method(C.Structure):
@@ -178,6 +186,7 @@ def _load():
     l.b2_stream_query.argtypes = [C.c_void_p, C.c_int64, C.POINTER(StreamState)]
     l.b2_stream_take_pending.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
     l.b2_stream_results.argtypes = [C.c_void_p, C.POINTER(StreamBatchResult)]
+    l.b2_stream_write.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p]
     l.b2_counters_read.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
     l.b2_counters_device_ptr.restype = C.c_void_p; l.b2_counters_device_ptr.argtypes = [C.c_void_p]
     return l
@@ -193,7 +202,7 @@ ABI_SYMBOLS = ["b2_ctx_create", "b2_ctx_destroy", "b2_last_error", "b2_version",
                "b2_counters_device_ptr", "b2_counters_allreduce", "b2_h2_pack_requests", "b2_h2_conn_set_next_stream_id", "b2_h2_conn_peer_update",
                "b2_h2_client_conn_reset", "b2_h2_client_process_batch", "b2_h2_client_abandon_streams", "b2_h2_conn_set_gunzip",
                "b2_h2_serve_batch", "b2_stream_configure", "b2_stream_open", "b2_stream_set_connected", "b2_stream_close", "b2_stream_query",
-               "b2_stream_take_pending", "b2_stream_results"]
+               "b2_stream_take_pending", "b2_stream_results", "b2_stream_write"]
 
 ECHO_METHOD = dict(service_full_name=b"example.EchoService", service_name=b"EchoService", method_name=b"Echo",
                    request_type_name=b"example.EchoRequest", handler=1, echo_attachment=1,
@@ -391,11 +400,11 @@ class Context:
         _check(lib.b2_stream_configure(self._h, max_streams, pending_bytes, out_bytes))
 
     def stream_open(self, streams):
-        """streams: STREAM_DESC_DT array or a list of (stream_id, remote_stream_id, host_socket_id, flags)."""
+        """streams: STREAM_DESC_DT array or a list of (stream_id, remote_stream_id, host_socket_id, flags[, max_buf_size])."""
         if not isinstance(streams, np.ndarray):
             a = np.zeros(len(streams), STREAM_DESC_DT)
             for i, t in enumerate(streams):
-                a[i] = tuple(t) + (0,)
+                a[i] = tuple(t) + (0,) * (5 - len(t))
             streams = a
         streams = np.ascontiguousarray(streams, dtype=STREAM_DESC_DT)
         _check(lib.b2_stream_open(self._h, streams.ctypes.data, len(streams)))
@@ -432,6 +441,38 @@ class Context:
             return np.ctypeslib.as_array((C.c_uint8 * nbytes).from_address(ptr)).view(dt) if nbytes else np.zeros(0, dt)
         return (view(r.msgs, 32 * r.n_msgs, STREAM_MSG_DT), view(r.events, 80 * r.n_events, STREAM_EVENT_DT), view(r.out, r.out_bytes, np.uint8),
                 view(r.ctrl, r.ctrl_bytes, np.uint8), view(r.run_ctrl, 8 * r.n_runs, np.uint32).reshape(-1, 2))
+
+    def stream_write(self, writes, data=None, max_segment_size=0, out_cap=None, out=None):
+        """StreamWrite for a batch of writes (b2_stream_write).  writes: STREAM_WRITE_DT array or a list of (stream_id, flags, src_off,
+        src_len); data: the bytes host-sourced writes index.  Returns (results, out): write i's frames are
+        out[results[i]["out_off"]:results[i]["out_off"] + results[i]["out_len"]]."""
+        if not isinstance(writes, np.ndarray):
+            a = np.zeros(len(writes), STREAM_WRITE_DT)
+            for i, t in enumerate(writes):
+                a[i] = tuple(t) + (0,) * (5 - len(t))
+            writes = a
+        writes = np.ascontiguousarray(writes, dtype=STREAM_WRITE_DT)
+        n = len(writes)
+        if data is None:
+            ptr, nb = None, 0
+        else:
+            data = np.ascontiguousarray(np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray)) else data, dtype=np.uint8)
+            ptr, nb = data.ctypes.data, data.nbytes
+        if out is None:
+            if out_cap is None:         # the bound the call checks: align16(len + ceil(len / seg) * 38) per write
+                seg = max_segment_size or STREAM_W_DEFAULT_SEGMENT
+                lens = np.where(writes["flags"] & STREAM_W_FROM_MSG, 0, writes["src_len"]).astype(np.int64)
+                if np.any(writes["flags"] & STREAM_W_FROM_MSG):
+                    sm = self.stream_results()[0]
+                    fm = (writes["flags"] & STREAM_W_FROM_MSG) != 0
+                    idx = writes["src_off"][fm].astype(np.int64)
+                    lens[fm] = np.where(idx < len(sm), sm["len"][np.minimum(idx, max(len(sm) - 1, 0))] if len(sm) else 0, 0)
+                nfr = np.maximum(1, (lens + seg - 1) // seg)
+                out_cap = int(((lens + nfr * 38 + 15) // 16 * 16).sum())
+            out = np.empty(max(1, out_cap), np.uint8)
+        res = np.zeros(n, STREAM_WRITE_RESULT_DT)
+        _check(lib.b2_stream_write(self._h, ptr, nb, writes.ctypes.data, n, max_segment_size, out.ctypes.data, out.nbytes, res.ctypes.data))
+        return res, out
 
     def batch_info(self):
         out = (C.c_uint32 * 4)()

@@ -59,6 +59,11 @@ struct b2_ctx {
     void* d_st_block[10] = {}; void* h_st_mapped[5] = {}; uint32_t* h_st_cnts = nullptr; uint8_t* h_st_out = nullptr; uint8_t* h_st_ctl = nullptr; uint8_t* d_st_ctl = nullptr;
     b2_stream_msg* h_st_msgs = nullptr; b2_stream_event* h_st_events = nullptr; uint8_t* h_st_ctrl = nullptr; uint32_t* h_st_run_ctrl = nullptr;
     cudaEvent_t st_ev[6] = {};
+    const uint8_t* st_input = nullptr;      // the input bytes of the last batch with a stream pass (B2_STREAM_W_FROM_MSG of IN_INPUT messages); null once overwritten
+    // the sending side (b2_stream_write): staging of its own, grown on demand: [0] host-sourced payloads [1] frames [2] per-write
+    // records and scratch [3] per-table-slot scratch; pinned: the records as the host resolved them, the counters
+    void* d_sw[4] = {}; size_t sw_have[4] = {}; SwRec* h_sw_recs = nullptr; size_t h_sw_have = 0; uint32_t* h_sw_cnts = nullptr;
+    cudaEvent_t sw_ev[8] = {}; bool sw_ran = false;
     // pinned host mirrors
     b2_run_status* h_run_status = nullptr; b2_msg_desc* h_msgs = nullptr; uint8_t* h_resp = nullptr;
     uint32_t* h_totals = nullptr; uint32_t* h_run_tile_base = nullptr;
@@ -78,6 +83,10 @@ struct b2_ctx {
     uint8_t* d_small = nullptr; uint8_t* h_small = nullptr;     // [totals | run_status | msgs | resp]
     bool small = false, small_copy_queued = false, use_fused_small = true; uint32_t small_msgs = 0, small_resp = 0, small_off_rs = 0, small_off_msgs = 0, small_off_resp = 0, small_total = 0;
 };
+
+// d_bytes is about to hold another call's bytes: B2_STREAM_W_FROM_MSG can no longer read the device copy of the last batch's input
+// (a B2_INPUT_PULL batch was read in the caller's region, which stays)
+static void input_overwritten(b2_ctx* c) { if (c->st_input == c->d_bytes) c->st_input = nullptr; }
 
 static uint32_t g_crc_tab_host[256];
 static void crc_table_init() {
@@ -407,7 +416,7 @@ extern "C" int b2_batch_upload(b2_ctx* c, const void* bytes, uint32_t nbytes, co
             for (uint32_t t = t0; t < t1; t++) { uint32_t* q = ti + 4 * (size_t)t; q[0] = runs[r].offset; q[1] = runs[r].length; q[2] = t - t0; q[3] = r | (runs[r].flags << 24); }
         }
     }
-    c->h2_last_in = 0; c->h2_last_out = 0;       // the device copies of the last h2 batch are about to be overwritten
+    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);       // the device copies of the last h2 batch are about to be overwritten
     if (c->input_mode == B2_INPUT_PULL) {
         // no copy: the kernels read the caller's pinned block in place (it must stay untouched until collect)
         void* dp = nullptr;
@@ -446,7 +455,7 @@ static int launch_stream_pass(b2_ctx* c, const BatchPtrs& B, cudaStream_t s, uin
     k_stream_run<<<grid(c->st_max, 4, sms * 8), 128, 0, s>>>(B, S); CU(cudaEventRecord(c->st_ev[4], s));
     k_stream_rst<<<grid(c->n_runs, 4, sms * 4), 128, 0, s>>>(B, S); CU(cudaEventRecord(c->st_ev[5], s));
     CU(cudaMemcpyAsync(c->h_st_cnts, S.cnts, 64, cudaMemcpyDeviceToHost, s));
-    launches += 5; c->stream_ran = true;
+    launches += 5; c->stream_ran = true; c->st_input = B.bytes;
     return B2_OK;
 }
 
@@ -723,6 +732,9 @@ static void stream_free(b2_ctx* c) {
     for (void*& p : c->h_st_mapped) { cudaFreeHost(p); p = nullptr; }
     cudaFreeHost(c->h_st_cnts); c->h_st_cnts = nullptr; cudaFreeHost(c->h_st_out); c->h_st_out = nullptr;
     for (cudaEvent_t& e : c->st_ev) if (e) { cudaEventDestroy(e); e = nullptr; }
+    for (int i = 0; i < 4; i++) { cudaFree(c->d_sw[i]); c->d_sw[i] = nullptr; c->sw_have[i] = 0; }
+    cudaFreeHost(c->h_sw_recs); c->h_sw_recs = nullptr; c->h_sw_have = 0; cudaFreeHost(c->h_sw_cnts); c->h_sw_cnts = nullptr;
+    for (cudaEvent_t& e : c->sw_ev) if (e) { cudaEventDestroy(e); e = nullptr; }
     cudaGetLastError();
 }
 static int stream_configure(b2_ctx* c, uint32_t max_streams, uint32_t pending_bytes, uint32_t out_bytes);
@@ -734,7 +746,7 @@ extern "C" int b2_stream_configure(b2_ctx* c, uint32_t max_streams, uint32_t pen
 static int stream_configure(b2_ctx* c, uint32_t max_streams, uint32_t pending_bytes, uint32_t out_bytes) {
     if (!c || max_streams == 0 || max_streams > (1u << 24) || pending_bytes == 0 || (pending_bytes & 15u)) { set_err("max_streams in 1 .. 2^24, pending_bytes a non-zero multiple of 16"); return B2_E_INVAL; }
     if (c->has_streams) { set_err("the stream table is already configured"); return B2_E_INVAL; }
-    static_assert(sizeof(StreamEnt) == 64 && sizeof(b2_stream_msg) == 32 && sizeof(b2_stream_event) == 80 && sizeof(b2_stream_desc) == 32 && sizeof(b2_stream_state) == 32, "stream ABI layout");
+    static_assert(sizeof(StreamEnt) == 80 && sizeof(b2_stream_msg) == 32 && sizeof(b2_stream_event) == 80 && sizeof(b2_stream_desc) == 32 && sizeof(b2_stream_state) == 32, "stream ABI layout");
     CU(cudaSetDevice(c->opt.device));
     CU(cudaStreamSynchronize(c->stream));
     ring_halt(c);
@@ -798,7 +810,7 @@ extern "C" int b2_stream_open(b2_ctx* c, const b2_stream_desc* streams, uint32_t
         uint32_t h = stream_hash((long long)d.stream_id, cap);
         while (c->st_state[h] == 1) h = (h + 1) & (cap - 1);
         StreamEnt e; memset(&e, 0, sizeof e);
-        e.id = d.stream_id; e.remote_id = d.remote_stream_id; e.host_socket = d.host_socket_id;
+        e.id = d.stream_id; e.remote_id = d.remote_stream_id; e.host_socket = d.host_socket_id; e.max_buf = d.max_buf_size;
         e.flags = kStUsed | ((d.flags & B2_STREAM_CONNECTED) ? kStConnected : 0u) | ((d.flags & B2_STREAM_NEED_FEEDBACK) ? kStNeedFeedback : 0u);
         e.pool_idx = c->st_pool_free.back(); c->st_pool_free.pop_back();
         c->st_state[h] = 1; c->st_keys[h] = (long long)d.stream_id; c->st_pool[h] = e.pool_idx; c->st_open++;
@@ -881,6 +893,100 @@ extern "C" int b2_stream_results(b2_ctx* c, b2_stream_batch_result* out) {
     out->msgs = c->h_st_msgs; out->n_msgs = n[0]; out->events = c->h_st_events; out->n_events = n[1];
     out->out = c->h_st_out; out->out_bytes = n[2]; out->ctrl = c->h_st_ctrl; out->ctrl_bytes = n[3];
     out->run_ctrl = c->h_st_run_ctrl; out->n_runs = c->n_runs;
+    return B2_OK;
+}
+
+// ---- the sending side of a Stream (b2_stream_write, k_sw_*) ---------------------------------------------------------------------
+// Staging of its own (never d_bytes / d_msgs / d_resp or the stream pass's results): the last batch's results and input bytes stay as
+// they are, so FROM_MSG writes can read them in place.
+static const char* const kSwStages[7] = { "stream_write_route", "stream_write_alloc", "stream_write_group", "stream_write_admit",
+                                          "stream_write_scan", "stream_write_frames", "stream_write_copy" };
+static int sw_reserve(b2_ctx* c, int i, size_t need) {          // device staging i holds at least `need` bytes (+ 32 of slack)
+    if (need <= c->sw_have[i] && c->d_sw[i]) return B2_OK;
+    size_t n = 4096; while (n < need) n <<= 1;
+    cudaFree(c->d_sw[i]); c->d_sw[i] = nullptr; c->sw_have[i] = 0;
+    if (cudaMalloc(&c->d_sw[i], n + 32) != cudaSuccess) { cudaGetLastError(); set_err("cudaMalloc of the stream write staging failed"); return B2_E_NOMEM; }
+    c->sw_have[i] = n;
+    return B2_OK;
+}
+extern "C" int b2_stream_write(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_stream_write_desc* writes, uint32_t n,
+                               uint32_t max_segment_size, void* out, uint32_t out_cap, b2_stream_write_result* results) {
+    static_assert(sizeof(b2_stream_write_desc) == 24 && sizeof(b2_stream_write_result) == 32 && sizeof(SwRec) == 24, "stream write ABI layout");
+    if (!c || !c->has_streams || (!bytes && nbytes) || (!writes && n) || (!results && n) || (!out && out_cap)) { set_err("no stream table (b2_stream_configure) or null argument"); return B2_E_INVAL; }
+    if (c->stream_armed) { set_err("a submitted batch must be collected first: the stream table belongs to it"); return B2_E_INVAL; }
+    if (n > c->opt.max_msgs || nbytes > c->opt.max_batch_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    CU(cudaSetDevice(c->opt.device));
+    const uint64_t seg = max_segment_size ? max_segment_size : 512ull << 20;       // -stream_write_max_segment_size (stream.cpp:39)
+    const uint32_t n_msgs = c->stream_valid && c->stream_ran ? c->h_st_cnts[0] : 0;
+    if ((size_t)n * sizeof(SwRec) > c->h_sw_have) {
+        cudaFreeHost(c->h_sw_recs); c->h_sw_recs = nullptr; c->h_sw_have = 0;
+        size_t m = 4096; while (m < (size_t)n * sizeof(SwRec)) m <<= 1;
+        if (cudaHostAlloc((void**)&c->h_sw_recs, m, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); set_err("cudaHostAlloc of the stream write records failed"); return B2_E_NOMEM; }
+        c->h_sw_have = m;
+    }
+    int rc = sw_reserve(c, 0, nbytes);
+    if (rc != B2_OK) return rc;
+    // every argument is checked before anything changes; each record carries its payload's device address
+    const uint8_t* d_in = static_cast<const uint8_t*>(c->d_sw[0]);
+    uint64_t bound = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        const b2_stream_write_desc& w = writes[i];
+        SwRec& r = c->h_sw_recs[i];
+        r.id = w.stream_id; r.pad = 0;
+        if (w.flags & ~B2_STREAM_W_FROM_MSG) { set_err("unknown b2_stream_write flag"); return B2_E_INVAL; }
+        if (w.flags & B2_STREAM_W_FROM_MSG) {
+            if (w.src_off >= n_msgs) { set_err("B2_STREAM_W_FROM_MSG: no such message in the last collected batch"); return B2_E_INVAL; }
+            const b2_stream_msg& m = c->h_st_msgs[w.src_off];
+            if ((m.flags & B2_STREAM_MSG_IN_INPUT) && !c->st_input) { set_err("B2_STREAM_W_FROM_MSG: a later call overwrote the last batch's input bytes on the device"); return B2_E_INVAL; }
+            r.src = ((m.flags & B2_STREAM_MSG_IN_INPUT) ? c->st_input : c->sp.out) + m.off; r.len = m.len;
+        } else {
+            if ((uint64_t)w.src_off + w.src_len > nbytes) { set_err("write outside bytes"); return B2_E_INVAL; }
+            r.src = d_in + w.src_off; r.len = w.src_len;
+        }
+        const uint64_t nfr = r.len <= seg ? 1 : (r.len + seg - 1) / seg;
+        bound += (r.len + nfr * kSwHeadMax + 15) & ~15ull;
+    }
+    if (bound > out_cap || bound > c->opt.max_resp_bytes) { set_err("out_cap (or max_resp_bytes) below the sum of align16(len + ceil(len / seg) * 38)"); return B2_E_CAPACITY; }
+    if (n == 0) return B2_OK;
+    const size_t cap = c->sp.cap;
+    const size_t o_res = ((size_t)n * 24 + 15) & ~(size_t)15, o_slot = o_res + 32 * (size_t)n, o_group = o_slot + ((4 * (size_t)n + 15) & ~(size_t)15),
+                 o_fb = o_group + 8 * (size_t)n, o_cb = o_fb + ((4 * (size_t)n + 15) & ~(size_t)15);
+    if ((rc = sw_reserve(c, 1, bound)) != B2_OK || (rc = sw_reserve(c, 2, o_cb + 4 * (size_t)n)) != B2_OK || (rc = sw_reserve(c, 3, 64 + 16 * cap)) != B2_OK) return rc;
+    if (!c->h_sw_cnts) {
+        if (cudaHostAlloc((void**)&c->h_sw_cnts, 64, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); set_err("cudaHostAlloc failed"); return B2_E_NOMEM; }
+        for (cudaEvent_t& e : c->sw_ev) CU(cudaEventCreate(&e));
+    }
+    uint8_t* blk = static_cast<uint8_t*>(c->d_sw[2]);
+    uint32_t* per_slot = static_cast<uint32_t*>(c->d_sw[3]);
+    SwPass P;
+    P.tab = c->sp.tab; P.cap = c->sp.cap; P.recs = reinterpret_cast<const SwRec*>(blk); P.n = n; P.seg = (uint32_t)seg;
+    P.cnts = per_slot; P.cnt = per_slot + 16; P.fill = P.cnt + cap; P.base = P.fill + cap; P.touched = P.base + cap;
+    P.res = reinterpret_cast<b2_stream_write_result*>(blk + o_res); P.slot = reinterpret_cast<uint32_t*>(blk + o_slot); P.group = reinterpret_cast<uint32_t*>(blk + o_group);
+    P.frame_base = reinterpret_cast<uint32_t*>(blk + o_fb); P.chunk_base = reinterpret_cast<uint32_t*>(blk + o_cb);
+    P.out = static_cast<uint8_t*>(c->d_sw[1]);
+    cudaStream_t s = c->stream;
+    const uint32_t sms = c->n_sms, streams = n < c->st_max ? n : c->st_max;
+    auto grid = [&](uint32_t items, uint32_t per_block, uint32_t most) { const uint32_t g = (items + per_block - 1) / per_block; return g < 1 ? 1u : g < most ? g : most; };
+    CU(cudaMemcpyAsync(blk, c->h_sw_recs, sizeof(SwRec) * (size_t)n, cudaMemcpyHostToDevice, s));
+    if (nbytes) CU(cudaMemcpyAsync(c->d_sw[0], bytes, nbytes, cudaMemcpyHostToDevice, s));
+    CU(cudaMemsetAsync(per_slot, 0, 64 + 8 * cap, s));                 // counters | cnt | fill
+    CU(cudaEventRecord(c->sw_ev[0], s));
+    k_sw_route<<<grid(n, 256, sms * 4), 256, 0, s>>>(P); CU(cudaEventRecord(c->sw_ev[1], s));
+    k_sw_alloc<<<grid(streams, 256, sms), 256, 0, s>>>(P); CU(cudaEventRecord(c->sw_ev[2], s));
+    k_sw_group<<<grid(n, 256, sms * 4), 256, 0, s>>>(P); CU(cudaEventRecord(c->sw_ev[3], s));
+    k_sw_admit<<<grid(streams, 4, sms * 8), 128, 0, s>>>(P); CU(cudaEventRecord(c->sw_ev[4], s));
+    k_sw_scan<<<1, kSmallThreads, 0, s>>>(P); CU(cudaEventRecord(c->sw_ev[5], s));
+    k_sw_frames<<<sms * 8, 256, 0, s>>>(P); CU(cudaEventRecord(c->sw_ev[6], s));
+    k_sw_copy<<<sms * 8, 256, 0, s>>>(P); CU(cudaEventRecord(c->sw_ev[7], s));
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(results, P.res, sizeof(b2_stream_write_result) * (size_t)n, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(c->h_sw_cnts, P.cnts, 64, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    c->sw_ran = true;
+    if (c->h_sw_cnts[2]) {
+        CU(cudaMemcpyAsync(out, P.out, c->h_sw_cnts[2], cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+    }
     return B2_OK;
 }
 
@@ -1046,6 +1152,9 @@ extern "C" int b2_stage_times(b2_ctx* c, const char** names, float* ms, int cap)
     if (c->stream_valid && c->stream_ran) {          // the stream pass of the last collected batch, kernel by kernel
         for (int i = 0; i < 5; i++, total++) if (total < cap) { names[total] = kStreamStages[i]; float t = 0.f; cudaEventElapsedTime(&t, c->st_ev[i], c->st_ev[i + 1]); ms[total] = t; }
     }
+    if (c->sw_ran) {                                 // the last b2_stream_write, kernel by kernel
+        for (int i = 0; i < 7; i++, total++) if (total < cap) { names[total] = kSwStages[i]; float t = 0.f; cudaEventElapsedTime(&t, c->sw_ev[i], c->sw_ev[i + 1]); ms[total] = t; }
+    }
     return total;
 }
 
@@ -1103,7 +1212,7 @@ extern "C" int b2_crc32c_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, co
     if (nbytes > c->opt.max_batch_bytes || n > c->opt.max_msgs) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     for (uint32_t i = 0; i < n; i++) if ((uint64_t)offs[i] + lens[i] > nbytes) { set_err("slice outside buffer"); return B2_E_INVAL; }
     CU(cudaSetDevice(c->opt.device));
-    c->h2_last_in = 0; c->h2_last_out = 0;       // the device copies of the last h2 batch are about to be overwritten
+    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);       // the device copies of the last h2 batch are about to be overwritten
     CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(c->d_frame_off, offs, 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(c->d_slot, lens, 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
@@ -1147,7 +1256,7 @@ extern "C" int b2_snappy_uncompress_batch(b2_ctx* c, const void* bytes, uint32_t
     CU(cudaSetDevice(c->opt.device));
     uint32_t* d_offs = c->d_frame_off; uint32_t* d_lens = c->d_slot; uint32_t* d_ooffs = c->d_frame_run;
     uint32_t* d_caps = (uint32_t*)c->d_jobs; int32_t* d_olens = (int32_t*)c->d_aux;
-    c->h2_last_in = 0; c->h2_last_out = 0;       // the device copies of the last h2 batch are about to be overwritten
+    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);       // the device copies of the last h2 batch are about to be overwritten
     CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_offs, offs, 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_lens, lens, 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
@@ -1184,7 +1293,7 @@ extern "C" int b2_snappy_compress_batch(b2_ctx* c, const void* bytes, uint32_t n
     }
     CU(cudaSetDevice(c->opt.device));
     uint32_t* d_offs = c->d_frame_off; uint32_t* d_lens = c->d_slot; uint32_t* d_ooffs = c->d_frame_run; uint32_t* d_olens = (uint32_t*)c->d_aux;
-    c->h2_last_in = 0; c->h2_last_out = 0;       // the device copies of the last h2 batch are about to be overwritten
+    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);       // the device copies of the last h2 batch are about to be overwritten
     CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_offs, offs, 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_lens, lens, 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
@@ -1290,7 +1399,7 @@ extern "C" int b2_hpack_decode_batch(b2_ctx* c, const void* bytes, uint32_t nbyt
     CU(cudaSetDevice(c->opt.device));
     uint32_t* d_conn = c->d_frame_off; uint32_t* d_off = c->d_frame_run; uint32_t* d_len = c->d_slot;
     uint32_t* d_first = (uint32_t*)c->d_jobs; uint32_t* d_olens = (uint32_t*)c->d_aux; int32_t* d_st = (int32_t*)c->d_aux + n; uint32_t* d_nh = (uint32_t*)c->d_aux + 2 * (size_t)n;
-    c->h2_last_in = 0; c->h2_last_out = 0;       // the device copies of the last h2 batch are about to be overwritten
+    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);       // the device copies of the last h2 batch are about to be overwritten
     CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_conn, conn.data(), 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_off, off.data(), 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
@@ -1314,7 +1423,7 @@ extern "C" int b2_h2_scan_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, c
     CU(cudaSetDevice(c->opt.device));
     static_assert(sizeof(b2_h2_frame) == sizeof(H2Frame), "frame layout");
     uint32_t* d_n = c->d_frame_off; uint32_t* d_cons = c->d_frame_run; uint32_t* d_err = c->d_slot;
-    c->h2_last_in = 0; c->h2_last_out = 0;       // the device copies of the last h2 batch are about to be overwritten
+    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);       // the device copies of the last h2 batch are about to be overwritten
     CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(c->d_meta, runs, sizeof(b2_run) * (size_t)n_runs, cudaMemcpyHostToDevice, c->stream));
     if (n_runs) k_h2_scan<<<(n_runs + 63) / 64, 64, 0, c->stream>>>(c->d_bytes, (const b2_run*)c->d_meta, n_runs, max_frame_size, (H2Frame*)c->d_unz, cap_per_run, d_n, d_cons, d_err);
@@ -1433,7 +1542,7 @@ static int h2_parse_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b
     CU(cudaSetDevice(c->opt.device));
     b2_h2_run_status* d_rs = reinterpret_cast<b2_h2_run_status*>(c->d_run_status);      // 32 B each, like b2_run_status
     M* d_descs = reinterpret_cast<M*>(c->d_msgs);                                        // 64 B each, like b2_msg_desc
-    c->h2_last_in = 0; c->h2_last_out = 0;       // the device copies of the last h2 batch are about to be overwritten
+    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);       // the device copies of the last h2 batch are about to be overwritten
     CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(c->d_meta, runs, sizeof(b2_run) * (size_t)n_runs, cudaMemcpyHostToDevice, c->stream));
     if constexpr (kClient) k_h2_client_consume<<<(n_runs + 31) / 32, 32, 0, c->stream>>>(c->d_bytes, (const b2_run*)c->d_meta, n_runs, c->d_h2, c->d_hpack,
@@ -1657,7 +1766,7 @@ extern "C" int b2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes, c
     CU(cudaSetDevice(c->opt.device));
     ReqDesc* d_reqs = reinterpret_cast<ReqDesc*>(c->d_msgs);
     uint32_t* d_offs = c->d_frame_off; uint32_t* d_lens = c->d_slot;
-    c->h2_last_in = 0; c->h2_last_out = 0;       // the device copies of the last h2 batch are about to be overwritten
+    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);       // the device copies of the last h2 batch are about to be overwritten
     if (nbytes) CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_reqs, reqs, sizeof(b2_request) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_offs, out_offs, 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
@@ -1698,7 +1807,7 @@ extern "C" int b2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbytes, 
     CU(cudaSetDevice(c->opt.device));
     ReplyDesc* d_reps = reinterpret_cast<ReplyDesc*>(c->d_msgs);
     uint32_t* d_offs = c->d_frame_off; uint32_t* d_lens = c->d_slot;
-    c->h2_last_in = 0; c->h2_last_out = 0;
+    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);
     if (nbytes) CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_reps, reps, sizeof(b2_reply) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_offs, out_offs, 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));

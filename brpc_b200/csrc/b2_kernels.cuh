@@ -2869,13 +2869,15 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_ring(RingDev R, BatchPtrs 
 constexpr uint32_t kStUsed = 1, kStConnected = 2, kStNeedFeedback = 4, kStClosed = 8, kStHandedOver = 16, kStTomb = 32;
 constexpr int32_t kFrameRst = 1, kFrameClose = 2, kFrameData = 3, kFrameFeedback = 4;     // brpc::FrameType (streaming_rpc_meta.proto:32-38)
 constexpr uint32_t kStreamCtrlMax = 64;     // bytes of one control frame: 12 + stream_id, source_stream_id, frame_type, feedback{consumed_size} <= 49
-struct __align__(16) StreamEnt {            // 64 bytes
+struct __align__(16) StreamEnt {            // 80 bytes
     long long id, remote_id;
     unsigned long long host_socket, local_consumed, remote_consumed;
     uint32_t flags; int32_t error;
     uint32_t pending_len, pending_frames;   // the partial message in this stream's pool slot
     uint32_t pool_idx;                      // its slot of the pending pool (handed out by the host)
-    uint32_t pad;
+    uint32_t max_buf;                       // StreamOptions::max_buf_size (0: no window)
+    unsigned long long produced;            // Stream::_produced (b2_stream_write; kept only with a window)
+    uint32_t pad[2];
 };
 struct StreamPass {
     StreamEnt* tab; uint32_t cap;           // open addressing on the id, cap a power of two; the host picks the slots (b2_stream_open)
@@ -2897,14 +2899,32 @@ B2_HD uint32_t stream_hash(long long id, uint32_t cap) {
     unsigned long long x = (unsigned long long)id * 0x9e3779b97f4a7c15ull;
     return (uint32_t)(x >> 32) & (cap - 1);
 }
-__device__ __forceinline__ uint32_t stream_probe(const StreamPass& S, long long id) {
-    uint32_t h = stream_hash(id, S.cap);
-    for (uint32_t k = 0; k < S.cap; k++, h = (h + 1) & (S.cap - 1)) {
-        const uint32_t f = S.tab[h].flags;
+__device__ __forceinline__ uint32_t stream_probe(const StreamEnt* tab, uint32_t cap, long long id) {
+    uint32_t h = stream_hash(id, cap);
+    for (uint32_t k = 0; k < cap; k++, h = (h + 1) & (cap - 1)) {
+        const uint32_t f = tab[h].flags;
         if (f == 0) return kNone;
-        if ((f & kStUsed) && S.tab[h].id == id) return h;
+        if ((f & kStUsed) && tab[h].id == id) return h;
     }
     return kNone;
+}
+__device__ __forceinline__ uint32_t stream_probe(const StreamPass& S, long long id) { return stream_probe(S.tab, S.cap, id); }
+// a stream's slice of frame / write indices in ascending order: bitonic sort by one warp over the slice padded to a power of two
+__device__ __forceinline__ void warp_sort_slice(uint32_t* g, uint32_t n, uint32_t lane) {
+    uint32_t P = 1; while (P < n) P <<= 1;
+    for (uint32_t i = n + lane; i < P; i += 32) g[i] = kNone;
+    __syncwarp();
+    for (uint32_t k = 2; k <= P; k <<= 1)
+        for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+            for (uint32_t i = lane; i < P; i += 32) {
+                const uint32_t l = i ^ j;
+                if (l > i) {
+                    const uint32_t a = g[i], b = g[l];
+                    if (((i & k) == 0) ? a > b : a < b) { g[i] = b; g[l] = a; }
+                }
+            }
+            __syncwarp();
+        }
 }
 // PackStreamMessage (policy/streaming_rpc_protocol.cpp:42-58) of a frame without payload; returns its length (<= kStreamCtrlMax)
 __device__ __forceinline__ uint32_t stream_ctrl_frame(uint8_t* o, long long stream_id, bool has_source, long long source, int32_t type, bool has_fb, unsigned long long consumed) {
@@ -2973,23 +2993,9 @@ __global__ void __launch_bounds__(128) k_stream_run(BatchPtrs B, StreamPass S) {
         const uint32_t s = S.touched[t], n = S.cnt[s];
         uint32_t* g = S.group + S.base[s];
         b2_stream_msg* tm = S.tmp_msgs + S.base[s];
-        {   // the slice in msgs[] order: bitonic sort over the padded slice
-            uint32_t P = 1; while (P < n) P <<= 1;
-            for (uint32_t i = n + lane; i < P; i += 32) g[i] = kNone;
-            __syncwarp();
-            for (uint32_t k = 2; k <= P; k <<= 1)
-                for (uint32_t j = k >> 1; j > 0; j >>= 1) {
-                    for (uint32_t i = lane; i < P; i += 32) {
-                        const uint32_t l = i ^ j;
-                        if (l > i) {
-                            const uint32_t a = g[i], b = g[l];
-                            if (((i & k) == 0) ? a > b : a < b) { g[i] = b; g[l] = a; }
-                        }
-                    }
-                    __syncwarp();
-                }
-        }
+        warp_sort_slice(g, n, lane);                         // the slice in msgs[] order
         StreamEnt e = S.tab[s];
+        const unsigned long long rc0 = e.remote_consumed;   // (SetRemoteConsumed's was_full: produced does not move during a batch)
         __syncwarp();                                        // every lane holds the entry before lane 0 may publish the walk's result
         uint8_t* pend = S.pool + (size_t)e.pool_idx * S.pending_bytes;
         uint32_t nm = 0, ev = 0, handover = kNone;
@@ -3068,6 +3074,8 @@ __global__ void __launch_bounds__(128) k_stream_run(BatchPtrs B, StreamPass S) {
         if (closed) for (uint32_t q = k + lane; q < n; q += 32) if (stream_wants_rst(B.msgs[g[q]])) S.rst[g[q]] = 1;
         // one Consume for the batch, then the control frames: FEEDBACK before CLOSE
         e.local_consumed += consumed;
+        // SetRemoteConsumed (stream.cpp:362-401) wakes the StreamWait waiters when the stream goes from full to not full
+        if (e.max_buf && e.produced >= rc0 + e.max_buf && e.produced < e.remote_consumed + e.max_buf) ev |= B2_STREAM_EV_WRITABLE;
         uint32_t first = 0;
         if (lane == 0) {
             b2_stream_event E;
@@ -3136,6 +3144,194 @@ __global__ void k_stream_ctl(StreamEnt* tab, uint32_t slot, int op, long long re
         if ((e.flags & kStNeedFeedback) && e.local_consumed > 0) len = stream_ctrl_frame(frame, e.remote_id, true, e.id, kFrameFeedback, true, e.local_consumed);
     }
     *frame_len = len;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------------
+// streaming_rpc: the sending side of a Stream (b2_stream_write).  StreamWrite (stream.cpp:782-794) -> AppendIfNotFull (:326-360) ->
+// CutMessageIntoFileDescriptor (:148-215) + PackStreamMessage (policy/streaming_rpc_protocol.cpp:42-58) for a batch of writes, in array
+// order per stream.  Writes of one stream depend on each other only through the sum of the earlier lengths, so admission is a
+// segmented prefix sum: write k is not full exactly when produced + T_k < remote_consumed + max_buf_size (T_k: the lengths of the
+// stream's earlier writes of the call; after the first refusal every later write is full too, so refusals never need to leave T).
+//   k_sw_route   thread/write         table probe; an id that does not resolve (or was closed by the peer) is answered EINVAL here
+//   k_sw_alloc   thread/stream        a power-of-two slice of the group array per touched stream
+//   k_sw_group   thread/write         every stream's write indices into its slice
+//   k_sw_admit   warp/stream          the slice in array order, the statuses from one warp prefix sum, produced stored once
+//   k_sw_scan    one block            out offsets (16-aligned), frame and chunk numbers of the admitted writes, in array order
+//   k_sw_frames  thread/frame         the 12-byte head + StreamFrameMeta of every frame
+//   k_sw_copy    warp/(write, chunk)  the payloads: aligned 16-byte stores fed from shifted 16-byte loads (warp_copy_shifted)
+constexpr uint32_t kSwChunk = 8192;          // payload bytes of one copy work item
+constexpr uint32_t kSwHeadMax = 38;          // 12 + stream_id (1 + 10) + source_stream_id (1 + 10) + frame_type (2) + has_continuation (2)
+constexpr int32_t kErrEAGAIN = 11, kErrEINVAL = 22;
+struct SwRec { long long id; const uint8_t* src; uint32_t len, pad; };   // a write as the host resolved it: the payload's device address
+struct SwPass {
+    StreamEnt* tab; uint32_t cap;
+    const SwRec* recs; uint32_t n; uint32_t seg;
+    uint32_t* cnts;                         // [16] [0] touched streams [1] group words [2] out bytes [3] frames [4] copy chunks
+    uint32_t* cnt; uint32_t* fill; uint32_t* base; uint32_t* touched;   // [cap] each, as the stream pass's
+    uint32_t* slot;                         // [n] table slot of every write (kNone: answered by k_sw_route)
+    uint32_t* group;                        // [2n] slices padded to a power of two
+    uint32_t* frame_base; uint32_t* chunk_base;   // [n] exclusive scans of n_frames / copy chunks
+    b2_stream_write_result* res;            // [n]
+    uint8_t* out;
+};
+__device__ __forceinline__ uint32_t sw_meta_len(long long remote, long long id) {
+    return 1 + varint_len((uint64_t)remote) + 1 + varint_len((uint64_t)id) + 2 + 2;
+}
+// bytes r .. r + 15 of the 32 bytes lo:hi (little-endian words)
+__device__ __forceinline__ uint4 shift16(const uint4& lo, const uint4& hi, uint32_t r) {
+    const uint32_t q = r >> 2, sh = (r & 3u) * 8u;
+    const uint32_t v0 = q == 0 ? lo.x : q == 1 ? lo.y : q == 2 ? lo.z : lo.w;
+    const uint32_t v1 = q == 0 ? lo.y : q == 1 ? lo.z : q == 2 ? lo.w : hi.x;
+    const uint32_t v2 = q == 0 ? lo.z : q == 1 ? lo.w : q == 2 ? hi.x : hi.y;
+    const uint32_t v3 = q == 0 ? lo.w : q == 1 ? hi.x : q == 2 ? hi.y : hi.z;
+    const uint32_t v4 = q == 0 ? hi.x : q == 1 ? hi.y : q == 2 ? hi.z : hi.w;
+    return make_uint4(__funnelshift_r(v0, v1, sh), __funnelshift_r(v1, v2, sh), __funnelshift_r(v2, v3, sh), __funnelshift_r(v3, v4, sh));
+}
+// dst[0, n) = src[0, n) by one warp, for any alignment of either: every aligned 16-byte word of dst is one store, assembled from the
+// two aligned 16-byte words of src that hold its bytes; the edges (< 16 bytes each) go byte by byte, so bytes next to the range are not
+// touched.  A load never leaves the aligned 16-byte word of a byte inside src (so never its allocation); src must not change while the
+// kernel runs (the read-only path).
+__device__ __forceinline__ void warp_copy_shifted(uint8_t* dst, const uint8_t* src, uint32_t n, uint32_t lane) {
+    const uintptr_t d0 = (uintptr_t)dst, a0 = (d0 + 15u) & ~(uintptr_t)15u, a1 = (d0 + n) & ~(uintptr_t)15u;
+    if (n < 32) { if (lane < n) dst[lane] = src[lane]; return; }
+    const uint32_t head = (uint32_t)(a0 - d0), tail = (uint32_t)(a1 - d0), nw = (uint32_t)((a1 - a0) >> 4);
+    if (lane < head) dst[lane] = src[lane];
+    if (lane < n - tail) dst[tail + lane] = src[tail + lane];
+    const uintptr_t s = (uintptr_t)(src + head);
+    const uint32_t r = (uint32_t)(s & 15u);
+    const uint4* sw = reinterpret_cast<const uint4*>(s - r);
+    uint4* dw = reinterpret_cast<uint4*>(a0);
+    if (r == 0) for (uint32_t k = lane; k < nw; k += 32) dw[k] = __ldg(sw + k);
+    else for (uint32_t k = lane; k < nw; k += 32) dw[k] = shift16(__ldg(sw + k), __ldg(sw + k + 1), r);
+}
+
+__global__ void __launch_bounds__(256) k_sw_route(SwPass P) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < P.n; i += gridDim.x * blockDim.x) {
+        uint32_t s = stream_probe(P.tab, P.cap, P.recs[i].id);
+        if (s != kNone && (P.tab[s].flags & kStClosed)) s = kNone;       // Close SetFailed's the fake socket (stream.cpp:710)
+        if (s == kNone) {                                                // Socket::Address fails: EINVAL (:785-788)
+            b2_stream_write_result r; r.status = kErrEINVAL; r.n_frames = 0; r.out_off = 0; r.out_len = 0; r.produced = 0; r.host_socket_id = 0;
+            P.res[i] = r;
+        } else if (atomicAdd(&P.cnt[s], 1u) == 0) P.touched[atomicAdd(&P.cnts[0], 1u)] = s;
+        P.slot[i] = s;
+    }
+}
+__global__ void __launch_bounds__(256) k_sw_alloc(SwPass P) {
+    const uint32_t n = P.cnts[0];
+    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
+        const uint32_t s = P.touched[t], c = P.cnt[s];
+        uint32_t p = 1; while (p < c) p <<= 1;
+        P.base[s] = atomicAdd(&P.cnts[1], p);
+    }
+}
+__global__ void __launch_bounds__(256) k_sw_group(SwPass P) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < P.n; i += gridDim.x * blockDim.x) {
+        const uint32_t s = P.slot[i];
+        if (s != kNone) P.group[P.base[s] + atomicAdd(&P.fill[s], 1u)] = i;
+    }
+}
+__global__ void __launch_bounds__(128) k_sw_admit(SwPass P) {
+    const uint32_t lane = threadIdx.x & 31, n_warps = (gridDim.x * blockDim.x) >> 5, n_touched = P.cnts[0];
+    for (uint32_t t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; t < n_touched; t += n_warps) {
+        const uint32_t s = P.touched[t], n = P.cnt[s];
+        uint32_t* g = P.group + P.base[s];
+        warp_sort_slice(g, n, lane);                                     // the stream's writes in array order
+        const StreamEnt& E = P.tab[s];
+        const uint32_t flags = E.flags, max_buf = E.max_buf;
+        const unsigned long long p0 = E.produced, limit = E.remote_consumed + max_buf, sock = E.host_socket;
+        const uint32_t head = 12 + sw_meta_len(E.remote_id, E.id);
+        const bool handed = flags & kStHandedOver, conn = flags & kStConnected, window = max_buf > 0;
+        const bool charged = window && conn && !handed;                  // (AppendIfNotFull charges only under a window, :329-345)
+        unsigned long long carry = 0, t_full = ~0ull;                    // T of the first refusal: produced stays there
+        for (uint32_t k0 = 0; k0 < n; k0 += 32) {
+            const bool on = k0 + lane < n;
+            const uint32_t i = on ? g[k0 + lane] : 0, len = on ? P.recs[i].len : 0;
+            unsigned long long x = len;
+            for (uint32_t o = 1; o < 32; o <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+            const unsigned long long T = carry + x - len;
+            const bool full = window && !handed && (charged ? p0 + T : p0) >= limit;
+            const uint32_t fb = __ballot_sync(0xffffffffu, on && full && charged);
+            if (fb && t_full == ~0ull) t_full = __shfl_sync(0xffffffffu, T, __ffs(fb) - 1);
+            if (on) {
+                b2_stream_write_result r; r.n_frames = 0; r.out_off = 0; r.out_len = 0; r.host_socket_id = sock;
+                if (handed) r.status = B2_STREAM_W_HANDED_OVER;
+                else if (full) r.status = kErrEAGAIN;
+                else if (len == 0) r.status = kErrEINVAL;                // Socket::Write of an empty IOBuf (socket.cpp:1609-1610)
+                else if (!conn) r.status = B2_STREAM_W_NOT_CONNECTED;
+                else {
+                    r.status = 0;
+                    r.n_frames = len <= P.seg ? 1u : (len - 1) / P.seg + 1;
+                    r.out_len = len + r.n_frames * head;
+                }
+                r.produced = !charged ? p0 : full ? p0 + t_full : p0 + T + len;
+                P.res[i] = r;
+            }
+            carry += __shfl_sync(0xffffffffu, x, 31);
+        }
+        if (lane == 0 && charged) P.tab[s].produced = p0 + (t_full != ~0ull ? t_full : carry);
+    }
+}
+__global__ void __launch_bounds__(kSmallThreads) k_sw_scan(SwPass P) {
+    __shared__ uint32_t warp_tot[kSmallWarps];
+    const uint32_t per = (P.n + kSmallThreads - 1) / kSmallThreads;
+    const uint32_t i0 = min(P.n, threadIdx.x * per), i1 = min(P.n, i0 + per);
+    uint32_t b = 0, f = 0, c = 0;
+    for (uint32_t i = i0; i < i1; i++) {
+        const b2_stream_write_result& r = P.res[i];
+        b += (r.out_len + 15u) & ~15u; f += r.n_frames; c += r.n_frames ? (P.recs[i].len + kSwChunk - 1) / kSwChunk : 0u;
+    }
+    uint32_t tb, tf, tc;
+    uint32_t ob = block_excl_scan(b, warp_tot, tb), of = block_excl_scan(f, warp_tot, tf), oc = block_excl_scan(c, warp_tot, tc);
+    for (uint32_t i = i0; i < i1; i++) {
+        b2_stream_write_result& r = P.res[i];
+        r.out_off = ob; P.frame_base[i] = of; P.chunk_base[i] = oc;
+        ob += (r.out_len + 15u) & ~15u; of += r.n_frames; oc += r.n_frames ? (P.recs[i].len + kSwChunk - 1) / kSwChunk : 0u;
+    }
+    if (threadIdx.x == 0) { P.cnts[2] = tb; P.cnts[3] = tf; P.cnts[4] = tc; }
+}
+// the write that holds item x of a numbering (frame_base / chunk_base): the last i with base[i] <= x (writes without items share their
+// successor's base and are never the last such i)
+__device__ __forceinline__ uint32_t sw_owner(const uint32_t* base, uint32_t n, uint32_t x) {
+    uint32_t lo = 0, hi = n;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (base[mid] <= x) lo = mid + 1; else hi = mid; }
+    return lo - 1;
+}
+__global__ void __launch_bounds__(256) k_sw_frames(SwPass P) {
+    const uint32_t nf = P.cnts[3];
+    for (uint32_t f = blockIdx.x * blockDim.x + threadIdx.x; f < nf; f += gridDim.x * blockDim.x) {
+        const uint32_t i = sw_owner(P.frame_base, P.n, f), k = f - P.frame_base[i];
+        const b2_stream_write_result& r = P.res[i];
+        const long long id = P.recs[i].id, remote = P.tab[P.slot[i]].remote_id;
+        const uint32_t len = P.recs[i].len, ml = sw_meta_len(remote, id);
+        const bool more = k + 1 < r.n_frames;                            // has_continuation: data left after this segment
+        const uint32_t plen = more ? P.seg : len - k * P.seg;
+        uint8_t* o = P.out + r.out_off + (size_t)k * (12 + ml + P.seg);
+        o[0] = 'S'; o[1] = 'T'; o[2] = 'R'; o[3] = 'M'; put_be32(o + 4, ml + plen); put_be32(o + 8, ml);
+        uint8_t* m = o + 12;
+        *m++ = 0x08; m = put_varint(m, (uint64_t)remote);
+        *m++ = 0x10; m = put_varint(m, (uint64_t)id);
+        *m++ = 0x18; *m++ = (uint8_t)kFrameData;
+        *m++ = 0x20; *m = more ? 1 : 0;
+        if (!more) for (uint8_t* z = o + 12 + ml + plen; ((uintptr_t)z & 15u) != 0; z++) *z = 0;     // the gap to the next write's frames
+    }
+}
+__global__ void __launch_bounds__(256) k_sw_copy(SwPass P) {
+    const uint32_t lane = threadIdx.x & 31, n_warps = (gridDim.x * blockDim.x) >> 5, nc = P.cnts[4];
+    for (uint32_t c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; c < nc; c += n_warps) {
+        const uint32_t i = sw_owner(P.chunk_base, P.n, c), q = c - P.chunk_base[i];
+        const SwRec w = P.recs[i];
+        const b2_stream_write_result& r = P.res[i];
+        const uint64_t head = 12 + sw_meta_len(P.tab[P.slot[i]].remote_id, w.id), seg = P.seg;
+        const uint32_t lo = q * kSwChunk, hi = min(w.len, lo + kSwChunk);
+        uint8_t* o = P.out + r.out_off;
+        // payload byte p of frame p / seg sits at (p / seg + 1) * head + p
+        if (r.n_frames == 1) warp_copy_shifted(o + head + lo, w.src + lo, hi - lo, lane);
+        else if (seg < 64) { for (uint32_t p = lo + lane; p < hi; p += 32) o[(p / seg + 1) * head + p] = w.src[p]; }
+        else for (uint64_t k = lo / seg; k * seg < hi; k++) {
+            const uint32_t a = (uint32_t)max((uint64_t)lo, k * seg), b = (uint32_t)min((uint64_t)hi, (k + 1) * seg);
+            warp_copy_shifted(o + (k + 1) * head + a, w.src + a, b - a, lane);
+        }
+    }
 }
 
 #endif  // __CUDACC__

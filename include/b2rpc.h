@@ -798,7 +798,8 @@ typedef struct b2_stream_desc {
     int64_t  stream_id;               /* what peers put in StreamFrameMeta.stream_id */
     int64_t  remote_stream_id;        /* _remote_settings.stream_id (CONNECTED) */
     uint64_t host_socket_id;          /* opaque; echoed in the events: where FEEDBACK / CLOSE go */
-    uint32_t flags, reserved;
+    uint32_t flags;
+    uint32_t max_buf_size;            /* StreamOptions::max_buf_size when > 0: the write window (b2_stream_write); 0 = no window */
 } b2_stream_desc;                     /* 32 bytes */
 typedef struct b2_stream_state {
     uint64_t local_consumed, remote_consumed;
@@ -819,6 +820,7 @@ typedef struct b2_stream_msg {
 #define B2_STREAM_EV_CLOSED_BY_RST         2u   /* error ECONNRESET */
 #define B2_STREAM_EV_CLOSED_BY_CLOSE       4u   /* error 0 */
 #define B2_STREAM_EV_HANDED_OVER           8u
+#define B2_STREAM_EV_WRITABLE             16u   /* a FEEDBACK of this batch took the stream from full to not full: wake StreamWait */
 typedef struct b2_stream_event {
     int64_t  stream_id;
     uint64_t host_socket_id;
@@ -857,6 +859,57 @@ int  b2_stream_query(b2_ctx* ctx, int64_t stream_id, b2_stream_state* out);
 /* The partial message of a stream (a HANDED_OVER one hands it out this way), at most cap bytes; it is gone from the device afterwards. */
 int  b2_stream_take_pending(b2_ctx* ctx, int64_t stream_id, void* out, uint32_t cap, uint32_t* len);
 int  b2_stream_results(b2_ctx* ctx, b2_stream_batch_result* out);
+
+/* ---- streaming_rpc, the sending side of a Stream on the device ---------------------------------------------------------------------
+ * b2_stream_write: brpc::StreamWrite (src/brpc/stream.cpp:782-794) for a batch of writes against the stream table, applied in array
+ * order as if one thread called StreamWrite for each in turn.  Per write, in this order:
+ *   Socket::Address (:785-788): an id that is not open — never opened, closed locally, or closed by the peer's RST / CLOSE (Close
+ *     SetFailed's the fake socket, :710) — gets EINVAL (produced and host_socket_id 0);
+ *   a HANDED_OVER stream gets B2_STREAM_W_HANDED_OVER: its FEEDBACK frames reach only the host, so the device window is stale;
+ *   AppendIfNotFull (:326-360): with max_buf_size > 0 and produced >= remote_consumed + max_buf_size -> EAGAIN, nothing charged; else
+ *     produced += len (checked BEFORE the add, so one write may overshoot the window).  Without a window produced is not kept (0);
+ *   Socket::Write of an empty message (socket.cpp:1609-1610) -> EINVAL (after the window check, produced -= 0);
+ *   a stream that is not connected -> B2_STREAM_W_NOT_CONNECTED, nothing charged (brpc queues such writes in the fake socket until
+ *     SetConnected; the device has no remote_stream_id to frame them with: write again after b2_stream_set_connected);
+ *   else the frames (CutMessageIntoFileDescriptor :148-215 + PackStreamMessage, policy/streaming_rpc_protocol.cpp:42-58): "STRM",
+ *     BE32 body_size, BE32 meta_size, StreamFrameMeta{stream_id = remote_stream_id, source_stream_id = id, frame_type = DATA,
+ *     has_continuation}, the payload.  len > max_segment_size is cut into ceil(len / seg) frames, all but the last with
+ *     has_continuation = true; otherwise one frame with has_continuation = false.
+ * Each admitted write's frames are contiguous at out + results[i].out_off; out_off is 16-aligned and grows in array order, and the
+ * alignment gaps between writes are zero bytes.  Write them to
+ * host_socket_id in array order (WriteToHostSocket).  brpc leaves the interleaving of different streams on one socket to scheduling;
+ * this call fixes it to array order.  Not modelled: _remote_settings.writable() (brpc fails such writes later with EBADF: check it
+ * before writing), window adaptation (-socket_max_streams_unconsumed_bytes / min_buf_size), write_in_background, StreamWait timeouts.
+ * The call checks everything before any state changes and then fails with B2_E_INVAL / B2_E_CAPACITY: no table, a batch submitted and
+ * not collected, an unknown flag, src_off + src_len > nbytes, a FROM_MSG index not below the last collected batch's n_msgs, more
+ * writes than max_msgs, nbytes > max_batch_bytes, or out_cap (and max_resp_bytes) below the sum over writes of
+ * align16(len + ceil(len / seg) * 38) (38: the longest DATA frame head, 12 + a 26-byte meta; len 0 counts as one frame).
+ * B2_STREAM_W_FROM_MSG takes the payload where the receive pass left msgs[src_off] of the last collected batch (b2_stream_results):
+ * the batch's input bytes (B2_STREAM_MSG_IN_INPUT: the device copy, or the caller's mapped region with B2_INPUT_PULL, which must be
+ * unchanged) or the stream out region — nothing crosses PCIe to the device.  The device copy of the batch's input lasts until the next
+ * call that uploads bytes to the context (b2_pack_*, b2_h2_*, b2_hpack_decode_batch, b2_crc32c_batch, the snappy batch calls; a batch
+ * call ends the last batch altogether): after such a call a FROM_MSG write of a B2_STREAM_MSG_IN_INPUT message fails with B2_E_INVAL,
+ * while out-region messages (and, with B2_INPUT_PULL, the caller's region) can still be written.
+ * The call has its own staging: b2_stream_results and b2_batch_result stay valid and unchanged across any number of write calls. */
+#define B2_STREAM_W_FROM_MSG       1u    /* payload = msgs[src_off] of the last collected batch's b2_stream_batch_result */
+#define B2_STREAM_W_NOT_CONNECTED  (-1)  /* statuses of the device; negative, so they never collide with an errno */
+#define B2_STREAM_W_HANDED_OVER    (-2)
+typedef struct b2_stream_write_desc {
+    int64_t  stream_id;               /* the local StreamId (b2_stream_desc.stream_id) */
+    uint32_t flags;                   /* B2_STREAM_W_FROM_MSG */
+    uint32_t src_off, src_len;        /* the message inside `bytes`; FROM_MSG: src_off = message index, src_len ignored */
+    uint32_t reserved;
+} b2_stream_write_desc;               /* 24 bytes (not "b2_stream_write": that name is the function) */
+typedef struct b2_stream_write_result {
+    int32_t  status;                  /* what StreamWrite returns: 0, EAGAIN, EINVAL; or B2_STREAM_W_* */
+    uint32_t n_frames;
+    uint32_t out_off, out_len;        /* the write's frames inside out (len 0 unless status 0) */
+    uint64_t produced;                /* _produced after this write */
+    uint64_t host_socket_id;          /* where the frames go (WriteToHostSocket) */
+} b2_stream_write_result;             /* 32 bytes */
+/* max_segment_size: -stream_write_max_segment_size (stream.cpp:39); 0 = brpc's default, 512 MiB. */
+int  b2_stream_write(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2_stream_write_desc* writes, uint32_t n,
+                     uint32_t max_segment_size, void* out, uint32_t out_cap, b2_stream_write_result* results);
 
 /* ---- counters (bvar::Adder-like, SURVEY §8e): per-GPU totals accumulated by
  * the kernels: [0] in_bytes [1] in_msgs [2] out_bytes [3] out_msgs [4] errors
