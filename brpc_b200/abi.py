@@ -186,6 +186,7 @@ def _load():
     l.b2_stream_query.argtypes = [C.c_void_p, C.c_int64, C.POINTER(StreamState)]
     l.b2_stream_take_pending.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
     l.b2_stream_results.argtypes = [C.c_void_p, C.POINTER(StreamBatchResult)]
+    l.b2_stream_ring_enable.argtypes = [C.c_void_p, C.c_uint32]
     l.b2_stream_write.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p]
     l.b2_counters_read.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
     l.b2_counters_device_ptr.restype = C.c_void_p; l.b2_counters_device_ptr.argtypes = [C.c_void_p]
@@ -202,7 +203,7 @@ ABI_SYMBOLS = ["b2_ctx_create", "b2_ctx_destroy", "b2_last_error", "b2_version",
                "b2_counters_device_ptr", "b2_counters_allreduce", "b2_h2_pack_requests", "b2_h2_conn_set_next_stream_id", "b2_h2_conn_peer_update",
                "b2_h2_client_conn_reset", "b2_h2_client_process_batch", "b2_h2_client_abandon_streams", "b2_h2_conn_set_gunzip",
                "b2_h2_serve_batch", "b2_stream_configure", "b2_stream_open", "b2_stream_set_connected", "b2_stream_close", "b2_stream_query",
-               "b2_stream_take_pending", "b2_stream_results", "b2_stream_write"]
+               "b2_stream_take_pending", "b2_stream_results", "b2_stream_write", "b2_stream_ring_enable"]
 
 ECHO_METHOD = dict(service_full_name=b"example.EchoService", service_name=b"EchoService", method_name=b"Echo",
                    request_type_name=b"example.EchoRequest", handler=1, echo_attachment=1,
@@ -432,8 +433,13 @@ class Context:
         _check(lib.b2_stream_take_pending(self._h, stream_id, buf.ctypes.data, cap, C.byref(n)))
         return buf[:n.value].tobytes()
 
+    def stream_ring_enable(self, out_bytes):
+        """Run the stream pass on the ring too (b2_stream_ring_enable): after stream_configure, before the first ring call."""
+        _check(lib.b2_stream_ring_enable(self._h, out_bytes))
+
     def stream_results(self):
-        """(msgs, events, out, ctrl, run_ctrl) of the last collected batch: views of context-owned memory, valid until the next batch call."""
+        """(msgs, events, out, ctrl, run_ctrl) of the last collected batch or ring ticket: views of context-owned memory, valid until the
+        next batch call (a ring ticket's: until its slot is reused)."""
         r = StreamBatchResult()
         _check(lib.b2_stream_results(self._h, C.byref(r)))
 

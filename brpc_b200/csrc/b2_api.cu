@@ -31,6 +31,11 @@ constexpr int kMaxStages = 16;
 constexpr uint32_t kSmallBytes = 128 << 10;        // batches up to this size take the latency path
 constexpr uint32_t kSmallRuns = 512, kSmallMsgs = 1024;   // == kSmallThreads, 2 * kSmallThreads of k_small
 constexpr size_t kSmallBlock = 64 + kSmallRuns * 32 + kSmallMsgs * (64 + 16) + (kSmallBytes + kSmallMsgs * 80 + 4096);
+// a ring slot's stream section (b2_stream_ring_enable), and the device staging k_ring fills before it pushes the section:
+// [counters 64 | events | msgs | ctrl | run_ctrl | out], each part sized for what one ticket of <= kSmallMsgs messages can produce
+// (touched streams <= messages; per message at most one RST frame, per stream one FEEDBACK and one CLOSE frame)
+constexpr uint32_t kSecEvents = 64, kSecMsgs = kSecEvents + kSmallMsgs * 80, kSecCtrl = kSecMsgs + kSmallMsgs * 32,
+                   kSecRunCtrl = kSecCtrl + 3 * kStreamCtrlMax * kSmallMsgs, kSecOut = kSecRunCtrl + kSmallRuns * 8;
 struct Stage { const char* name; cudaEvent_t ev; };
 }
 
@@ -49,6 +54,10 @@ struct b2_ctx {
     uint8_t* ring_slots = nullptr; volatile uint32_t* ring_ctl = nullptr; uint32_t* d_ring_ticket = nullptr; cudaStream_t ring_stream = nullptr;
     uint32_t ring_next = 1, ring_stride = 0, ring_off_runs = 0, ring_off_in = 0, ring_off_out = 0; bool ring_collected[8] = { true, true, true, true, true, true, true, true };
     const void* ring_bytes[8] = {}; const void* ring_pin_base = nullptr; unsigned long long ring_pin_dev = 0; uint64_t ring_launches = 0;
+    // the stream pass on the ring (b2_stream_ring_enable): the ring's StreamPass writes its results into d_st_ring, k_ring pushes them
+    // to the slot's section at ring_off_st; tickets are collected in order (ring_next_wait); st_view_ticket: the ticket b2_stream_results
+    // describes (0: the last batch call's pass)
+    bool st_ring = false; StreamPass sp_ring = {}; uint8_t* d_st_ring = nullptr; uint32_t ring_off_st = 0, ring_next_wait = 1, st_view_ticket = 0;
     ulonglong2* d_iov = nullptr; b2_iovec* h_iov = nullptr; const void* host_bytes = nullptr;      // B2_RESP_IOVEC
     uint4* d_refs = nullptr; b2_resp_ref* h_refs = nullptr; int input_mode = B2_INPUT_COPY, resp_mode = B2_RESP_COPY; const uint8_t* pull_bytes = nullptr; uint32_t small_off_refs = 0;
     uint32_t* d_crc_adv = nullptr; unsigned long long* d_counters = nullptr; uint32_t* d_totals = nullptr; DevMethod* d_methods = nullptr;
@@ -375,7 +384,7 @@ extern "C" int b2_batch_upload(b2_ctx* c, const void* bytes, uint32_t nbytes, co
     if ((c->input_mode != B2_INPUT_PULL && nbytes > c->opt.max_batch_bytes) || nbytes >= (1u << 31) || n_runs > c->opt.max_runs) { set_err("batch exceeds ctx capacity"); return B2_E_CAPACITY; }
     uint64_t covered = 0; for (uint32_t r = 0; r < n_runs; r++) covered += runs[r].length;
     if (c->input_mode == B2_INPUT_PULL && covered > c->opt.max_batch_bytes) { set_err("runs exceed ctx capacity"); return B2_E_CAPACITY; }
-    c->stream_valid = false;
+    c->stream_valid = false; c->st_view_ticket = 0;
     c->covered = covered;                           // (what the runs hold: with B2_INPUT_PULL nbytes spans the caller's whole arena)
     CU(cudaSetDevice(c->opt.device));
     if (c->adaptive_tile) {
@@ -455,6 +464,7 @@ static int launch_stream_pass(b2_ctx* c, const BatchPtrs& B, cudaStream_t s, uin
     k_stream_run<<<grid(c->st_max, 4, sms * 8), 128, 0, s>>>(B, S); CU(cudaEventRecord(c->st_ev[4], s));
     k_stream_rst<<<grid(c->n_runs, 4, sms * 4), 128, 0, s>>>(B, S); CU(cudaEventRecord(c->st_ev[5], s));
     CU(cudaMemcpyAsync(c->h_st_cnts, S.cnts, 64, cudaMemcpyDeviceToHost, s));
+    if (c->st_ring) CU(cudaMemsetAsync(S.cnt, 0, 8 * (size_t)S.cap, s));     // cnt | fill: zero when the ring's next ticket starts
     launches += 5; c->stream_ran = true; c->st_input = B.bytes;
     return B2_OK;
 }
@@ -734,6 +744,7 @@ static void stream_free(b2_ctx* c) {
     for (cudaEvent_t& e : c->st_ev) if (e) { cudaEventDestroy(e); e = nullptr; }
     for (int i = 0; i < 4; i++) { cudaFree(c->d_sw[i]); c->d_sw[i] = nullptr; c->sw_have[i] = 0; }
     cudaFreeHost(c->h_sw_recs); c->h_sw_recs = nullptr; c->h_sw_have = 0; cudaFreeHost(c->h_sw_cnts); c->h_sw_cnts = nullptr;
+    cudaFree(c->d_st_ring); c->d_st_ring = nullptr;
     for (cudaEvent_t& e : c->sw_ev) if (e) { cudaEventDestroy(e); e = nullptr; }
     cudaGetLastError();
 }
@@ -785,6 +796,13 @@ static int stream_configure(b2_ctx* c, uint32_t max_streams, uint32_t pending_by
     return B2_OK;
 }
 
+// a ring ticket of a context whose ring runs the stream pass is submitted and not collected: the table belongs to k_ring
+static bool ring_owns_table(const b2_ctx* c) {
+    if (!c->st_ring) return false;
+    for (uint32_t k = 0; k < kRingSlots; k++) if (!c->ring_collected[k]) { set_err("a ring ticket is outstanding: b2_ring_wait it first, the stream table belongs to it"); return true; }
+    return false;
+}
+
 static uint32_t stream_find(const b2_ctx* c, int64_t id) {
     const uint32_t cap = c->sp.cap;
     uint32_t h = stream_hash((long long)id, cap);
@@ -797,6 +815,7 @@ static uint32_t stream_find(const b2_ctx* c, int64_t id) {
 
 extern "C" int b2_stream_open(b2_ctx* c, const b2_stream_desc* streams, uint32_t n) {
     if (!c || !c->has_streams || (!streams && n)) { set_err("no stream table (b2_stream_configure) or null argument"); return B2_E_INVAL; }
+    if (ring_owns_table(c)) return B2_E_INVAL;
     if (c->st_open + (uint64_t)n > c->st_max) { set_err("stream table full"); return B2_E_CAPACITY; }
     CU(cudaSetDevice(c->opt.device));
     CU(cudaStreamSynchronize(c->stream));
@@ -832,6 +851,7 @@ extern "C" int b2_stream_open(b2_ctx* c, const b2_stream_desc* streams, uint32_t
 static int stream_ctl(b2_ctx* c, int64_t id, int op, int64_t remote, uint32_t flags, void* frame, uint32_t frame_cap, uint32_t* frame_len, uint32_t* slot_out) {
     if (!c || !c->has_streams || !frame_len || (!frame && frame_cap)) { set_err("no stream table (b2_stream_configure) or null argument"); return B2_E_INVAL; }
     if (frame_cap < kStreamCtrlMax) { set_err("frame_cap must be at least 64"); return B2_E_INVAL; }
+    if (ring_owns_table(c)) return B2_E_INVAL;
     const uint32_t slot = stream_find(c, id);
     if (slot == kNone) { set_err("stream id is not open"); return B2_E_INVAL; }
     CU(cudaSetDevice(c->opt.device));
@@ -875,6 +895,7 @@ extern "C" int b2_stream_query(b2_ctx* c, int64_t stream_id, b2_stream_state* ou
 }
 extern "C" int b2_stream_take_pending(b2_ctx* c, int64_t stream_id, void* out, uint32_t cap, uint32_t* len) {
     if (!len || (!out && cap)) { set_err("null argument"); return B2_E_INVAL; }
+    if (c && ring_owns_table(c)) return B2_E_INVAL;
     StreamEnt e; uint32_t slot;
     int rc = stream_read(c, stream_id, &e, &slot); if (rc != B2_OK) return rc;
     if (e.pending_len > cap) { set_err("the pending bytes do not fit"); return B2_E_CAPACITY; }
@@ -886,8 +907,17 @@ extern "C" int b2_stream_take_pending(b2_ctx* c, int64_t stream_id, void* out, u
 }
 extern "C" int b2_stream_results(b2_ctx* c, b2_stream_batch_result* out) {
     if (!c || !out || !c->has_streams) { set_err("no stream table (b2_stream_configure) or null argument"); return B2_E_INVAL; }
-    if (!c->stream_valid) { set_err("no collected batch of b2_process_batch / b2_batch_collect"); return B2_E_INVAL; }
+    if (!c->stream_valid) { set_err("no collected batch of b2_process_batch / b2_batch_collect / b2_ring_wait"); return B2_E_INVAL; }
     memset(out, 0, sizeof *out);
+    if (c->st_view_ticket) {                               // a ticket the ring served: the slot's stream section
+        const uint8_t* slot = c->ring_slots + (size_t)(c->st_view_ticket % kRingSlots) * c->ring_stride, *sec = slot + c->ring_off_st;
+        const uint32_t* n = reinterpret_cast<const uint32_t*>(sec);
+        out->msgs = reinterpret_cast<const b2_stream_msg*>(sec + kSecMsgs); out->n_msgs = n[0];
+        out->events = reinterpret_cast<const b2_stream_event*>(sec + kSecEvents); out->n_events = n[1];
+        out->out = sec + kSecOut; out->out_bytes = n[2]; out->ctrl = sec + kSecCtrl; out->ctrl_bytes = n[3];
+        out->run_ctrl = reinterpret_cast<const uint32_t*>(sec + kSecRunCtrl); out->n_runs = reinterpret_cast<const RingSlotHdr*>(slot)->n_runs;
+        return B2_OK;
+    }
     if (!c->stream_ran) return B2_OK;                      // (a batch without runs)
     const uint32_t* n = c->h_st_cnts;
     out->msgs = c->h_st_msgs; out->n_msgs = n[0]; out->events = c->h_st_events; out->n_events = n[1];
@@ -914,10 +944,18 @@ extern "C" int b2_stream_write(b2_ctx* c, const void* bytes, uint32_t nbytes, co
     static_assert(sizeof(b2_stream_write_desc) == 24 && sizeof(b2_stream_write_result) == 32 && sizeof(SwRec) == 24, "stream write ABI layout");
     if (!c || !c->has_streams || (!bytes && nbytes) || (!writes && n) || (!results && n) || (!out && out_cap)) { set_err("no stream table (b2_stream_configure) or null argument"); return B2_E_INVAL; }
     if (c->stream_armed) { set_err("a submitted batch must be collected first: the stream table belongs to it"); return B2_E_INVAL; }
+    if (ring_owns_table(c)) return B2_E_INVAL;
     if (n > c->opt.max_msgs || nbytes > c->opt.max_batch_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     CU(cudaSetDevice(c->opt.device));
     const uint64_t seg = max_segment_size ? max_segment_size : 512ull << 20;       // -stream_write_max_segment_size (stream.cpp:39)
-    const uint32_t n_msgs = c->stream_valid && c->stream_ran ? c->h_st_cnts[0] : 0;
+    // FROM_MSG: the messages b2_stream_results describes — a ring ticket's only while it is the most recent one (the next ticket
+    // overwrites the device input and the ring's out staging)
+    const b2_stream_msg* from_msgs = c->h_st_msgs; const uint8_t* from_out = c->sp.out;
+    uint32_t n_msgs = c->stream_valid && c->stream_ran ? c->h_st_cnts[0] : 0;
+    if (c->stream_valid && c->st_view_ticket) {
+        b2_stream_batch_result v; b2_stream_results(c, &v);
+        from_msgs = v.msgs; from_out = c->sp_ring.out; n_msgs = c->st_view_ticket + 1 == c->ring_next ? v.n_msgs : 0;
+    }
     if ((size_t)n * sizeof(SwRec) > c->h_sw_have) {
         cudaFreeHost(c->h_sw_recs); c->h_sw_recs = nullptr; c->h_sw_have = 0;
         size_t m = 4096; while (m < (size_t)n * sizeof(SwRec)) m <<= 1;
@@ -935,10 +973,10 @@ extern "C" int b2_stream_write(b2_ctx* c, const void* bytes, uint32_t nbytes, co
         r.id = w.stream_id; r.pad = 0;
         if (w.flags & ~B2_STREAM_W_FROM_MSG) { set_err("unknown b2_stream_write flag"); return B2_E_INVAL; }
         if (w.flags & B2_STREAM_W_FROM_MSG) {
-            if (w.src_off >= n_msgs) { set_err("B2_STREAM_W_FROM_MSG: no such message in the last collected batch"); return B2_E_INVAL; }
-            const b2_stream_msg& m = c->h_st_msgs[w.src_off];
+            if (w.src_off >= n_msgs) { set_err("B2_STREAM_W_FROM_MSG: no such message in the last collected batch (or ring ticket, when it is the most recent)"); return B2_E_INVAL; }
+            const b2_stream_msg& m = from_msgs[w.src_off];
             if ((m.flags & B2_STREAM_MSG_IN_INPUT) && !c->st_input) { set_err("B2_STREAM_W_FROM_MSG: a later call overwrote the last batch's input bytes on the device"); return B2_E_INVAL; }
-            r.src = ((m.flags & B2_STREAM_MSG_IN_INPUT) ? c->st_input : c->sp.out) + m.off; r.len = m.len;
+            r.src = ((m.flags & B2_STREAM_MSG_IN_INPUT) ? c->st_input : from_out) + m.off; r.len = m.len;
         } else {
             if ((uint64_t)w.src_off + w.src_len > nbytes) { set_err("write outside bytes"); return B2_E_INVAL; }
             r.src = d_in + w.src_off; r.len = w.src_len;
@@ -990,6 +1028,23 @@ extern "C" int b2_stream_write(b2_ctx* c, const void* bytes, uint32_t nbytes, co
     return B2_OK;
 }
 
+extern "C" int b2_stream_ring_enable(b2_ctx* c, uint32_t out_bytes) {
+    if (!c || !c->has_streams) { set_err("no stream table (b2_stream_configure)"); return B2_E_INVAL; }
+    if (c->st_ring || c->ring_slots) { set_err("b2_stream_ring_enable: once, before the context's first ring call"); return B2_E_INVAL; }
+    if (out_bytes > (256u << 20)) { set_err("out_bytes above 256 MiB"); return B2_E_CAPACITY; }
+    CU(cudaSetDevice(c->opt.device));
+    CU(cudaStreamSynchronize(c->stream));
+    if (cudaMalloc((void**)&c->d_st_ring, (size_t)kSecOut + ((out_bytes + 15u) & ~15u) + 16) != cudaSuccess) { cudaGetLastError(); set_err("cudaMalloc of the ring's stream staging failed"); return B2_E_NOMEM; }
+    CU(cudaMemset(c->sp.cnts, 0, 4 * (16 + 2 * (size_t)c->sp.cap)));         // counters | cnt | fill: the ring's tickets start from zeros
+    StreamPass R = c->sp;                   // table, pool and scratch shared with the batch calls; results and counters its own
+    R.cnts = reinterpret_cast<uint32_t*>(c->d_st_ring);
+    R.events = reinterpret_cast<b2_stream_event*>(c->d_st_ring + kSecEvents); R.msgs = reinterpret_cast<b2_stream_msg*>(c->d_st_ring + kSecMsgs);
+    R.ctrl = c->d_st_ring + kSecCtrl; R.run_ctrl = reinterpret_cast<uint32_t*>(c->d_st_ring + kSecRunCtrl);
+    R.out = c->d_st_ring + kSecOut; R.out_cap = out_bytes;
+    c->sp_ring = R; c->st_ring = true;
+    return B2_OK;
+}
+
 // ---- the persistent latency path: submit ring + resident kernel (k_ring) ---------------------------------------------------------
 static void ring_halt(b2_ctx* c) {
     if (!c->ring_ctl) return;
@@ -1000,7 +1055,7 @@ static void ring_halt(b2_ctx* c) {
 static int ring_launch(b2_ctx* c) {
     RingDev R;
     R.slots = c->ring_slots; R.slot_stride = c->ring_stride; R.off_runs = c->ring_off_runs; R.off_in = c->ring_off_in; R.off_out = c->ring_off_out;
-    R.ctl = c->ring_ctl; R.next_ticket = c->d_ring_ticket;
+    R.ctl = c->ring_ctl; R.next_ticket = c->d_ring_ticket; R.off_st = c->ring_off_st;
     unsigned long long idle_ms = 20; if (const char* e = getenv("B2_RING_IDLE_MS")) idle_ms = (unsigned long long)atoi(e);
     R.idle_ns = idle_ms * 1000000ull;
     R.d_bytes = c->d_bytes; R.d_meta = c->d_meta; R.d_small = c->d_small;
@@ -1009,7 +1064,9 @@ static int ring_launch(b2_ctx* c) {
     c->small = was_small;
     B.bytes = c->d_bytes;
     c->ring_ctl[1] = 1; __sync_synchronize();
-    k_ring<<<1, kSmallThreads, sizeof(SmallSmem), c->ring_stream>>>(R, B, c->cfg);
+    StreamPass SP = {};                     // (tab null: the ring runs no stream pass)
+    if (c->st_ring) SP = c->sp_ring;
+    k_ring<<<1, kSmallThreads, sizeof(SmallSmem), c->ring_stream>>>(R, B, c->cfg, SP);
     c->ring_launches++;
     CU(cudaGetLastError());
     return B2_OK;
@@ -1021,13 +1078,15 @@ extern "C" int b2_ring_start(b2_ctx* c) {
         c->ring_off_runs = sizeof(RingSlotHdr);
         c->ring_off_in = (c->ring_off_runs + kSmallRuns * (uint32_t)sizeof(b2_run) + 255u) & ~255u;
         c->ring_off_out = (c->ring_off_in + kSmallBytes + 1024u + 255u) & ~255u;
-        c->ring_stride = (uint32_t)((c->ring_off_out + kSmallBlock + 4095u) & ~4095u);
+        c->ring_off_st = (c->ring_off_out + kSmallBlock + 255u) & ~255u;
+        const uint64_t end = c->st_ring ? (uint64_t)c->ring_off_st + kSecOut + ((c->sp_ring.out_cap + 15u) & ~15u) : (uint64_t)c->ring_off_out + kSmallBlock;
+        c->ring_stride = (uint32_t)((end + 4095u) & ~4095ull);
         CU(cudaHostAlloc((void**)&c->ring_slots, (size_t)c->ring_stride * kRingSlots, cudaHostAllocMapped | cudaHostAllocPortable));
         memset(c->ring_slots, 0, (size_t)c->ring_stride * kRingSlots);
         CU(cudaHostAlloc((void**)&c->ring_ctl, 64, cudaHostAllocMapped | cudaHostAllocPortable));
         memset((void*)c->ring_ctl, 0, 64);
-        CU(cudaMalloc((void**)&c->d_ring_ticket, 4));
-        const uint32_t one = 1; CU(cudaMemcpy(c->d_ring_ticket, &one, 4, cudaMemcpyHostToDevice));
+        CU(cudaMalloc((void**)&c->d_ring_ticket, 8));
+        const uint32_t init[2] = { 1, 0 }; CU(cudaMemcpy(c->d_ring_ticket, init, 8, cudaMemcpyHostToDevice));
         CU(cudaStreamCreateWithFlags(&c->ring_stream, cudaStreamNonBlocking));
         CU(cudaFuncSetAttribute(k_ring, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmallSmem)));
     }
@@ -1038,7 +1097,7 @@ extern "C" int b2_ring_stop(b2_ctx* c) { if (!c) return B2_E_INVAL; cudaSetDevic
 
 extern "C" int b2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs, uint32_t* ticket) {
     if (!c || !bytes || !runs || !ticket || n_runs == 0) { set_err("null argument"); return B2_E_INVAL; }
-    if (c->has_streams) { set_err("the ring path does not run the stream pass: use b2_batch_submit on a context with a stream table"); return B2_E_INVAL; }
+    if (c->has_streams && !c->st_ring) { set_err("the ring path runs the stream pass only after b2_stream_ring_enable: use b2_batch_submit on a context with a stream table"); return B2_E_INVAL; }
     if (nbytes > kSmallBytes || n_runs > kSmallRuns) { set_err("b2_ring_submit serves batches up to 128 KiB / 512 runs: use b2_batch_submit"); return B2_E_CAPACITY; }
     if (!c->ring_slots) { int rc = b2_ring_start(c); if (rc != B2_OK) return rc; }
     const uint32_t t = c->ring_next, si = t % kRingSlots;
@@ -1078,6 +1137,7 @@ extern "C" int b2_ring_wait(b2_ctx* c, uint32_t ticket, b2_batch_result* out) {
     uint8_t* slot = c->ring_slots + (size_t)si * c->ring_stride;
     RingSlotHdr* h = reinterpret_cast<RingSlotHdr*>(slot);
     if (c->ring_collected[si]) { set_err("ticket already collected"); return B2_E_INVAL; }
+    if (c->st_ring && ticket != c->ring_next_wait) { set_err("a context whose ring runs the stream pass collects its tickets in ticket order"); return B2_E_INVAL; }
     uint64_t spins = 0;
     while (h->done != ticket) {
 #if defined(__x86_64__)
@@ -1091,9 +1151,21 @@ extern "C" int b2_ring_wait(b2_ctx* c, uint32_t ticket, b2_batch_result* out) {
     }
     __sync_synchronize();
     c->ring_collected[si] = true;
+    if (c->st_ring) c->ring_next_wait = ticket + 1;
     memset(out, 0, sizeof *out);
     const uint8_t* ob = slot + c->ring_off_out;
     const uint32_t* tot = reinterpret_cast<const uint32_t*>(ob);
+    if ((tot[2] & 3u) && c->st_ring) {
+        // k_ring ran no stream pass for this ticket and parks before the next one's pull: the big pipeline serves the ticket (its own
+        // stream pass included) while the kernel waits, then ctl[3] releases it — the table sees the tickets in ticket order
+        const bool allow = c->allow_small; c->allow_small = false;
+        const int rc = b2_process_batch(c, c->ring_bytes[si], h->nbytes, reinterpret_cast<const b2_run*>(slot + c->ring_off_runs), h->n_runs, out);
+        c->allow_small = allow;
+        __sync_synchronize();
+        c->ring_ctl[3] = ticket;
+        __sync_synchronize();
+        return rc;
+    }
     if (tot[2] & 3u) {
         // more messages / reply bytes than the compact block holds: the big pipeline serves this batch (after the ring is quiet)
         for (uint32_t k = 0; k < kRingSlots; k++) if (!c->ring_collected[k]) { set_err("ring overflow fallback needs the other tickets collected first"); return B2_E_CAPACITY; }
@@ -1109,6 +1181,7 @@ extern "C" int b2_ring_wait(b2_ctx* c, uint32_t ticket, b2_batch_result* out) {
     out->refs = h->by_ref ? reinterpret_cast<const b2_resp_ref*>(ob + h->off_refs) : nullptr;
     if (c->resp_mode == B2_RESP_IOVEC) refs_to_iov(c, out, c->ring_bytes[si]);
     out->n_launches = 0; out->kernel_ms = 0.f;
+    if (c->st_ring) { c->stream_valid = true; c->st_view_ticket = ticket; c->st_input = c->d_bytes; }
     if (out->n_msgs) { const uint32_t now = h->nbytes / out->n_msgs; c->avg_frame = c->avg_frame ? (uint32_t)(((uint64_t)c->avg_frame * 3 + now) / 4) : now; }
     return B2_OK;
 }

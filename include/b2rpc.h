@@ -335,7 +335,12 @@ int  b2_batch_collect(b2_ctx* ctx, b2_batch_result* out);
  * submissions.  The kernel retires after 20 ms without work (B2_RING_IDLE_MS) so that it never blocks device-wide
  * synchronisation for long, and comes back with the next submission.  A batch whose results do not fit the compact block is
  * served by the big pipeline inside b2_ring_wait (needs every other ticket collected).  Not to be mixed with concurrent
- * batch calls on the same context. */
+ * batch calls on the same context.
+ * With a stream table and b2_stream_ring_enable the ring also runs the stream pass (below) after each ticket's batch, in the same
+ * kernel, and each slot carries the ticket's stream results.  On such a context tickets are collected in ticket order
+ * (b2_ring_wait of any other ticket fails with B2_E_INVAL), and a ticket that overflows the compact block keeps its place: the
+ * kernel runs no pass for it and parks before the next ticket until b2_ring_wait has served it through the big pipeline (stream
+ * pass included) and released the kernel through a control word; the tickets behind it need not be collected first. */
 int  b2_ring_start(b2_ctx* ctx);
 int  b2_ring_stop(b2_ctx* ctx);
 int  b2_ring_submit(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs, uint32_t* ticket);
@@ -786,7 +791,8 @@ int  b2_h2_serve_batch(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2
  * (handover_msg), the parts gathered in earlier batches are fetched once with b2_stream_take_pending, and from then on the stream's
  * frames are described per frame only (no routing, no RST) until b2_stream_close.
  * Not modelled: _parse_rpc_response (open a client stream after the host took the RPC response), idle timers, messages_in_batch.
- * The ring path does not run the pass: b2_ring_submit fails with B2_E_INVAL on a context that has a table.  The measurement entry
+ * The ring path runs the pass only after b2_stream_ring_enable (below); without it b2_ring_submit fails with B2_E_INVAL on a context
+ * that has a table.  The measurement entry
  * points (b2_batch_execute, b2_batch_execute_many, b2_batch_launch) do not run it either: they replay one batch, and fail with
  * B2_E_INVAL between b2_batch_submit and b2_batch_collect on a context with a table.  When one batch completes more multi-frame bytes
  * than the out region holds, WHICH of the competing streams is handed over is unspecified (room is handed out as the warps ask). */
@@ -859,6 +865,18 @@ int  b2_stream_query(b2_ctx* ctx, int64_t stream_id, b2_stream_state* out);
 /* The partial message of a stream (a HANDED_OVER one hands it out this way), at most cap bytes; it is gone from the device afterwards. */
 int  b2_stream_take_pending(b2_ctx* ctx, int64_t stream_id, void* out, uint32_t cap, uint32_t* len);
 int  b2_stream_results(b2_ctx* ctx, b2_stream_batch_result* out);
+/* The stream pass on the latency path: after b2_stream_configure and before the context's first ring call (later, or twice:
+ * B2_E_INVAL).  k_ring then runs the pass of every ticket on the same table, with the same rules and results as a batch call.
+ * out_bytes: the reassembled multi-frame bytes one ticket may complete (a ticket that completes more hands streams over by the rule
+ * above; the batch calls keep b2_stream_configure's out region).  After b2_ring_wait(t), b2_stream_results describes ticket t: pointers
+ * into the slot's stream section, valid until the slot is reused by the 8th later submission (or, for a ticket that overflowed the
+ * compact block, the batch call's results, valid until the next call).  While a ticket is outstanding, b2_stream_open / _set_connected /
+ * _close / _take_pending and b2_stream_write fail with B2_E_INVAL and leave the table untouched; between tickets they work as always.
+ * B2_STREAM_W_FROM_MSG after ring tickets resolves against the ticket b2_stream_results describes, and only while that is the most
+ * recent ticket: its B2_STREAM_MSG_IN_INPUT messages are read from the ring's device copy of its input and its out-region messages from
+ * the ring's device out region, both overwritten by the next ticket; otherwise every FROM_MSG index fails with B2_E_INVAL.  The table,
+ * the pool and the pending messages live in device memory and survive the kernel's idle retirement and relaunch unchanged. */
+int  b2_stream_ring_enable(b2_ctx* ctx, uint32_t out_bytes);
 
 /* ---- streaming_rpc, the sending side of a Stream on the device ---------------------------------------------------------------------
  * b2_stream_write: brpc::StreamWrite (src/brpc/stream.cpp:782-794) for a batch of writes against the stream table, applied in array
