@@ -89,6 +89,14 @@ class BatchResult(C.Structure):
                 ("kernel_ms", C.c_float), ("n_launches", C.c_uint32), ("refs", C.c_void_p), ("iov", C.c_void_p)]
 
 
+class H2RingResult(C.Structure):
+    _fields_ = [("runs", C.c_void_p), ("n_runs", C.c_uint32), ("n_msgs", C.c_uint32), ("msgs", C.c_void_p), ("out", C.c_void_p),
+                ("region", C.c_uint32), ("replies", C.c_void_p), ("spans", C.c_void_p), ("status", C.c_int32)]
+
+
+assert C.sizeof(H2RingResult) == 64
+
+
 class StreamState(C.Structure):
     _fields_ = [("local_consumed", C.c_uint64), ("remote_consumed", C.c_uint64), ("pending_bytes", C.c_uint32), ("flags", C.c_uint32),
                 ("error_code", C.c_int32), ("reserved", C.c_uint32)]
@@ -176,6 +184,9 @@ def _load():
     l.b2_h2_conn_set_gunzip.argtypes = [C.c_void_p, C.c_uint32, C.c_int]
     l.b2_h2_serve_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32,
                                     C.POINTER(C.c_uint32), C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p]
+    l.b2_h2_ring_enable.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]
+    l.b2_h2_ring_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
+    l.b2_h2_ring_wait.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(H2RingResult)]
     l.b2_h2_pack_responses.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     l.b2_pack_requests.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     l.b2_pack_responses.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
@@ -203,7 +214,8 @@ ABI_SYMBOLS = ["b2_ctx_create", "b2_ctx_destroy", "b2_last_error", "b2_version",
                "b2_counters_device_ptr", "b2_counters_allreduce", "b2_h2_pack_requests", "b2_h2_conn_set_next_stream_id", "b2_h2_conn_peer_update",
                "b2_h2_client_conn_reset", "b2_h2_client_process_batch", "b2_h2_client_abandon_streams", "b2_h2_conn_set_gunzip",
                "b2_h2_serve_batch", "b2_stream_configure", "b2_stream_open", "b2_stream_set_connected", "b2_stream_close", "b2_stream_query",
-               "b2_stream_take_pending", "b2_stream_results", "b2_stream_write", "b2_stream_ring_enable"]
+               "b2_stream_take_pending", "b2_stream_results", "b2_stream_write", "b2_stream_ring_enable", "b2_h2_ring_enable", "b2_h2_ring_submit",
+               "b2_h2_ring_wait"]
 
 ECHO_METHOD = dict(service_full_name=b"example.EchoService", service_name=b"EchoService", method_name=b"Echo",
                    request_type_name=b"example.EchoRequest", handler=1, echo_attachment=1,
@@ -653,6 +665,38 @@ class Context:
         _check(lib.b2_h2_serve_batch(self._h, data.ctypes.data, data.nbytes, runs.ctypes.data, n, rs.ctypes.data, msgs.ctypes.data, msg_cap,
                                      C.byref(nm), out.ctypes.data, out.nbytes, replies.ctypes.data, replies.nbytes, spans.ctypes.data))
         return rs, msgs[:nm.value], out, replies, spans
+
+    # ---- h2/gRPC on the latency path (b2_h2_ring_*) ----
+    def h2_ring_enable(self, max_bytes, msg_cap, out_cap, replies_cap):
+        """Serve h2 batches on the resident k_h2_ring with these per-ticket caps (b2_h2_ring_enable): after h2_configure, before the first
+        ring call."""
+        _check(lib.b2_h2_ring_enable(self._h, max_bytes, msg_cap, out_cap, replies_cap))
+
+    def h2_ring_submit(self, data, runs, ptr=None, nbytes=None):
+        """One batch of server connection runs (runs[i].socket_id = connection).  Returns the ticket."""
+        runs = np.ascontiguousarray(runs, dtype=RUN_DT)
+        if ptr is None:
+            data = np.ascontiguousarray(data, dtype=np.uint8); ptr, nbytes = data.ctypes.data, data.nbytes
+            self._ring_keep = data
+        t = C.c_uint32(0)
+        _check(lib.b2_h2_ring_submit(self._h, ptr, nbytes, runs.ctypes.data, len(runs), C.byref(t)))
+        return t.value
+
+    def h2_ring_wait(self, ticket):
+        """(run_status, msgs, out, replies, spans) of the ticket, as h2_serve_batch returns them: views of the ticket's pinned slot, valid
+        until the slot is reused by the 8th later submission.  out covers n_runs * region bytes, replies every span."""
+        res = H2RingResult()
+        _check(lib.b2_h2_ring_wait(self._h, ticket, C.byref(res)))
+        if res.status < 0:
+            raise B2Error(res.status, "h2 ring ticket %d" % ticket)
+
+        def view(ptr, nbytes, dt=np.uint8):
+            return np.ctypeslib.as_array((C.c_uint8 * nbytes).from_address(ptr)).view(dt) if nbytes else np.zeros(0, dt)
+        n = res.n_runs
+        spans = view(res.spans, 16 * n, H2_REPLY_SPAN_DT)
+        rep_end = int((spans["off"].astype(np.int64) + spans["len"]).max()) if n else 0
+        return (view(res.runs, 32 * n, H2_RUN_STATUS_DT), view(res.msgs, 64 * res.n_msgs, H2_MSG_DT), view(res.out, res.region * n),
+                view(res.replies, rep_end), spans)
 
     def pack_requests(self, data, reqs, out_cap=None):
         """reqs: REQUEST_DT array (offsets into data).  Returns the packed frame of every request (b"" = rejected)."""

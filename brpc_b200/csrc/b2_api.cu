@@ -58,6 +58,10 @@ struct b2_ctx {
     // to the slot's section at ring_off_st; tickets are collected in order (ring_next_wait); st_view_ticket: the ticket b2_stream_results
     // describes (0: the last batch call's pass)
     bool st_ring = false; StreamPass sp_ring = {}; uint8_t* d_st_ring = nullptr; uint32_t ring_off_st = 0, ring_next_wait = 1, st_view_ticket = 0;
+    // h2/gRPC on the ring (b2_h2_ring_enable): the context runs k_h2_ring instead of k_ring.  The caps every ticket is served with, and the
+    // parts of a slot behind its header, runs and staged input
+    bool h2_ring = false; uint32_t h2r_max_bytes = 0, h2r_msg_cap = 0, h2r_out_cap = 0, h2r_replies_cap = 0;
+    uint32_t h2r_off_args = 0, h2r_off_rs = 0, h2r_off_msgs = 0, h2r_off_spans = 0, h2r_off_out = 0, h2r_off_replies = 0;
     ulonglong2* d_iov = nullptr; b2_iovec* h_iov = nullptr; const void* host_bytes = nullptr;      // B2_RESP_IOVEC
     uint4* d_refs = nullptr; b2_resp_ref* h_refs = nullptr; int input_mode = B2_INPUT_COPY, resp_mode = B2_RESP_COPY; const uint8_t* pull_bytes = nullptr; uint32_t small_off_refs = 0;
     uint32_t* d_crc_adv = nullptr; unsigned long long* d_counters = nullptr; uint32_t* d_totals = nullptr; DevMethod* d_methods = nullptr;
@@ -161,6 +165,15 @@ extern "C" uint64_t b2_block_pool_host_allocs(void) { std::lock_guard<std::mutex
 
 static void ring_halt(b2_ctx* c);
 static void stream_free(b2_ctx* c);
+// Every call that uploads to the context or touches h2 state is refused while an h2 ring ticket is outstanding: the ticket uses the same
+// device scratch and connection state.  A call that writes h2 connection state also retires k_h2_ring first: the resident CTA reads that
+// state through L1, and a launch boundary is where L1 is known not to hold lines another kernel wrote since.
+static bool h2_ring_refuses(b2_ctx* c, bool writes_h2_state) {
+    if (!c->h2_ring) return false;
+    for (uint32_t k = 0; k < kRingSlots; k++) if (!c->ring_collected[k]) { set_err("an h2 ring ticket is outstanding: b2_h2_ring_wait it first"); return true; }
+    if (writes_h2_state) ring_halt(c);
+    return false;
+}
 extern "C" void b2_ctx_destroy(b2_ctx* c) {
     if (!c) return;
     cudaSetDevice(c->opt.device);
@@ -285,6 +298,7 @@ extern "C" int b2_ctx_create(const b2_options* o, b2_ctx** out) {
 
 extern "C" int b2_set_server_identity(b2_ctx* c, const char* ip_port) {
     if (!c) return B2_E_INVAL;
+    if (h2_ring_refuses(c, true)) return B2_E_INVAL;              // (the identity is a launch argument of k_h2_ring)
     const size_t n = ip_port ? strlen(ip_port) : 0;
     if (n >= sizeof c->cfg.identity) { set_err("identity too long"); return B2_E_INVAL; }
     memset(c->cfg.identity, 0, sizeof c->cfg.identity);
@@ -380,6 +394,7 @@ static BatchPtrs make_ptrs(b2_ctx* c) {
 
 extern "C" int b2_batch_upload(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs) {
     if (!c || (!bytes && nbytes) || (!runs && n_runs)) { set_err("null argument"); return B2_E_INVAL; }
+    if (h2_ring_refuses(c, false)) return B2_E_INVAL;
     // (B2_INPUT_PULL: `bytes` is the caller's whole pinned arena and nothing is copied — what is bounded is the bytes the runs cover)
     if ((c->input_mode != B2_INPUT_PULL && nbytes > c->opt.max_batch_bytes) || nbytes >= (1u << 31) || n_runs > c->opt.max_runs) { set_err("batch exceeds ctx capacity"); return B2_E_CAPACITY; }
     uint64_t covered = 0; for (uint32_t r = 0; r < n_runs; r++) covered += runs[r].length;
@@ -944,7 +959,7 @@ extern "C" int b2_stream_write(b2_ctx* c, const void* bytes, uint32_t nbytes, co
     static_assert(sizeof(b2_stream_write_desc) == 24 && sizeof(b2_stream_write_result) == 32 && sizeof(SwRec) == 24, "stream write ABI layout");
     if (!c || !c->has_streams || (!bytes && nbytes) || (!writes && n) || (!results && n) || (!out && out_cap)) { set_err("no stream table (b2_stream_configure) or null argument"); return B2_E_INVAL; }
     if (c->stream_armed) { set_err("a submitted batch must be collected first: the stream table belongs to it"); return B2_E_INVAL; }
-    if (ring_owns_table(c)) return B2_E_INVAL;
+    if (ring_owns_table(c) || h2_ring_refuses(c, false)) return B2_E_INVAL;
     if (n > c->opt.max_msgs || nbytes > c->opt.max_batch_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     CU(cudaSetDevice(c->opt.device));
     const uint64_t seg = max_segment_size ? max_segment_size : 512ull << 20;       // -stream_write_max_segment_size (stream.cpp:39)
@@ -1030,7 +1045,7 @@ extern "C" int b2_stream_write(b2_ctx* c, const void* bytes, uint32_t nbytes, co
 
 extern "C" int b2_stream_ring_enable(b2_ctx* c, uint32_t out_bytes) {
     if (!c || !c->has_streams) { set_err("no stream table (b2_stream_configure)"); return B2_E_INVAL; }
-    if (c->st_ring || c->ring_slots) { set_err("b2_stream_ring_enable: once, before the context's first ring call"); return B2_E_INVAL; }
+    if (c->st_ring || c->ring_slots || c->h2_ring) { set_err("b2_stream_ring_enable: once, before the context's first ring call"); return B2_E_INVAL; }
     if (out_bytes > (256u << 20)) { set_err("out_bytes above 256 MiB"); return B2_E_CAPACITY; }
     CU(cudaSetDevice(c->opt.device));
     CU(cudaStreamSynchronize(c->stream));
@@ -1052,6 +1067,8 @@ static void ring_halt(b2_ctx* c) {
     cudaStreamSynchronize(c->ring_stream);
     c->ring_ctl[0] = 0; c->ring_ctl[1] = 0; __sync_synchronize();
 }
+static H2RingDev h2_ring_dev(const b2_ctx* c);
+// (re)launches the context's resident kernel: k_h2_ring after b2_h2_ring_enable, else k_ring
 static int ring_launch(b2_ctx* c) {
     RingDev R;
     R.slots = c->ring_slots; R.slot_stride = c->ring_stride; R.off_runs = c->ring_off_runs; R.off_in = c->ring_off_in; R.off_out = c->ring_off_out;
@@ -1059,6 +1076,14 @@ static int ring_launch(b2_ctx* c) {
     unsigned long long idle_ms = 20; if (const char* e = getenv("B2_RING_IDLE_MS")) idle_ms = (unsigned long long)atoi(e);
     R.idle_ns = idle_ms * 1000000ull;
     R.d_bytes = c->d_bytes; R.d_meta = c->d_meta; R.d_small = c->d_small;
+    if (c->h2_ring) {
+        const H2RingDev H = h2_ring_dev(c);
+        c->ring_ctl[1] = 1; __sync_synchronize();
+        k_h2_ring<<<1, kSmallThreads, kH2RingSmem, c->ring_stream>>>(R, H);
+        c->ring_launches++;
+        CU(cudaGetLastError());
+        return B2_OK;
+    }
     const bool was_small = c->small; c->small = false;
     BatchPtrs B = make_ptrs(c);
     c->small = was_small;
@@ -1071,6 +1096,20 @@ static int ring_launch(b2_ctx* c) {
     CU(cudaGetLastError());
     return B2_OK;
 }
+// the kRingSlots slots of `end` bytes each (pinned + mapped), the control words, the ticket counter and the ring stream: once per context,
+// for whichever resident kernel it runs
+static int ring_alloc(b2_ctx* c, uint64_t end) {
+    if (end > (1ull << 31)) { set_err("ring slot too large: lower the capacities"); return B2_E_CAPACITY; }
+    c->ring_stride = (uint32_t)((end + 4095u) & ~4095ull);
+    CU(cudaHostAlloc((void**)&c->ring_slots, (size_t)c->ring_stride * kRingSlots, cudaHostAllocMapped | cudaHostAllocPortable));
+    memset(c->ring_slots, 0, (size_t)c->ring_stride * kRingSlots);
+    CU(cudaHostAlloc((void**)&c->ring_ctl, 64, cudaHostAllocMapped | cudaHostAllocPortable));
+    memset((void*)c->ring_ctl, 0, 64);
+    CU(cudaMalloc((void**)&c->d_ring_ticket, 8));
+    const uint32_t init[2] = { 1, 0 }; CU(cudaMemcpy(c->d_ring_ticket, init, 8, cudaMemcpyHostToDevice));
+    CU(cudaStreamCreateWithFlags(&c->ring_stream, cudaStreamNonBlocking));
+    return B2_OK;
+}
 extern "C" int b2_ring_start(b2_ctx* c) {
     if (!c) return B2_E_INVAL;
     CU(cudaSetDevice(c->opt.device));
@@ -1080,33 +1119,15 @@ extern "C" int b2_ring_start(b2_ctx* c) {
         c->ring_off_out = (c->ring_off_in + kSmallBytes + 1024u + 255u) & ~255u;
         c->ring_off_st = (c->ring_off_out + kSmallBlock + 255u) & ~255u;
         const uint64_t end = c->st_ring ? (uint64_t)c->ring_off_st + kSecOut + ((c->sp_ring.out_cap + 15u) & ~15u) : (uint64_t)c->ring_off_out + kSmallBlock;
-        c->ring_stride = (uint32_t)((end + 4095u) & ~4095ull);
-        CU(cudaHostAlloc((void**)&c->ring_slots, (size_t)c->ring_stride * kRingSlots, cudaHostAllocMapped | cudaHostAllocPortable));
-        memset(c->ring_slots, 0, (size_t)c->ring_stride * kRingSlots);
-        CU(cudaHostAlloc((void**)&c->ring_ctl, 64, cudaHostAllocMapped | cudaHostAllocPortable));
-        memset((void*)c->ring_ctl, 0, 64);
-        CU(cudaMalloc((void**)&c->d_ring_ticket, 8));
-        const uint32_t init[2] = { 1, 0 }; CU(cudaMemcpy(c->d_ring_ticket, init, 8, cudaMemcpyHostToDevice));
-        CU(cudaStreamCreateWithFlags(&c->ring_stream, cudaStreamNonBlocking));
+        int rc = ring_alloc(c, end); if (rc != B2_OK) return rc;
         CU(cudaFuncSetAttribute(k_ring, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmallSmem)));
     }
     if (!c->ring_ctl[1]) return ring_launch(c);
     return B2_OK;
 }
-extern "C" int b2_ring_stop(b2_ctx* c) { if (!c) return B2_E_INVAL; cudaSetDevice(c->opt.device); ring_halt(c); return B2_OK; }
-
-extern "C" int b2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs, uint32_t* ticket) {
-    if (!c || !bytes || !runs || !ticket || n_runs == 0) { set_err("null argument"); return B2_E_INVAL; }
-    if (c->has_streams && !c->st_ring) { set_err("the ring path runs the stream pass only after b2_stream_ring_enable: use b2_batch_submit on a context with a stream table"); return B2_E_INVAL; }
-    if (nbytes > kSmallBytes || n_runs > kSmallRuns) { set_err("b2_ring_submit serves batches up to 128 KiB / 512 runs: use b2_batch_submit"); return B2_E_CAPACITY; }
-    if (!c->ring_slots) { int rc = b2_ring_start(c); if (rc != B2_OK) return rc; }
-    const uint32_t t = c->ring_next, si = t % kRingSlots;
-    if (!c->ring_collected[si]) { set_err("submit ring full: b2_ring_wait the oldest ticket first"); return B2_E_CAPACITY; }
-    for (uint32_t r = 0; r < n_runs; r++)
-        if ((runs[r].offset & 15u) || (uint64_t)runs[r].offset + runs[r].length > nbytes) { set_err("run offset must be 16-aligned and inside the batch"); return B2_E_INVAL; }
-    uint8_t* slot = c->ring_slots + (size_t)si * c->ring_stride;
-    RingSlotHdr* h = reinterpret_cast<RingSlotHdr*>(slot);
-    // the batch bytes: in place when they already live in pinned + mapped memory (b2_block_alloc), else staged into the slot
+// the batch bytes as the kernel pulls them: in place when they already live in pinned + mapped memory (b2_block_alloc), else staged into
+// the slot at ring_off_in
+static unsigned long long ring_stage(b2_ctx* c, uint8_t* slot, const void* bytes, uint32_t nbytes) {
     unsigned long long dev = 0;
     if (bytes == c->ring_pin_base) dev = c->ring_pin_dev;
     else {
@@ -1116,12 +1137,10 @@ extern "C" int b2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, con
         } else cudaGetLastError();
     }
     if (!dev) { memcpy(slot + c->ring_off_in, bytes, nbytes); dev = (unsigned long long)(uintptr_t)(slot + c->ring_off_in); }
-    memcpy(slot + c->ring_off_runs, runs, sizeof(b2_run) * (size_t)n_runs);
-    uint32_t mb = nbytes / 12 + 1; if (mb > kSmallMsgs) mb = kSmallMsgs; if (mb > c->opt.max_msgs) mb = c->opt.max_msgs;
-    h->n_runs = n_runs; h->nbytes = nbytes; h->small_msgs = mb; h->small_resp = nbytes + mb * 80 + 2048;
-    h->off_rs = 64; h->off_msgs = 64 + n_runs * 32; h->off_refs = h->off_msgs + mb * 64; h->off_resp = (h->off_refs + mb * 16 + 255u) & ~255u;
-    h->total = h->off_resp + h->small_resp; h->by_ref = c->cfg.by_ref; h->bytes_dev = dev;
-    c->ring_bytes[si] = bytes; c->ring_collected[si] = false;
+    return dev;
+}
+// rings the doorbell of ticket t in its slot (everything else the host stores there first) and relaunches the kernel if it idled out
+static int ring_ring(b2_ctx* c, RingSlotHdr* h, uint32_t t, uint32_t* ticket) {
     __sync_synchronize();
     h->submit = t;
     __sync_synchronize();
@@ -1130,14 +1149,8 @@ extern "C" int b2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, con
     if (!c->ring_ctl[1]) { CU(cudaSetDevice(c->opt.device)); return ring_launch(c); }   // the kernel idled out (or was never started)
     return B2_OK;
 }
-
-extern "C" int b2_ring_wait(b2_ctx* c, uint32_t ticket, b2_batch_result* out) {
-    if (!c || !out || !c->ring_slots || ticket == 0 || ticket >= c->ring_next || ticket + kRingSlots < c->ring_next) { set_err("bad ring ticket"); return B2_E_INVAL; }
-    const uint32_t si = ticket % kRingSlots;
-    uint8_t* slot = c->ring_slots + (size_t)si * c->ring_stride;
-    RingSlotHdr* h = reinterpret_cast<RingSlotHdr*>(slot);
-    if (c->ring_collected[si]) { set_err("ticket already collected"); return B2_E_INVAL; }
-    if (c->st_ring && ticket != c->ring_next_wait) { set_err("a context whose ring runs the stream pass collects its tickets in ticket order"); return B2_E_INVAL; }
+// spins until the kernel released `ticket`; starts the kernel again when it lost the exit race with the submission
+static int ring_spin(b2_ctx* c, const RingSlotHdr* h, uint32_t ticket) {
     uint64_t spins = 0;
     while (h->done != ticket) {
 #if defined(__x86_64__)
@@ -1150,6 +1163,41 @@ extern "C" int b2_ring_wait(b2_ctx* c, uint32_t ticket, b2_batch_result* out) {
         }
     }
     __sync_synchronize();
+    return B2_OK;
+}
+extern "C" int b2_ring_stop(b2_ctx* c) { if (!c) return B2_E_INVAL; cudaSetDevice(c->opt.device); ring_halt(c); return B2_OK; }
+
+extern "C" int b2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs, uint32_t* ticket) {
+    if (!c || !bytes || !runs || !ticket || n_runs == 0) { set_err("null argument"); return B2_E_INVAL; }
+    if (c->has_streams && !c->st_ring) { set_err("the ring path runs the stream pass only after b2_stream_ring_enable: use b2_batch_submit on a context with a stream table"); return B2_E_INVAL; }
+    if (c->h2_ring) { set_err("this context's ring serves h2 (b2_h2_ring_enable): use b2_h2_ring_submit"); return B2_E_INVAL; }
+    if (nbytes > kSmallBytes || n_runs > kSmallRuns) { set_err("b2_ring_submit serves batches up to 128 KiB / 512 runs: use b2_batch_submit"); return B2_E_CAPACITY; }
+    if (!c->ring_slots) { int rc = b2_ring_start(c); if (rc != B2_OK) return rc; }
+    const uint32_t t = c->ring_next, si = t % kRingSlots;
+    if (!c->ring_collected[si]) { set_err("submit ring full: b2_ring_wait the oldest ticket first"); return B2_E_CAPACITY; }
+    for (uint32_t r = 0; r < n_runs; r++)
+        if ((runs[r].offset & 15u) || (uint64_t)runs[r].offset + runs[r].length > nbytes) { set_err("run offset must be 16-aligned and inside the batch"); return B2_E_INVAL; }
+    uint8_t* slot = c->ring_slots + (size_t)si * c->ring_stride;
+    RingSlotHdr* h = reinterpret_cast<RingSlotHdr*>(slot);
+    const unsigned long long dev = ring_stage(c, slot, bytes, nbytes);
+    memcpy(slot + c->ring_off_runs, runs, sizeof(b2_run) * (size_t)n_runs);
+    uint32_t mb = nbytes / 12 + 1; if (mb > kSmallMsgs) mb = kSmallMsgs; if (mb > c->opt.max_msgs) mb = c->opt.max_msgs;
+    h->n_runs = n_runs; h->nbytes = nbytes; h->small_msgs = mb; h->small_resp = nbytes + mb * 80 + 2048;
+    h->off_rs = 64; h->off_msgs = 64 + n_runs * 32; h->off_refs = h->off_msgs + mb * 64; h->off_resp = (h->off_refs + mb * 16 + 255u) & ~255u;
+    h->total = h->off_resp + h->small_resp; h->by_ref = c->cfg.by_ref; h->bytes_dev = dev;
+    c->ring_bytes[si] = bytes; c->ring_collected[si] = false;
+    return ring_ring(c, h, t, ticket);
+}
+
+extern "C" int b2_ring_wait(b2_ctx* c, uint32_t ticket, b2_batch_result* out) {
+    if (!c || !out || !c->ring_slots || ticket == 0 || ticket >= c->ring_next || ticket + kRingSlots < c->ring_next) { set_err("bad ring ticket"); return B2_E_INVAL; }
+    const uint32_t si = ticket % kRingSlots;
+    uint8_t* slot = c->ring_slots + (size_t)si * c->ring_stride;
+    RingSlotHdr* h = reinterpret_cast<RingSlotHdr*>(slot);
+    if (c->ring_collected[si]) { set_err("ticket already collected"); return B2_E_INVAL; }
+    if (c->st_ring && ticket != c->ring_next_wait) { set_err("a context whose ring runs the stream pass collects its tickets in ticket order"); return B2_E_INVAL; }
+    if (c->h2_ring) { set_err("this context's ring serves h2: use b2_h2_ring_wait"); return B2_E_INVAL; }
+    { int rc = ring_spin(c, h, ticket); if (rc != B2_OK) return rc; }
     c->ring_collected[si] = true;
     if (c->st_ring) c->ring_next_wait = ticket + 1;
     memset(out, 0, sizeof *out);
@@ -1282,6 +1330,7 @@ __global__ void k_crc32c_batch(const uint8_t* bytes, const uint32_t* offs, const
 extern "C" int b2_crc32c_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const uint32_t* offs, const uint32_t* lens,
                                uint32_t n, uint32_t* out) {
     if (!c || !bytes || !offs || !lens || !out) { set_err("null argument"); return B2_E_INVAL; }
+    if (h2_ring_refuses(c, false)) return B2_E_INVAL;
     if (nbytes > c->opt.max_batch_bytes || n > c->opt.max_msgs) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     for (uint32_t i = 0; i < n; i++) if ((uint64_t)offs[i] + lens[i] > nbytes) { set_err("slice outside buffer"); return B2_E_INVAL; }
     CU(cudaSetDevice(c->opt.device));
@@ -1311,6 +1360,7 @@ __global__ void k_snappy_batch(const uint8_t* bytes, const uint32_t* offs, const
 extern "C" int b2_snappy_uncompress_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const uint32_t* offs, const uint32_t* lens,
                                           uint32_t n, void* out, uint32_t out_cap, uint32_t* out_offs, int32_t* out_lens) {
     if (!c || !bytes || !offs || !lens || !out || !out_offs || !out_lens) { set_err("null argument"); return B2_E_INVAL; }
+    if (h2_ring_refuses(c, false)) return B2_E_INVAL;
     if (nbytes > c->opt.max_batch_bytes || n > c->opt.max_msgs || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     // output layout from the announced lengths (the preamble varint), nothing else is read on the host
     std::vector<uint32_t> caps(n);
@@ -1356,6 +1406,7 @@ __global__ void __launch_bounds__(256) k_snappy_compress_batch(const uint8_t* by
 extern "C" int b2_snappy_compress_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const uint32_t* offs, const uint32_t* lens,
                                         uint32_t n, void* out, uint32_t out_cap, uint32_t* out_offs, uint32_t* out_lens) {
     if (!c || !bytes || !offs || !lens || !out || !out_offs || !out_lens) { set_err("null argument"); return B2_E_INVAL; }
+    if (h2_ring_refuses(c, false)) return B2_E_INVAL;
     if (nbytes > c->opt.max_batch_bytes || n > c->opt.max_msgs || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     uint64_t total = 0;
     for (uint32_t i = 0; i < n; i++) {
@@ -1449,6 +1500,7 @@ extern "C" int b2_snappy_raw_uncompress(const char* compressed, size_t compresse
 
 extern "C" int b2_hpack_reset(b2_ctx* c, uint32_t conn, uint32_t max_table_size) {
     if (!c || conn >= B2_HPACK_MAX_CONNS || max_table_size > 4096) { set_err("bad connection / table size"); return B2_E_INVAL; }
+    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
     CU(cudaSetDevice(c->opt.device));
     k_hpack_reset<<<1, 1, 0, c->stream>>>(c->d_hpack, conn, max_table_size);
     CU(cudaStreamSynchronize(c->stream));
@@ -1458,6 +1510,7 @@ extern "C" int b2_hpack_reset(b2_ctx* c, uint32_t conn, uint32_t max_table_size)
 extern "C" int b2_hpack_decode_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_hpack_block* blocks, uint32_t n,
                                      void* out, uint32_t per_block_cap, uint32_t* out_lens, int32_t* status, uint32_t* n_headers) {
     if (!c || !bytes || !blocks || !out || !out_lens || !status || !n_headers) { set_err("null argument"); return B2_E_INVAL; }
+    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
     if (nbytes > c->opt.max_batch_bytes || n > c->opt.max_msgs / 4 || (uint64_t)n * per_block_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     std::vector<uint32_t> conn(n), off(n), len(n), first;
     for (uint32_t i = 0; i < n; i++) {
@@ -1491,6 +1544,7 @@ extern "C" int b2_hpack_decode_batch(b2_ctx* c, const void* bytes, uint32_t nbyt
 extern "C" int b2_h2_scan_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs, uint32_t max_frame_size,
                                 b2_h2_frame* frames, uint32_t cap_per_run, uint32_t* n_frames, uint32_t* consumed, uint32_t* err) {
     if (!c || !bytes || !runs || !frames || !n_frames || !consumed || !err) { set_err("null argument"); return B2_E_INVAL; }
+    if (h2_ring_refuses(c, false)) return B2_E_INVAL;
     if (nbytes > c->opt.max_batch_bytes || n_runs > c->opt.max_runs || (uint64_t)n_runs * cap_per_run * sizeof(b2_h2_frame) > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     for (uint32_t r = 0; r < n_runs; r++) if ((uint64_t)runs[r].offset + runs[r].length > nbytes) { set_err("run outside buffer"); return B2_E_INVAL; }
     CU(cudaSetDevice(c->opt.device));
@@ -1525,7 +1579,7 @@ static int h2_ensure(b2_ctx* c) {
 }
 static H2Pool h2_pool(const b2_ctx* c) { H2Pool p; p.streams = c->d_h2_streams; p.slots = c->d_h2_slots; p.pending = c->h2_pending; p.stream_bytes = c->h2_stream_bytes; return p; }
 extern "C" int b2_h2_configure(b2_ctx* c, uint32_t max_conns, uint32_t max_pending, uint32_t stream_bytes) {
-    if (!c || c->d_h2) { set_err("b2_h2_configure must precede the first h2 call on the context"); return B2_E_INVAL; }
+    if (!c || c->d_h2) { set_err("b2_h2_configure must precede the first h2 call on the context"); return B2_E_INVAL; }   // (b2_h2_ring_enable is an h2 call)
     if (max_conns == 0 || max_conns > B2_HPACK_MAX_CONNS || max_pending == 0 || max_pending > 65536 || stream_bytes < B2_H2_HEADER_BYTES + 16 || (stream_bytes & 15u)) {
         set_err("bad h2 capacities"); return B2_E_INVAL;
     }
@@ -1534,6 +1588,7 @@ extern "C" int b2_h2_configure(b2_ctx* c, uint32_t max_conns, uint32_t max_pendi
 }
 extern "C" int b2_h2_conn_reset(b2_ctx* c, uint32_t conn) {
     if (!c || conn >= c->h2_max_conns) { set_err("bad connection index"); return B2_E_INVAL; }
+    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     k_h2_conn_reset<<<1, 1, 0, c->stream>>>(c->d_h2, c->d_hpack, conn, h2_pool(c));
     CU(cudaStreamSynchronize(c->stream));
@@ -1542,6 +1597,7 @@ extern "C" int b2_h2_conn_reset(b2_ctx* c, uint32_t conn) {
 }
 extern "C" int b2_h2_conn_set_gunzip(b2_ctx* c, uint32_t conn, int enable) {
     if (!c || conn >= c->h2_max_conns) { set_err("bad connection index"); return B2_E_INVAL; }
+    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     CU(cudaSetDevice(c->opt.device));
     if (enable && !c->d_h2_gz_merge) {                            // once per context: the merge scratch of the select pass
@@ -1602,6 +1658,7 @@ static int h2_parse_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b
     static_assert(sizeof(M) == 64 && sizeof(b2_h2_run_status) == 32, "h2 ABI layout");
     if (nbytes > c->opt.max_batch_bytes || n_runs > c->opt.max_runs || out_cap > 2ull * c->opt.max_resp_bytes || cap > c->opt.max_msgs ||
         (serve && serve->replies_cap > c->opt.max_resp_bytes)) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
     *n_descs = 0;
     if (n_runs == 0) return B2_OK;
     for (uint32_t r = 0; r < n_runs; r++) {
@@ -1674,6 +1731,7 @@ extern "C" int b2_h2_serve_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, 
 extern "C" int b2_h2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_h2_response* resps, uint32_t n,
                                     void* out, uint32_t out_cap, uint32_t* out_offs, uint32_t* out_lens) {
     if (!c || (!bytes && nbytes) || !resps || !out || !out_offs || !out_lens) { set_err("null argument"); return B2_E_INVAL; }
+    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
     static_assert(sizeof(b2_h2_response) == 48, "h2 response ABI layout");
     if (nbytes > c->opt.max_resp_bytes || n > c->opt.max_msgs || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     if (n == 0) return B2_OK;
@@ -1717,6 +1775,7 @@ extern "C" int b2_h2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbyte
 extern "C" int b2_h2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_h2_request* reqs, uint32_t n,
                                    void* out, uint32_t out_cap, b2_h2_request_result* results) {
     if (!c || !bytes || !reqs || !out || !results) { set_err("null argument"); return B2_E_INVAL; }
+    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
     static_assert(sizeof(b2_h2_request) == 48 && sizeof(b2_h2_request_result) == 16, "h2 request ABI layout");
     if (nbytes > c->opt.max_resp_bytes || n > c->opt.max_msgs || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     if (n == 0) return B2_OK;
@@ -1771,6 +1830,7 @@ extern "C" int b2_h2_conn_peer_update(b2_ctx* c, uint32_t conn, const b2_h2_peer
     static_assert(sizeof(b2_h2_peer_update) == 24, "peer update ABI layout");
     if ((u->set & B2_H2_PEER_MAX_FRAME_SIZE) && (u->max_frame_size < 16384u || u->max_frame_size > 16777215u)) { set_err("max_frame_size out of range"); return B2_E_INVAL; }   // ParseH2Settings :166-211
     if ((u->set & B2_H2_PEER_STREAM_WINDOW) && u->stream_window_size > 0x7fffffffu) { set_err("stream_window_size out of range"); return B2_E_INVAL; }
+    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     if (conn >= c->h2_max_conns) { set_err("conn out of range"); return B2_E_INVAL; }
     CU(cudaSetDevice(c->opt.device));
@@ -1783,6 +1843,7 @@ extern "C" int b2_h2_conn_peer_update(b2_ctx* c, uint32_t conn, const b2_h2_peer
 }
 extern "C" int b2_h2_conn_set_next_stream_id(b2_ctx* c, uint32_t conn, uint32_t next_id) {
     if (!c) { set_err("null argument"); return B2_E_INVAL; }
+    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     if (conn >= c->h2_max_conns) { set_err("conn out of range"); return B2_E_INVAL; }
     CU(cudaSetDevice(c->opt.device));
@@ -1794,6 +1855,7 @@ extern "C" int b2_h2_conn_set_next_stream_id(b2_ctx* c, uint32_t conn, uint32_t 
 // the receiving half of a client connection: see include/b2rpc.h
 extern "C" int b2_h2_client_conn_reset(b2_ctx* c, uint32_t conn) {
     if (!c || conn >= c->h2_max_conns) { set_err("bad connection index"); return B2_E_INVAL; }
+    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     CU(cudaSetDevice(c->opt.device));
     k_h2_client_conn_reset<<<1, 1, 0, c->stream>>>(c->d_h2, c->d_hpack, conn, h2_pool(c));
@@ -1803,6 +1865,7 @@ extern "C" int b2_h2_client_conn_reset(b2_ctx* c, uint32_t conn) {
 }
 extern "C" int b2_h2_client_abandon_streams(b2_ctx* c, uint32_t conn, const uint32_t* stream_ids, uint32_t n) {
     if (!c || (!stream_ids && n)) { set_err("null argument"); return B2_E_INVAL; }
+    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
     if (conn >= c->h2_max_conns) { set_err("bad connection index"); return B2_E_INVAL; }
     if ((uint64_t)n * 4 > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }   // (the ids go to the second half of the scratch)
     if (n == 0) return B2_OK;
@@ -1823,6 +1886,7 @@ extern "C" int b2_h2_client_process_batch(b2_ctx* c, const void* bytes, uint32_t
 extern "C" int b2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_request* reqs, uint32_t n,
                                 void* out, uint32_t out_cap, uint32_t* out_offs, uint32_t* out_lens) {
     if (!c || (!bytes && nbytes) || !reqs || !out || !out_offs || !out_lens) { set_err("null argument"); return B2_E_INVAL; }
+    if (h2_ring_refuses(c, false)) return B2_E_INVAL;
     static_assert(sizeof(b2_request) == 64 && sizeof(ReqDesc) == 64, "request ABI layout");
     if (nbytes > c->opt.max_batch_bytes || n > c->opt.max_msgs || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     if (n == 0) return B2_OK;
@@ -1855,6 +1919,7 @@ extern "C" int b2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes, c
 extern "C" int b2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_reply* reps, uint32_t n,
                                  void* out, uint32_t out_cap, uint32_t* out_offs, uint32_t* out_lens) {
     if (!c || (!bytes && nbytes) || !reps || !out || !out_offs || !out_lens) { set_err("null argument"); return B2_E_INVAL; }
+    if (h2_ring_refuses(c, false)) return B2_E_INVAL;
     static_assert(sizeof(b2_reply) == 88 && sizeof(ReplyDesc) == 88, "reply ABI layout");
     if (nbytes > c->opt.max_batch_bytes || (uint64_t)n * sizeof(b2_reply) > (uint64_t)c->opt.max_msgs * 64 || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     if (n == 0) return B2_OK;
@@ -1889,5 +1954,97 @@ extern "C" int b2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbytes, 
     CU(cudaMemcpyAsync(out, c->d_resp, (size_t)total, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     c->uploaded = false; c->executed = false;
+    return B2_OK;
+}
+
+// ---- h2/gRPC on the latency path: k_h2_ring on the same submit ring (include/b2rpc.h, b2_h2_ring_enable) ---------------------------
+static H2RingDev h2_ring_dev(const b2_ctx* c) {
+    H2RingDev H;
+    H.off_args = c->h2r_off_args; H.off_rs = c->h2r_off_rs; H.off_msgs = c->h2r_off_msgs; H.off_spans = c->h2r_off_spans;
+    H.off_out = c->h2r_off_out; H.off_replies = c->h2r_off_replies;
+    H.conns = c->d_h2; H.hps = c->d_hpack; H.methods = c->d_methods; H.n_methods = c->cfg.n_methods; H.pool = h2_pool(c);
+    H.cfg.n_methods = c->cfg.n_methods; H.cfg.identity_len = c->cfg.identity_len; memcpy(H.cfg.identity, c->cfg.identity, sizeof H.cfg.identity);
+    // the scratch of b2_h2_serve_batch (h2_parse_batch, h2_gz_launch, h2_serve_launch)
+    H.rs = reinterpret_cast<b2_h2_run_status*>(c->d_run_status); H.msgs = reinterpret_cast<b2_h2_msg*>(c->d_msgs); H.out = c->d_unz;
+    H.merge = c->d_h2_gz_merge; H.gz = c->d_frame_off;
+    H.strided = reinterpret_cast<b2_h2_response*>(c->d_heads); H.strided_offs = c->d_frame_run;
+    H.list = reinterpret_cast<b2_h2_response*>(c->d_aux); H.list_offs = c->d_slot; H.first = c->d_run_tile_base;
+    H.spans = reinterpret_cast<b2_h2_reply_span*>(c->d_refs); H.replies = c->d_resp;
+    return H;
+}
+extern "C" int b2_h2_ring_enable(b2_ctx* c, uint32_t max_bytes, uint32_t msg_cap, uint32_t out_cap, uint32_t replies_cap) {
+    if (!c) { set_err("null argument"); return B2_E_INVAL; }
+    if (c->h2_ring || c->ring_slots || c->st_ring) { set_err("b2_h2_ring_enable: once, before the context's first ring call, and not with b2_stream_ring_enable"); return B2_E_INVAL; }
+    if (max_bytes == 0 || msg_cap == 0 || out_cap == 0 || replies_cap == 0) { set_err("capacities must be non-zero"); return B2_E_INVAL; }
+    if (max_bytes > c->opt.max_batch_bytes || out_cap > 2ull * c->opt.max_resp_bytes || msg_cap > c->opt.max_msgs || replies_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    int rc = h2_ensure(c); if (rc != B2_OK) return rc;
+    CU(cudaSetDevice(c->opt.device));
+    static_assert(sizeof(RingSlotHdr) + sizeof(H2RingArgs) <= 256, "h2 ring slot header");
+    // [RingSlotHdr | args | runs | staged input | statuses | msgs | spans | out | replies]
+    auto up = [](uint64_t v) { return (uint32_t)((v + 255u) & ~255ull); };
+    const uint64_t runs = (uint64_t)c->opt.max_runs;
+    c->h2r_off_args = sizeof(RingSlotHdr);
+    c->ring_off_runs = 256;
+    c->ring_off_in = up(c->ring_off_runs + runs * sizeof(b2_run));
+    c->h2r_off_rs = up((uint64_t)c->ring_off_in + max_bytes + 16);
+    c->h2r_off_msgs = up(c->h2r_off_rs + runs * sizeof(b2_h2_run_status));
+    c->h2r_off_spans = up(c->h2r_off_msgs + (uint64_t)msg_cap * sizeof(b2_h2_msg));
+    c->h2r_off_out = up(c->h2r_off_spans + runs * sizeof(b2_h2_reply_span));
+    c->h2r_off_replies = up((uint64_t)c->h2r_off_out + out_cap + 16);
+    rc = ring_alloc(c, (uint64_t)c->h2r_off_replies + replies_cap + 16); if (rc != B2_OK) return rc;
+    CU(cudaFuncSetAttribute(k_h2_ring, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kH2RingSmem));
+    c->h2r_max_bytes = max_bytes; c->h2r_msg_cap = msg_cap; c->h2r_out_cap = out_cap; c->h2r_replies_cap = replies_cap;
+    c->h2_ring = true;
+    return B2_OK;
+}
+extern "C" int b2_h2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs, uint32_t* ticket) {
+    if (!c || !bytes || !runs || !ticket || n_runs == 0) { set_err("null argument"); return B2_E_INVAL; }
+    if (!c->h2_ring) { set_err("b2_h2_ring_enable first"); return B2_E_INVAL; }
+    // the argument checks of b2_h2_serve_batch (h2_parse_batch) with the caps of b2_h2_ring_enable, and the slot's staging size
+    if (nbytes > c->h2r_max_bytes) { set_err("batch larger than b2_h2_ring_enable's max_bytes: use b2_h2_serve_batch"); return B2_E_CAPACITY; }
+    if (n_runs > c->opt.max_runs) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    for (uint32_t r = 0; r < n_runs; r++) {
+        if ((uint64_t)runs[r].offset + runs[r].length > nbytes) { set_err("run outside buffer"); return B2_E_INVAL; }
+        if (runs[r].socket_id >= c->h2_max_conns) { set_err("connection index out of range"); return B2_E_INVAL; }
+        for (uint32_t q = 0; q < r; q++) if (runs[q].socket_id == runs[r].socket_id) { set_err("one run per connection and batch"); return B2_E_INVAL; }
+    }
+    H2RingArgs a;
+    a.region = (c->h2r_out_cap / n_runs) & ~63u; a.per_run = c->h2r_msg_cap / n_runs; a.reply_region = (c->h2r_replies_cap / n_runs) & ~63u;
+    if (a.region < 256 || a.per_run == 0) { set_err("out_cap / msg_cap too small for the number of runs"); return B2_E_CAPACITY; }
+    a.gunzip = h2_gz_wanted(c, runs, n_runs) ? 1u : 0u;
+    const uint32_t t = c->ring_next, si = t % kRingSlots;
+    if (!c->ring_collected[si]) { set_err("submit ring full: b2_h2_ring_wait the oldest ticket first"); return B2_E_CAPACITY; }
+    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);       // the device copies of the last h2 batch are about to be overwritten
+    c->uploaded = false; c->executed = false;
+    uint8_t* slot = c->ring_slots + (size_t)si * c->ring_stride;
+    RingSlotHdr* h = reinterpret_cast<RingSlotHdr*>(slot);
+    h->bytes_dev = ring_stage(c, slot, bytes, nbytes);
+    memcpy(slot + c->ring_off_runs, runs, sizeof(b2_run) * (size_t)n_runs);
+    memcpy(slot + c->h2r_off_args, &a, sizeof a);
+    h->n_runs = n_runs; h->nbytes = nbytes;
+    c->ring_bytes[si] = bytes; c->ring_collected[si] = false;
+    return ring_ring(c, h, t, ticket);
+}
+extern "C" int b2_h2_ring_wait(b2_ctx* c, uint32_t ticket, b2_h2_ring_result* out) {
+    if (!c || !out || !c->h2_ring || !c->ring_slots || ticket == 0 || ticket >= c->ring_next || ticket + kRingSlots < c->ring_next) { set_err("bad h2 ring ticket"); return B2_E_INVAL; }
+    static_assert(sizeof(b2_h2_ring_result) == 64, "h2 ring result ABI layout");
+    const uint32_t si = ticket % kRingSlots;
+    const uint8_t* slot = c->ring_slots + (size_t)si * c->ring_stride;
+    const RingSlotHdr* h = reinterpret_cast<const RingSlotHdr*>(slot);
+    if (c->ring_collected[si]) { set_err("ticket already collected"); return B2_E_INVAL; }
+    { int rc = ring_spin(c, h, ticket); if (rc != B2_OK) return rc; }
+    c->ring_collected[si] = true;
+    const uint32_t n_runs = h->n_runs;
+    const b2_h2_run_status* rs = reinterpret_cast<const b2_h2_run_status*>(slot + c->h2r_off_rs);
+    uint32_t n_msgs = 0;
+    for (uint32_t r = 0; r < n_runs; r++) n_msgs += rs[r].n_msgs;
+    memset(out, 0, sizeof *out);
+    out->runs = rs; out->n_runs = n_runs; out->n_msgs = n_msgs;
+    out->msgs = reinterpret_cast<const b2_h2_msg*>(slot + c->h2r_off_msgs);
+    out->out = slot + c->h2r_off_out; out->region = (c->h2r_out_cap / n_runs) & ~63u;
+    out->replies = slot + c->h2r_off_replies; out->spans = reinterpret_cast<const b2_h2_reply_span*>(slot + c->h2r_off_spans);
+    if (n_msgs > c->h2r_msg_cap) { out->n_msgs = 0; out->status = B2_E_CAPACITY; }
+    // the most recent ticket's input and out regions stay on the device: b2_h2_pack_responses may take bodies and content-types from them
+    if (ticket + 1 == c->ring_next) { c->h2_last_in = h->nbytes; c->h2_last_out = (uint64_t)out->region * n_runs; }
     return B2_OK;
 }

@@ -605,14 +605,11 @@ B2_HD uint64_t h2_reply_bound(uint32_t body_len, uint32_t content_type_len, uint
 // One WARP per connection: lane 0 runs the serial part (window check, HPACK encode against the connection's table,
 // deferred WINDOW_UPDATE) into shared memory, then the whole warp writes the frames — the DATA payload, which is
 // nearly all of the bytes, with coalesced 16-byte copies.
-__global__ void __launch_bounds__(kH2PackWarps * 32) k_h2_pack(const uint8_t* bytes, const uint8_t* last_input, const uint8_t* last_out, const b2_h2_response* resps,
-                                                               const uint32_t* group_first, uint32_t n_groups, H2Conn* conns,
-                                                               uint8_t* out, const uint32_t* out_offs, uint32_t* out_lens) {
-    __shared__ __align__(16) uint8_t s_buf[kH2PackWarps][3][kH2FragCap];
-    const uint32_t lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    const uint32_t g = blockIdx.x * kH2PackWarps + w;
-    if (g >= n_groups) return;
-    uint8_t* frag = s_buf[w][0]; uint8_t* trailer = s_buf[w][1]; uint8_t* tmp = s_buf[w][2];
+// Connection group g, by one warp; buf: the warp's 3 * kH2FragCap bytes of shared scratch.  k_h2_pack and k_h2_ring call it.
+__device__ __forceinline__ void h2_pack_group(uint32_t g, uint32_t lane, uint8_t* buf, const uint8_t* bytes, const uint8_t* last_input, const uint8_t* last_out,
+                                              const b2_h2_response* resps, const uint32_t* group_first, H2Conn* conns,
+                                              uint8_t* out, const uint32_t* out_offs, uint32_t* out_lens) {
+    uint8_t* frag = buf; uint8_t* trailer = buf + kH2FragCap; uint8_t* tmp = buf + 2 * kH2FragCap;
     for (uint32_t i = group_first[g]; i < group_first[g + 1]; i++) {
         const b2_h2_response R = resps[i];
         uint8_t* o0 = out + out_offs[i]; uint8_t* o = o0;
@@ -678,6 +675,15 @@ __global__ void __launch_bounds__(kH2PackWarps * 32) k_h2_pack(const uint8_t* by
         if (lane == 0) out_lens[i] = (uint32_t)(o - o0);
         __syncwarp();                                                // the shared buffers are reused by the next response
     }
+}
+__global__ void __launch_bounds__(kH2PackWarps * 32) k_h2_pack(const uint8_t* bytes, const uint8_t* last_input, const uint8_t* last_out, const b2_h2_response* resps,
+                                                               const uint32_t* group_first, uint32_t n_groups, H2Conn* conns,
+                                                               uint8_t* out, const uint32_t* out_offs, uint32_t* out_lens) {
+    __shared__ __align__(16) uint8_t s_buf[kH2PackWarps][3][kH2FragCap];
+    const uint32_t lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const uint32_t g = blockIdx.x * kH2PackWarps + w;
+    if (g >= n_groups) return;
+    h2_pack_group(g, lane, s_buf[w][0], bytes, last_input, last_out, resps, group_first, conns, out, out_offs, out_lens);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1417,11 +1423,10 @@ __device__ __forceinline__ const uint8_t* h2gz_src(const M& m, const uint8_t* by
     n = grpc ? m.body_len - 5 : m.body_len;
     return ((m.flags & B2_H2_FLAG_BODY_IN_INPUT) ? bytes : out) + m.body_off + (grpc ? 5 : 0);
 }
+// The per-item bodies (run r, or descriptor slot t) of the four passes: the grid kernels below and k_h2_ring call them.
 template <class M>
-__global__ void k_h2_gz_select(const uint8_t* bytes, const b2_run* runs, uint32_t n_runs, const H2Conn* conns, const b2_h2_run_status* rs,
-                               M* msgs, uint32_t per_run, const uint8_t* out, uint8_t* merge_scratch, uint32_t* gz) {
-    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= n_runs) return;
+__device__ __forceinline__ void h2_gz_select_run(uint32_t r, const uint8_t* bytes, const b2_run* runs, const H2Conn* conns, const b2_h2_run_status* rs,
+                                                 M* msgs, uint32_t per_run, const uint8_t* out, uint8_t* merge_scratch, uint32_t* gz) {
     const bool on = conns[(uint32_t)runs[r].socket_id].pad0 & kH2Gunzip;
     uint8_t* const scratch = merge_scratch + (size_t)r * kH2HdrBytes;
     for (uint32_t i = 0; i < rs[r].n_msgs; i++) {
@@ -1452,10 +1457,9 @@ __global__ void k_h2_gz_select(const uint8_t* bytes, const b2_run* runs, uint32_
     }
 }
 template <class M>
-__global__ void k_h2_gz_size(const uint8_t* bytes, uint32_t n_runs, const b2_h2_run_status* rs, const M* msgs, uint32_t per_run,
-                             const uint8_t* out, uint32_t* gz) {
-    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= n_runs * per_run || t % per_run >= rs[t / per_run].n_msgs || gz[t] != kGzToSize) return;
+__device__ __forceinline__ void h2_gz_size_one(uint32_t t, const uint8_t* bytes, const b2_h2_run_status* rs, const M* msgs, uint32_t per_run,
+                                               const uint8_t* out, uint32_t* gz) {
+    if (t % per_run >= rs[t / per_run].n_msgs || gz[t] != kGzToSize) return;
     uint32_t n;
     const uint8_t* src = h2gz_src(msgs[t], bytes, out, n);
     bool big = false;
@@ -1463,9 +1467,7 @@ __global__ void k_h2_gz_size(const uint8_t* bytes, uint32_t n_runs, const b2_h2_
     gz[t] = big ? kGzToHost : bound;
 }
 template <class M>
-__global__ void k_h2_gz_place(uint32_t n_runs, b2_h2_run_status* rs, M* msgs, uint32_t per_run, uint32_t region, uint32_t* gz) {
-    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= n_runs) return;
+__device__ __forceinline__ void h2_gz_place_run(uint32_t r, b2_h2_run_status* rs, M* msgs, uint32_t per_run, uint32_t region, uint32_t* gz) {
     uint32_t cur = region / 4 + rs[r].first_msg;                    // (the consume kernel reports its blob bytes there, a multiple of 16)
     for (uint32_t i = 0; i < rs[r].n_msgs; i++) {
         const uint32_t slot = r * per_run + i, g = gz[slot];
@@ -1477,16 +1479,38 @@ __global__ void k_h2_gz_place(uint32_t n_runs, b2_h2_run_status* rs, M* msgs, ui
     rs[r].first_msg = cur - region / 4;                            // the strided copy-back brings the inflated bytes home
 }
 template <class M>
-__global__ void k_h2_gz_inflate(const uint8_t* bytes, uint32_t n_runs, const b2_h2_run_status* rs, M* msgs, uint32_t per_run,
-                                uint8_t* out, const uint32_t* gz) {
-    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= n_runs * per_run || t % per_run >= rs[t / per_run].n_msgs || gz[t] == kGzSkip) return;
+__device__ __forceinline__ void h2_gz_inflate_one(uint32_t t, const uint8_t* bytes, const b2_h2_run_status* rs, M* msgs, uint32_t per_run,
+                                                  uint8_t* out, const uint32_t* gz) {
+    if (t % per_run >= rs[t / per_run].n_msgs || gz[t] == kGzSkip) return;
     M& m = msgs[t];
     uint32_t n;
     const uint8_t* src = h2gz_src(m, bytes, out, n);
     bool big = false;
     m.msg_len = gz_input_stream<true>(src, n, B2_COMPRESS_TYPE_GZIP, out + m.msg_off, gz[t], &big);   // <= the bound: a failed check hands over less
     m.flags |= B2_H2_FLAG_GUNZIPPED;
+}
+template <class M>
+__global__ void k_h2_gz_select(const uint8_t* bytes, const b2_run* runs, uint32_t n_runs, const H2Conn* conns, const b2_h2_run_status* rs,
+                               M* msgs, uint32_t per_run, const uint8_t* out, uint8_t* merge_scratch, uint32_t* gz) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r < n_runs) h2_gz_select_run(r, bytes, runs, conns, rs, msgs, per_run, out, merge_scratch, gz);
+}
+template <class M>
+__global__ void k_h2_gz_size(const uint8_t* bytes, uint32_t n_runs, const b2_h2_run_status* rs, const M* msgs, uint32_t per_run,
+                             const uint8_t* out, uint32_t* gz) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < n_runs * per_run) h2_gz_size_one(t, bytes, rs, msgs, per_run, out, gz);
+}
+template <class M>
+__global__ void k_h2_gz_place(uint32_t n_runs, b2_h2_run_status* rs, M* msgs, uint32_t per_run, uint32_t region, uint32_t* gz) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r < n_runs) h2_gz_place_run(r, rs, msgs, per_run, region, gz);
+}
+template <class M>
+__global__ void k_h2_gz_inflate(const uint8_t* bytes, uint32_t n_runs, const b2_h2_run_status* rs, M* msgs, uint32_t per_run,
+                                uint8_t* out, const uint32_t* gz) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < n_runs * per_run) h2_gz_inflate_one(t, bytes, rs, msgs, per_run, out, gz);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1543,11 +1567,10 @@ __device__ __noinline__ uint32_t h2_serve_error(uint8_t* p, const H2ServeCfg& C,
 }
 // The records of run r go to resps / reply_offs[r * per_run ...], their count to spans[r].n_answered.  Reply i of the run gets
 // h2_reply_bound bytes at reply_offs (16-byte aligned) in the run's reply_region bytes of the packed replies.
-__global__ void k_h2_serve(const uint8_t* bytes, const b2_run* runs, uint32_t n_runs, const DevMethod* methods, const H2ServeCfg cfg,
-                           b2_h2_run_status* rs, b2_h2_msg* msgs, uint32_t per_run, uint8_t* out, uint32_t region,
-                           b2_h2_response* resps, uint32_t* reply_offs, uint32_t reply_region, b2_h2_reply_span* spans) {
-    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= n_runs) return;
+// k_h2_serve (a thread per run) and k_h2_ring call it.
+__device__ __forceinline__ void h2_serve_run(uint32_t r, const uint8_t* bytes, const b2_run* runs, const DevMethod* methods, const H2ServeCfg& cfg,
+                                             b2_h2_run_status* rs, b2_h2_msg* msgs, uint32_t per_run, uint8_t* out, uint32_t region,
+                                             b2_h2_response* resps, uint32_t* reply_offs, uint32_t reply_region, b2_h2_reply_span* spans) {
     const uint32_t gbase = r * region;
     uint32_t cur = region / 4 + rs[r].first_msg;                    // behind the parse's and the gunzip passes' bytes (a multiple of 16)
     uint32_t rep = 0, k = 0;
@@ -1616,34 +1639,48 @@ __global__ void k_h2_serve(const uint8_t* bytes, const b2_run* runs, uint32_t n_
     b2_h2_reply_span sp; sp.off = r * reply_region; sp.len = 0; sp.n_answered = k; sp.reserved = 0;
     spans[r] = sp;
 }
-// One warp: group_first (k_h2_pack's list of connections, one per run, empty ones included) = the exclusive prefix of the answered counts
-__global__ void k_h2_serve_scan(uint32_t n_runs, const b2_h2_reply_span* spans, uint32_t* group_first) {
-    const uint32_t lane = threadIdx.x, per = (n_runs + 31) / 32;
+__global__ void k_h2_serve(const uint8_t* bytes, const b2_run* runs, uint32_t n_runs, const DevMethod* methods, const H2ServeCfg cfg,
+                           b2_h2_run_status* rs, b2_h2_msg* msgs, uint32_t per_run, uint8_t* out, uint32_t region,
+                           b2_h2_response* resps, uint32_t* reply_offs, uint32_t reply_region, b2_h2_reply_span* spans) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r < n_runs) h2_serve_run(r, bytes, runs, methods, cfg, rs, msgs, per_run, out, region, resps, reply_offs, reply_region, spans);
+}
+// One warp: first[r] = the exclusive prefix of count(r) over the runs, first[n_runs] = the total.  Lane l sums a contiguous share.
+template <class F>
+__device__ __forceinline__ void h2_warp_scan_runs(uint32_t n_runs, uint32_t lane, F count, uint32_t* first) {
+    const uint32_t per = (n_runs + 31) / 32;
     const uint32_t lo = min(lane * per, n_runs), hi = min(lo + per, n_runs);
     uint32_t sum = 0;
-    for (uint32_t r = lo; r < hi; r++) sum += spans[r].n_answered;
+    for (uint32_t r = lo; r < hi; r++) sum += count(r);
     uint32_t incl = sum;
     for (uint32_t d = 1; d < 32; d <<= 1) {
         const uint32_t v = __shfl_sync(0xffffffffu, incl, lane >= d ? lane - d : lane);
         if (lane >= d) incl += v;
     }
     uint32_t at = incl - sum;
-    for (uint32_t r = lo; r < hi; r++) { group_first[r] = at; at += spans[r].n_answered; }
-    if (lane == 31) group_first[n_runs] = incl;
+    for (uint32_t r = lo; r < hi; r++) { first[r] = at; at += count(r); }
+    if (lane == 31) first[n_runs] = incl;
 }
-// one thread per descriptor slot: the records and reply offsets move from per_run strides into that list
+// One warp: group_first (k_h2_pack's list of connections, one per run, empty ones included) = the exclusive prefix of the answered counts
+__global__ void k_h2_serve_scan(uint32_t n_runs, const b2_h2_reply_span* spans, uint32_t* group_first) {
+    h2_warp_scan_runs(n_runs, threadIdx.x, [&](uint32_t r) { return spans[r].n_answered; }, group_first);
+}
+// one descriptor slot t: the record and reply offset move from per_run strides into that list
+__device__ __forceinline__ void h2_serve_compact_one(uint32_t t, uint32_t per_run, const b2_h2_reply_span* spans, const uint32_t* group_first,
+                                                     const b2_h2_response* strided, const uint32_t* strided_offs, b2_h2_response* resps, uint32_t* reply_offs) {
+    const uint32_t r = t / per_run, k = t % per_run;
+    if (k >= spans[r].n_answered) return;
+    resps[group_first[r] + k] = strided[t]; reply_offs[group_first[r] + k] = strided_offs[t];
+}
 __global__ void k_h2_serve_compact(uint32_t n_runs, uint32_t per_run, const b2_h2_reply_span* spans, const uint32_t* group_first,
                                    const b2_h2_response* strided, const uint32_t* strided_offs, b2_h2_response* resps, uint32_t* reply_offs) {
-    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x, r = t / per_run, k = t % per_run;
-    if (r >= n_runs || k >= spans[r].n_answered) return;
-    resps[group_first[r] + k] = strided[t]; reply_offs[group_first[r] + k] = strided_offs[t];
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < n_runs * per_run) h2_serve_compact_one(t, per_run, spans, group_first, strided, strided_offs, resps, reply_offs);
 }
 // One warp per run: the replies k_h2_pack wrote at their reserved offsets move down to follow each other.  The move is forward inside
 // the run's region: every 512-byte step is loaded whole before any of it is stored, and a step never stores past what it loaded.
-__global__ void __launch_bounds__(kH2PackWarps * 32) k_h2_serve_gather(uint32_t n_runs, const uint32_t* group_first, const uint32_t* reply_offs,
-                                                                       const uint32_t* reply_lens, uint8_t* replies, b2_h2_reply_span* spans) {
-    const uint32_t lane = threadIdx.x & 31, r = blockIdx.x * kH2PackWarps + (threadIdx.x >> 5);
-    if (r >= n_runs) return;
+__device__ __forceinline__ void h2_gather_run(uint32_t r, uint32_t lane, const uint32_t* group_first, const uint32_t* reply_offs,
+                                              const uint32_t* reply_lens, uint8_t* replies, b2_h2_reply_span* spans) {
     const uint32_t start = spans[r].off;
     uint32_t dst = start;
     for (uint32_t i = group_first[r]; i < group_first[r + 1]; i++) {
@@ -1664,5 +1701,107 @@ __global__ void __launch_bounds__(kH2PackWarps * 32) k_h2_serve_gather(uint32_t 
     }
     if (lane == 0) spans[r].len = dst - start;
 }
+__global__ void __launch_bounds__(kH2PackWarps * 32) k_h2_serve_gather(uint32_t n_runs, const uint32_t* group_first, const uint32_t* reply_offs,
+                                                                       const uint32_t* reply_lens, uint8_t* replies, b2_h2_reply_span* spans) {
+    const uint32_t lane = threadIdx.x & 31, r = blockIdx.x * kH2PackWarps + (threadIdx.x >> 5);
+    if (r < n_runs) h2_gather_run(r, lane, group_first, reply_offs, reply_lens, replies, spans);
+}
+
+#if defined(B2_KERNELS_RING)
+// ---------------------------------------------------------------------------------------------------------
+// k_h2_ring: b2_h2_serve_batch on the latency path (b2_h2_ring_*).  One resident CTA, fed through the same submit ring as k_ring
+// (ring_doorbell / ring_pull / ring_push / ring_stamp / ring_release of b2_kernels.cuh): per ticket the passes of the batch call, as block phases with
+// __syncthreads() where the batch call has kernel boundaries, on the same device scratch, then only the used parts are pushed into the
+// ticket's slot.  H2Conn, HpackState and the stream pool are read through L1: every call that writes them from another kernel retires
+// this one first (ring_halt), so a launch boundary lies between their writes and this CTA's loads.
+struct H2RingArgs { uint32_t per_run, region, reply_region, gunzip; };   // per ticket, from the host, at the slot's off_args
+struct H2RingDev {
+    uint32_t off_args, off_rs, off_msgs, off_spans, off_out, off_replies;  // the slot's parts behind RingSlotHdr (runs, staged input: RingDev)
+    H2Conn* conns; HpackState* hps; const DevMethod* methods; uint32_t n_methods; H2ServeCfg cfg; H2Pool pool;
+    // the scratch of b2_h2_serve_batch: the run statuses, per_run-strided descriptors, the out regions, the gunzip merge scratch, gz words
+    // (then the reply lengths), the strided records and their offsets, the list k_h2_pack reads and its offsets, group_first (then the
+    // first list index of every run's messages), the spans and the replies
+    b2_h2_run_status* rs; b2_h2_msg* msgs; uint8_t* out; uint8_t* merge; uint32_t* gz;
+    b2_h2_response* strided; uint32_t* strided_offs; b2_h2_response* list; uint32_t* list_offs; uint32_t* first;
+    b2_h2_reply_span* spans; uint8_t* replies;
+};
+constexpr uint32_t kH2RingSmem = kSmallWarps * 3 * kH2FragCap;          // k_h2_pack's scratch for each warp
+__global__ void __launch_bounds__(kSmallThreads, 1) k_h2_ring(RingDev R, H2RingDev H) {
+    extern __shared__ __align__(16) uint8_t h2_ring_raw[];
+    __shared__ uint32_t s_go;
+    __shared__ RingSlotHdr s_hdr;
+    __shared__ H2RingArgs s_args;
+    const uint32_t tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const uint8_t* bytes = R.d_bytes;
+    const b2_run* runs = reinterpret_cast<const b2_run*>(R.d_meta);
+    uint32_t ticket = R.next_ticket[0];
+    for (;;) {
+        uint8_t* slot = R.slots + (size_t)(ticket % kRingSlots) * R.slot_stride;
+        RingSlotHdr* hdr = reinterpret_cast<RingSlotHdr*>(slot);
+        if (tid == 0) s_go = ring_doorbell(R, hdr, ticket);
+        __syncthreads();
+        if (!s_go) break;
+        unsigned long long t[4] = { 0, 0, 0, 0 };                    // doorbell seen, header read, bytes pulled, replies packed
+        if (tid == 0) t[0] = globaltimer_ns();
+        ring_pull(R, slot, s_hdr, R.d_meta, t[1]);
+        if (tid < 4) reinterpret_cast<uint32_t*>(&s_args)[tid] = ld_sys_u32(reinterpret_cast<const volatile uint32_t*>(slot + H.off_args) + tid);
+        __threadfence();
+        __syncthreads();
+        if (tid == 0) t[2] = globaltimer_ns();
+        const uint32_t n_runs = s_hdr.n_runs, per_run = s_args.per_run, region = s_args.region, reply_region = s_args.reply_region, n_slots = n_runs * per_run;
+        for (uint32_t r = tid; r < n_runs; r += kSmallThreads)
+            h2_consume_run<false>(r, bytes, runs, H.conns, H.hps, H.methods, H.n_methods, H.rs, H.msgs, per_run, H.out, region, H.pool);
+        __syncthreads();
+        if (s_args.gunzip) {                                          // a run's connection opted in (b2_h2_conn_set_gunzip)
+            for (uint32_t r = tid; r < n_runs; r += kSmallThreads) h2_gz_select_run(r, bytes, runs, H.conns, H.rs, H.msgs, per_run, H.out, H.merge, H.gz);
+            __syncthreads();
+            for (uint32_t i = tid; i < n_slots; i += kSmallThreads) h2_gz_size_one(i, bytes, H.rs, H.msgs, per_run, H.out, H.gz);
+            __syncthreads();
+            for (uint32_t r = tid; r < n_runs; r += kSmallThreads) h2_gz_place_run(r, H.rs, H.msgs, per_run, region, H.gz);
+            __syncthreads();
+            for (uint32_t i = tid; i < n_slots; i += kSmallThreads) h2_gz_inflate_one(i, bytes, H.rs, H.msgs, per_run, H.out, H.gz);
+            __syncthreads();
+        }
+        for (uint32_t r = tid; r < n_runs; r += kSmallThreads)
+            h2_serve_run(r, bytes, runs, H.methods, H.cfg, H.rs, H.msgs, per_run, H.out, region, H.strided, H.strided_offs, reply_region, H.spans);
+        __syncthreads();
+        if (wid == 0) h2_warp_scan_runs(n_runs, lane, [&](uint32_t r) { return H.spans[r].n_answered; }, H.first);
+        __syncthreads();
+        for (uint32_t i = tid; i < n_slots; i += kSmallThreads) h2_serve_compact_one(i, per_run, H.spans, H.first, H.strided, H.strided_offs, H.list, H.list_offs);
+        __syncthreads();
+        for (uint32_t g = wid; g < n_runs; g += kSmallWarps)
+            h2_pack_group(g, lane, h2_ring_raw + wid * 3 * kH2FragCap, H.out, bytes, H.out, H.list, H.first, H.conns, H.replies, H.list_offs, H.gz);
+        __syncthreads();
+        for (uint32_t r = wid; r < n_runs; r += kSmallWarps) h2_gather_run(r, lane, H.first, H.list_offs, H.gz, H.replies, H.spans);
+        __syncthreads();
+        if (tid == 0) t[3] = globaltimer_ns();
+        // the descriptors become one list in run order (the batch call compacts them on the host): first[r] = run r's first list index
+        if (wid == 0) h2_warp_scan_runs(n_runs, lane, [&](uint32_t r) { return H.rs[r].n_msgs; }, H.first);
+        __syncthreads();
+        // push, a warp per run: its descriptors into the list, its control bytes and blob (whose length the status reports in first_msg)
+        // at the offsets the batch call uses, its replies, then the status with first_msg = the list index, and the span
+        for (uint32_t r = wid; r < n_runs; r += kSmallWarps) {
+            b2_h2_run_status st = H.rs[r];
+            const b2_h2_reply_span sp = H.spans[r];
+            const uint32_t f = H.first[r], base = r * region;
+            ring_push(slot + H.off_msgs + (size_t)f * sizeof(b2_h2_msg), reinterpret_cast<const uint8_t*>(H.msgs + (size_t)r * per_run), st.n_msgs * (uint32_t)sizeof(b2_h2_msg), lane, 32);
+            ring_push(slot + H.off_out + base, H.out + base, st.ctrl_len, lane, 32);
+            ring_push(slot + H.off_out + base + region / 4, H.out + base + region / 4, st.first_msg, lane, 32);
+            ring_push(slot + H.off_replies + sp.off, H.replies + sp.off, sp.len, lane, 32);
+            if (lane == 0) {
+                st.first_msg = f;
+                reinterpret_cast<b2_h2_run_status*>(slot + H.off_rs)[r] = st;
+                reinterpret_cast<b2_h2_reply_span*>(slot + H.off_spans)[r] = sp;
+            }
+        }
+        if (tid == 0) ring_stamp(hdr, t);
+        __threadfence_system();
+        __syncthreads();
+        if (tid == 0) ring_release(R, hdr, ticket);
+        ticket++;
+    }
+    if (tid == 0) R.next_ticket[0] = ticket;
+}
+#endif
 #endif
 }  // namespace b2

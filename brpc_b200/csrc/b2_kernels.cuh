@@ -2770,6 +2770,64 @@ __device__ __forceinline__ void st_sys_u32(volatile uint32_t* p, uint32_t v) {
     asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 __device__ __forceinline__ unsigned long long globaltimer_ns() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
+// The parts k_ring and k_h2_ring share.  Thread 0 waits for `ticket` in its slot: 1 when it came, 0 on `stop` or after idle_ns without
+// work.  A context whose ticket overflowed k_ring's compact block parks behind it (next_ticket[1]) until the host has served it through
+// the big pipeline and released it (ctl[3]): the stream table sees the tickets in ticket order, and the pull does not overwrite the device
+// input that pipeline reads.  k_h2_ring never parks (next_ticket[1] stays 0).
+__device__ __forceinline__ uint32_t ring_doorbell(const RingDev& R, RingSlotHdr* hdr, uint32_t ticket) {
+    const unsigned long long t0 = globaltimer_ns();
+    const uint32_t park = R.next_ticket[1];
+    auto ready = [&]() { return ld_sys_u32(&hdr->submit) == ticket && (park == 0 || ld_sys_u32(R.ctl + 3) == park); };
+    uint32_t go = 0;
+    for (;;) {
+        if (ready()) { go = 1; break; }
+        if (ld_sys_u32(R.ctl + 0)) break;
+        if (globaltimer_ns() - t0 > R.idle_ns) {
+            // leave: announce it first, then look once more so that a submission racing with the exit is not lost
+            st_sys_u32(R.ctl + 1, 0); __threadfence_system();
+            if (ready()) { st_sys_u32(R.ctl + 1, 1); go = 1; }
+            break;
+        }
+    }
+    if (go && park) R.next_ticket[1] = 0;
+    return go;
+}
+// The whole CTA: the slot header into s_hdr (the host's stores are ordered before `submit` by its release fence), then the runs (24 bytes
+// each) into runs_dst and the batch bytes into R.d_bytes, 16 bytes per thread per trip.  t_hdr: when the header was read (thread 0).
+__device__ __forceinline__ void ring_pull(const RingDev& R, const uint8_t* slot, RingSlotHdr& s_hdr, uint8_t* runs_dst, unsigned long long& t_hdr) {
+    const uint32_t tid = threadIdx.x, nt = blockDim.x;
+    if (tid < sizeof(RingSlotHdr) / 4) reinterpret_cast<uint32_t*>(&s_hdr)[tid] = ld_sys_u32(reinterpret_cast<const volatile uint32_t*>(slot) + tid);
+    __syncthreads();
+    if (tid == 0) t_hdr = globaltimer_ns();
+    const uint4* src = reinterpret_cast<const uint4*>(slot + R.off_runs);
+    uint4* dst = reinterpret_cast<uint4*>(runs_dst);
+    for (uint32_t k = tid; k < (s_hdr.n_runs * 24u + 15u) / 16u; k += nt) dst[k] = src[k];
+    const uint4* bs = reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(s_hdr.bytes_dev));
+    uint4* bd = reinterpret_cast<uint4*>(R.d_bytes);
+    const uint32_t nv = (s_hdr.nbytes + 15u) / 16u;
+    uint32_t k = tid;
+    for (; k + 3 * nt < nv; k += 4 * nt) {                            // four loads in flight per thread
+        const uint4 a = bs[k], b = bs[k + nt], c = bs[k + 2 * nt], d = bs[k + 3 * nt];
+        bd[k] = a; bd[k + nt] = b; bd[k + 2 * nt] = c; bd[k + 3 * nt] = d;
+    }
+    for (; k < nv; k += nt) bd[k] = bs[k];
+}
+// n bytes from device memory into the slot (mapped host memory) with 16-byte stores: posted PCIe writes.  src and dst 16-byte aligned;
+// the copy may read and write up to 15 bytes past n.
+__device__ __forceinline__ void ring_push(uint8_t* dst, const uint8_t* src, uint32_t n, uint32_t first, uint32_t step) {
+    const uint4* s = reinterpret_cast<const uint4*>(src);
+    uint4* d = reinterpret_cast<uint4*>(dst);
+    for (uint32_t k = first; k < (n + 15u) / 16u; k += step) d[k] = __ldcg(s + k);
+}
+// Thread 0, before the CTA makes its results visible system-wide (__threadfence_system(); __syncthreads()): the phase stamps.
+__device__ __forceinline__ void ring_stamp(RingSlotHdr* hdr, const unsigned long long (&t)[4]) {
+    hdr->stamps[0] = t[0]; hdr->stamps[1] = t[1]; hdr->stamps[2] = t[2]; hdr->stamps[3] = t[3]; hdr->stamps[4] = globaltimer_ns();
+}
+// Thread 0, after that: `done`, then the served count.
+__device__ __forceinline__ void ring_release(const RingDev& R, RingSlotHdr* hdr, uint32_t ticket) {
+    st_sys_u32(&hdr->done, ticket); st_sys_u32(R.ctl + 2, ticket + 1);
+}
+#define B2_KERNELS_RING 1                                             // b2_h2.cuh builds k_h2_ring on the parts above
 
 // ---------------------------------------------------------------------------------------------------------------------------------
 // streaming_rpc: the receiving side of a Stream on the device (b2_stream_*).  What brpc does with a STRM frame after the meta parse:
@@ -3109,50 +3167,13 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_ring(RingDev R, BatchPtrs 
     for (;;) {
         uint8_t* slot = R.slots + (size_t)(ticket % kRingSlots) * R.slot_stride;
         RingSlotHdr* hdr = reinterpret_cast<RingSlotHdr*>(slot);
-        if (tid == 0) {
-            const unsigned long long t0 = globaltimer_ns();
-            // a table context parks behind a ticket that overflowed the compact block (next_ticket[1]) until the host has served it
-            // through the big pipeline and released it (ctl[3]): the table sees the tickets in ticket order, and the pull below does not
-            // overwrite the device input that pipeline reads
-            const uint32_t park = R.next_ticket[1];
-            auto ready = [&]() { return ld_sys_u32(&hdr->submit) == ticket && (park == 0 || ld_sys_u32(R.ctl + 3) == park); };
-            uint32_t go = 0;
-            for (;;) {
-                if (ready()) { go = 1; break; }
-                if (ld_sys_u32(R.ctl + 0)) break;
-                if (globaltimer_ns() - t0 > R.idle_ns) {
-                    // leave: announce it first, then look once more so that a submission racing with the exit is not lost
-                    st_sys_u32(R.ctl + 1, 0); __threadfence_system();
-                    if (ready()) { st_sys_u32(R.ctl + 1, 1); go = 1; }
-                    break;
-                }
-            }
-            if (go && park) R.next_ticket[1] = 0;
-            s_go = go;
-        }
+        if (tid == 0) s_go = ring_doorbell(R, hdr, ticket);
         __syncthreads();
         if (!s_go) break;
-        unsigned long long t_seen = 0, t_hdr = 0, t_pull = 0, t_body = 0;
-        if (tid == 0) t_seen = globaltimer_ns();
-        // the slot header (the host's stores are ordered before `submit` by its release fence)
-        if (tid < sizeof(RingSlotHdr) / 4) reinterpret_cast<uint32_t*>(&s_hdr)[tid] = ld_sys_u32(reinterpret_cast<const volatile uint32_t*>(slot) + tid);
-        __syncthreads();
-        const uint32_t n_runs = s_hdr.n_runs, nbytes = s_hdr.nbytes;
-        if (tid == 0) t_hdr = globaltimer_ns();
-        {   // pull: runs (24 B each) + per-run tile base placeholder, then the batch bytes, 16 bytes per thread per trip
-            const uint4* src = reinterpret_cast<const uint4*>(slot + R.off_runs);
-            uint4* dst = reinterpret_cast<uint4*>(R.d_meta);
-            for (uint32_t k = tid; k < (n_runs * 24u + 15u) / 16u; k += kSmallThreads) dst[k] = src[k];
-            const uint4* bs = reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(s_hdr.bytes_dev));
-            uint4* bd = reinterpret_cast<uint4*>(R.d_bytes);
-            const uint32_t nv = (nbytes + 15u) / 16u;
-            uint32_t k = tid;
-            for (; k + 3 * kSmallThreads < nv; k += 4 * kSmallThreads) {              // four loads in flight per thread
-                const uint4 a = bs[k], b = bs[k + kSmallThreads], c = bs[k + 2 * kSmallThreads], d = bs[k + 3 * kSmallThreads];
-                bd[k] = a; bd[k + kSmallThreads] = b; bd[k + 2 * kSmallThreads] = c; bd[k + 3 * kSmallThreads] = d;
-            }
-            for (; k < nv; k += kSmallThreads) bd[k] = bs[k];
-        }
+        unsigned long long t[4] = { 0, 0, 0, 0 };                    // doorbell seen, header read, bytes pulled, body done
+        if (tid == 0) t[0] = globaltimer_ns();
+        ring_pull(R, slot, s_hdr, R.d_meta, t[1]);
+        const uint32_t n_runs = s_hdr.n_runs;
         BatchPtrs B = B0;
         B.bytes = R.d_bytes; B.runs = reinterpret_cast<const b2_run*>(R.d_meta); B.n_runs = n_runs;
         B.totals = reinterpret_cast<uint32_t*>(R.d_small);
@@ -3165,7 +3186,7 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_ring(RingDev R, BatchPtrs 
         if (tid < 16) { B.totals[tid] = 0; if (streams) SP.cnts[tid] = 0; }
         __threadfence();
         __syncthreads();
-        if (tid == 0) t_pull = globaltimer_ns();
+        if (tid == 0) t[2] = globaltimer_ns();
         small_body(B, Cb, S);
         __threadfence();
         __syncthreads();
@@ -3175,31 +3196,23 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_ring(RingDev R, BatchPtrs 
             __threadfence();
             __syncthreads();
         }
-        if (tid == 0) t_body = globaltimer_ns();
-        {   // push the compact block [totals | run_status | msgs | refs | resp] into the slot's output area
-            const uint32_t used = (B.totals[2] & 3u) ? 64u : s_hdr.off_resp + ((B.totals[1] + 15u) & ~15u);
-            const uint4* src = reinterpret_cast<const uint4*>(R.d_small);
-            uint4* dst = reinterpret_cast<uint4*>(slot + R.off_out);
-            for (uint32_t k = tid; k < (used + 15u) / 16u; k += kSmallThreads) dst[k] = __ldcg(src + k);
-        }
+        if (tid == 0) t[3] = globaltimer_ns();
+        // push the compact block [totals | run_status | msgs | refs | resp] into the slot's output area
+        ring_push(slot + R.off_out, R.d_small, (B.totals[2] & 3u) ? 64u : s_hdr.off_resp + ((B.totals[1] + 15u) & ~15u), tid, kSmallThreads);
         if (streams && !overflow) {   // ... and the stream section [counters | events | msgs | ctrl | run_ctrl | out], the used part of each
             const uint32_t n_msgs = __ldcg(SP.cnts + 0), n_ev = __ldcg(SP.cnts + 1), n_out = __ldcg(SP.cnts + 2), n_ctrl = __ldcg(SP.cnts + 3);
             const uint32_t len[6] = { 64u, n_ev * (uint32_t)sizeof(b2_stream_event), n_msgs * (uint32_t)sizeof(b2_stream_msg), n_ctrl, n_runs * 8u, n_out };
             const uint8_t* from[6] = { reinterpret_cast<const uint8_t*>(SP.cnts), reinterpret_cast<const uint8_t*>(SP.events), reinterpret_cast<const uint8_t*>(SP.msgs),
                                        SP.ctrl, reinterpret_cast<const uint8_t*>(SP.run_ctrl), SP.out };
             uint8_t* sec = slot + R.off_st;
-            for (int q = 0; q < 6; q++) {
-                const uint4* src = reinterpret_cast<const uint4*>(from[q]);
-                uint4* dst = reinterpret_cast<uint4*>(sec + (from[q] - from[0]));
-                for (uint32_t k = tid; k < (len[q] + 15u) / 16u; k += kSmallThreads) dst[k] = __ldcg(src + k);
-            }
+            for (int q = 0; q < 6; q++) ring_push(sec + (from[q] - from[0]), from[q], len[q], tid, kSmallThreads);
         }
-        if (tid == 0) { hdr->stamps[0] = t_seen; hdr->stamps[1] = t_hdr; hdr->stamps[2] = t_pull; hdr->stamps[3] = t_body; hdr->stamps[4] = globaltimer_ns(); }
+        if (tid == 0) ring_stamp(hdr, t);
         __threadfence_system();
         __syncthreads();
         if (tid == 0) {
             if (streams && overflow) R.next_ticket[1] = ticket;
-            st_sys_u32(&hdr->done, ticket); st_sys_u32(R.ctl + 2, ticket + 1);
+            ring_release(R, hdr, ticket);
         }
         ticket++;
     }

@@ -768,6 +768,40 @@ typedef struct b2_h2_reply_span { uint32_t off, len, n_answered, reserved; } b2_
 int  b2_h2_serve_batch(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
                        b2_h2_run_status* rs, b2_h2_msg* msgs, uint32_t msg_cap, uint32_t* n_msgs, void* out, uint32_t out_cap,
                        void* replies, uint32_t replies_cap, b2_h2_reply_span* spans);
+/* h2/gRPC on the latency path: b2_h2_serve_batch inside a resident kernel (k_h2_ring) fed through the submit ring of b2_ring_* — no
+ * launch, copy or stream synchronisation per batch.  A context runs either k_ring or k_h2_ring, never both.
+ * b2_h2_ring_enable: once, after b2_h2_configure and before the context's first ring call (after b2_ring_start / b2_ring_submit /
+ * b2_stream_ring_enable, or twice: B2_E_INVAL; b2_ring_submit / b2_ring_wait then fail with B2_E_INVAL).  The four capacities are per
+ * ticket and play the roles of b2_h2_serve_batch's nbytes bound, msg_cap, out_cap and replies_cap; they are checked against the context
+ * limits that call checks and fix the slot layout (header, runs, staged input, statuses, messages, spans, out, replies, times the 8 ring
+ * slots, all pinned + mapped host memory).  b2_ring_stop, b2_ring_launches, b2_ring_phase_ns ([2]: replies packed) and
+ * B2_RING_IDLE_MS apply to k_h2_ring as to k_ring.
+ * b2_h2_ring_submit: the argument checks of b2_h2_serve_batch (runs inside the buffer, socket_id < max_conns, one run per connection,
+ * n_runs <= max_runs, (out_cap / n_runs) & ~63 >= 256 and msg_cap / n_runs > 0), n_runs > 0, and nbytes <= max_bytes (else
+ * B2_E_CAPACITY: serve that batch with b2_h2_serve_batch).  Bytes in b2_block_alloc memory are pulled in place, others staged into the
+ * slot.  Connections with gunzip on (b2_h2_conn_set_gunzip) are served too.
+ * b2_h2_ring_wait: tickets may be waited in any order.  For any sequence of tickets the results equal, byte for byte, what
+ * b2_h2_serve_batch returns for the same sequence of batches with the same caps: run statuses, messages (B2_H2_FLAG_ANSWERED, the
+ * grpc-status in `reserved`), the defined bytes of out (run i's control bytes at ctrl_off, its blob from i * region + region / 4),
+ * spans and replies — and so does the connection state left behind (HPACK tables, windows, deferred WINDOW_UPDATEs, the stream pool).
+ * After the wait of the most recent ticket, b2_h2_pack_responses resolves B2_H2_RESP_BODY_IN_INPUT / _BODY_IN_OUT / _CT_IN_OUT
+ * against that ticket, as after the batch call.
+ * While a ticket is outstanding every call that uploads to the context or touches h2 state fails with B2_E_INVAL: the b2_h2_* and
+ * b2_hpack_* calls, the batch calls (b2_batch_upload / _submit, b2_process_batch), b2_pack_*, b2_crc32c_batch, the snappy batch calls,
+ * b2_stream_write and b2_set_server_identity — the ticket uses their device scratch.  Between tickets every call is allowed.  A call that
+ * writes h2 connection state (b2_h2_conn_reset / _set_gunzip / _peer_update / _set_next_stream_id, b2_h2_client_*, b2_h2_process_batch,
+ * b2_h2_serve_batch, b2_h2_pack_*, b2_hpack_*) and b2_set_server_identity first retire the resident kernel, which reads that state
+ * through L1; the next submission relaunches it (b2_ring_launches counts it). */
+typedef struct b2_h2_ring_result {    /* views into the ticket's pinned slot, valid until the slot is reused by the 8th later submission */
+    const b2_h2_run_status* runs; uint32_t n_runs, n_msgs;
+    const b2_h2_msg* msgs;            /* compacted: runs[i].first_msg is a list index, as b2_h2_serve_batch returns it */
+    const uint8_t* out; uint32_t region;   /* run i's control bytes and blob live at out + i * region, as in the batch call */
+    const uint8_t* replies; const b2_h2_reply_span* spans;
+    int32_t status;                   /* what b2_h2_serve_batch would have returned for this batch */
+} b2_h2_ring_result;                  /* 64 bytes */
+int  b2_h2_ring_enable(b2_ctx* ctx, uint32_t max_bytes, uint32_t msg_cap, uint32_t out_cap, uint32_t replies_cap);
+int  b2_h2_ring_submit(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs, uint32_t* ticket);
+int  b2_h2_ring_wait(b2_ctx* ctx, uint32_t ticket, b2_h2_ring_result* out);
 
 /* ---- streaming_rpc, the receiving side of a Stream on the device ------------------------------------------------------------------
  * Without a stream table a STRM frame ends as a B2_MSG_STREAM_FRAME descriptor and the host rebuilds brpc's Stream from the list.  With
