@@ -31,6 +31,14 @@ constexpr int kMaxStages = 16;
 constexpr uint32_t kSmallBytes = 128 << 10;        // batches up to this size take the latency path
 constexpr uint32_t kSmallRuns = 512, kSmallMsgs = 1024;   // == kSmallThreads, 2 * kSmallThreads of k_small
 constexpr size_t kSmallBlock = 64 + kSmallRuns * 32 + kSmallMsgs * (64 + 16) + (kSmallBytes + kSmallMsgs * 80 + 4096);
+// the compact output block of a small batch, as k_small and k_ring write it: [totals 64 | run statuses | msgs | refs | resp]
+// (msgs is bounded by max_msgs too: d_frame_off / d_aux / d_jobs / d_heads ... are sized by it)
+struct SmallLayout { uint32_t msgs, resp, off_rs, off_msgs, off_refs, off_resp, total; };
+SmallLayout small_layout(uint32_t nbytes, uint32_t n_runs, uint32_t max_msgs) {
+    const uint32_t mb = std::min(std::min(nbytes / 12 + 1, kSmallMsgs), max_msgs), resp = nbytes + mb * 80 + 2048, off_msgs = 64 + n_runs * 32;
+    const uint32_t off_refs = off_msgs + mb * 64, off_resp = (off_refs + mb * 16 + 255u) & ~255u;
+    return { mb, resp, 64, off_msgs, off_refs, off_resp, off_resp + resp };
+}
 // a ring slot's stream section (b2_stream_ring_enable), and the device staging k_ring fills before it pushes the section:
 // [counters 64 | events | msgs | ctrl | run_ctrl | out], each part sized for what one ticket of <= kSmallMsgs messages can produce
 // (touched streams <= messages; per message at most one RST frame, per stream one FEEDBACK and one CLOSE frame)
@@ -63,7 +71,7 @@ struct b2_ctx {
     bool h2_ring = false; uint32_t h2r_max_bytes = 0, h2r_msg_cap = 0, h2r_out_cap = 0, h2r_replies_cap = 0;
     uint32_t h2r_off_args = 0, h2r_off_rs = 0, h2r_off_msgs = 0, h2r_off_spans = 0, h2r_off_out = 0, h2r_off_replies = 0;
     ulonglong2* d_iov = nullptr; b2_iovec* h_iov = nullptr; const void* host_bytes = nullptr;      // B2_RESP_IOVEC
-    uint4* d_refs = nullptr; b2_resp_ref* h_refs = nullptr; int input_mode = B2_INPUT_COPY, resp_mode = B2_RESP_COPY; const uint8_t* pull_bytes = nullptr; uint32_t small_off_refs = 0;
+    uint4* d_refs = nullptr; b2_resp_ref* h_refs = nullptr; int input_mode = B2_INPUT_COPY, resp_mode = B2_RESP_COPY; const uint8_t* pull_bytes = nullptr;
     uint32_t* d_crc_adv = nullptr; unsigned long long* d_counters = nullptr; uint32_t* d_totals = nullptr; DevMethod* d_methods = nullptr;
     size_t meta_tile_off = 0; uint32_t max_tiles = 0; uint32_t n_sms = 132; bool use_tma_pack = true; uint32_t stage_mask = 7;  // debug: 1 front stages, 2 k_pack_tma, 4 k_pack_slow
     // stream table (b2_stream_*): the device side in `sp`; the host keeps the keys (it picks the table slots) and the free pool slots
@@ -94,12 +102,17 @@ struct b2_ctx {
     // small-batch (latency) mode: one compact H2D block, one compact output block, one D2H, one sync
     uint8_t* d_meta = nullptr; uint8_t* h_meta = nullptr;       // [runs | run_tile_base]
     uint8_t* d_small = nullptr; uint8_t* h_small = nullptr;     // [totals | run_status | msgs | resp]
-    bool small = false, small_copy_queued = false, use_fused_small = true; uint32_t small_msgs = 0, small_resp = 0, small_off_rs = 0, small_off_msgs = 0, small_off_resp = 0, small_total = 0;
+    bool small = false, small_copy_queued = false, use_fused_small = true; SmallLayout sm = {};
 };
 
-// d_bytes is about to hold another call's bytes: B2_STREAM_W_FROM_MSG can no longer read the device copy of the last batch's input
-// (a B2_INPUT_PULL batch was read in the caller's region, which stays)
-static void input_overwritten(b2_ctx* c) { if (c->st_input == c->d_bytes) c->st_input = nullptr; }
+// What a call overwrites on the device, and so which saved state it forgets; every call that writes the context's buffers says so first.
+// kDevInput, the input (d_bytes, d_meta): the last h2 batch b2_h2_pack_responses reads zero-copy, and the input copy B2_STREAM_W_FROM_MSG
+// reads (a B2_INPUT_PULL batch was read in the caller's region, which stays).  kDevBatch, the results and scratch: the uploaded batch.
+enum : unsigned { kDevInput = 1, kDevBatch = 2 };
+static void overwrites(b2_ctx* c, unsigned what) {
+    if (what & kDevInput) { c->h2_last_in = 0; c->h2_last_out = 0; if (c->st_input == c->d_bytes) c->st_input = nullptr; }
+    if (what & kDevBatch) { c->uploaded = false; c->executed = false; }
+}
 
 static uint32_t g_crc_tab_host[256];
 static void crc_table_init() {
@@ -165,12 +178,13 @@ extern "C" uint64_t b2_block_pool_host_allocs(void) { std::lock_guard<std::mutex
 
 static void ring_halt(b2_ctx* c);
 static void stream_free(b2_ctx* c);
+static bool ring_busy(const b2_ctx* c) { for (uint32_t k = 0; k < kRingSlots; k++) if (!c->ring_collected[k]) return true; return false; }
 // Every call that uploads to the context or touches h2 state is refused while an h2 ring ticket is outstanding: the ticket uses the same
 // device scratch and connection state.  A call that writes h2 connection state also retires k_h2_ring first: the resident CTA reads that
 // state through L1, and a launch boundary is where L1 is known not to hold lines another kernel wrote since.
 static bool h2_ring_refuses(b2_ctx* c, bool writes_h2_state) {
     if (!c->h2_ring) return false;
-    for (uint32_t k = 0; k < kRingSlots; k++) if (!c->ring_collected[k]) { set_err("an h2 ring ticket is outstanding: b2_h2_ring_wait it first"); return true; }
+    if (ring_busy(c)) { set_err("an h2 ring ticket is outstanding: b2_h2_ring_wait it first"); return true; }
     if (writes_h2_state) ring_halt(c);
     return false;
 }
@@ -329,7 +343,7 @@ extern "C" int b2_set_modes(b2_ctx* c, int input_mode, int resp_mode) {
     }
     ring_halt(c);
     c->input_mode = input_mode; c->resp_mode = resp_mode; c->cfg.by_ref = resp_mode != B2_RESP_COPY; c->cfg.pull = input_mode == B2_INPUT_PULL; c->cfg.pull_vecs = resp_mode != B2_RESP_COPY ? 6u : 8u;
-    c->uploaded = false; c->executed = false;
+    overwrites(c, kDevBatch);                       // (the uploaded batch was laid out for the old modes)
     return B2_OK;
 }
 
@@ -382,12 +396,12 @@ static BatchPtrs make_ptrs(b2_ctx* c) {
     B.tile_info = reinterpret_cast<const uint4*>(c->d_meta + c->meta_tile_off);
     if (c->input_mode == B2_INPUT_PULL) B.bytes = c->pull_bytes;          // the caller's pinned + mapped batch buffer, read in place
     if (c->small) {
-        B.refs = reinterpret_cast<uint4*>(c->d_small + c->small_off_refs);
+        B.refs = reinterpret_cast<uint4*>(c->d_small + c->sm.off_refs);
         B.totals = reinterpret_cast<uint32_t*>(c->d_small);
-        B.run_status = reinterpret_cast<b2_run_status*>(c->d_small + c->small_off_rs);
-        B.msgs = reinterpret_cast<b2_msg_desc*>(c->d_small + c->small_off_msgs);
-        B.resp = c->d_small + c->small_off_resp;
-        B.max_msgs = c->small_msgs; B.max_resp = c->small_resp;
+        B.run_status = reinterpret_cast<b2_run_status*>(c->d_small + c->sm.off_rs);
+        B.msgs = reinterpret_cast<b2_msg_desc*>(c->d_small + c->sm.off_msgs);
+        B.resp = c->d_small + c->sm.off_resp;
+        B.max_msgs = c->sm.msgs; B.max_resp = c->sm.resp;
     }
     return B;
 }
@@ -440,7 +454,7 @@ extern "C" int b2_batch_upload(b2_ctx* c, const void* bytes, uint32_t nbytes, co
             for (uint32_t t = t0; t < t1; t++) { uint32_t* q = ti + 4 * (size_t)t; q[0] = runs[r].offset; q[1] = runs[r].length; q[2] = t - t0; q[3] = r | (runs[r].flags << 24); }
         }
     }
-    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);       // the device copies of the last h2 batch are about to be overwritten
+    overwrites(c, kDevInput | kDevBatch);
     if (c->input_mode == B2_INPUT_PULL) {
         // no copy: the kernels read the caller's pinned block in place (it must stay untouched until collect)
         void* dp = nullptr;
@@ -452,25 +466,18 @@ extern "C" int b2_batch_upload(b2_ctx* c, const void* bytes, uint32_t nbytes, co
     CU(cudaMemcpyAsync(c->d_meta, c->h_meta, meta_bytes, cudaMemcpyHostToDevice, c->stream));
     // latency path: outputs of a small batch live in one compact block -> one D2H copy, one sync
     c->small = c->allow_small && nbytes <= kSmallBytes && n_runs <= kSmallRuns && n_runs > 0;
-    if (c->small) {
-        uint32_t mb = nbytes / 12 + 1; if (mb > kSmallMsgs) mb = kSmallMsgs;
-        if (mb > c->opt.max_msgs) mb = c->opt.max_msgs;      // d_frame_off / d_aux / d_jobs / d_heads ... are sized by opt.max_msgs
-        c->small_msgs = mb; c->small_resp = nbytes + mb * 80 + 2048;
-        c->small_off_rs = 64; c->small_off_msgs = 64 + n_runs * 32; c->small_off_refs = c->small_off_msgs + mb * 64;
-        c->small_off_resp = (c->small_off_refs + mb * 16 + 255u) & ~255u;
-        c->small_total = c->small_off_resp + c->small_resp;
-    }
+    if (c->small) c->sm = small_layout(nbytes, n_runs, c->opt.max_msgs);
     if (const char* e = getenv("B2_STAGE_MASK")) c->stage_mask = (uint32_t)atoi(e);   // timing experiments only (tools/overlap_probe.py)
-    c->uploaded = true; c->executed = false;
+    c->uploaded = true;
     return B2_OK;
 }
 
 // The stream pass of a batch call (k_stream_*): behind the stage that wrote msgs[], on the same stream, inside the call's synchronisation.
 static const char* const kStreamStages[5] = { "stream_route", "stream_alloc", "stream_group", "stream_run", "stream_rst" };
+static uint32_t grid(uint32_t items, uint32_t per_block, uint32_t most) { const uint32_t g = (items + per_block - 1) / per_block; return g < 1 ? 1u : g < most ? g : most; }
 static int launch_stream_pass(b2_ctx* c, const BatchPtrs& B, cudaStream_t s, uint32_t& launches) {
     const StreamPass& S = c->sp;
-    const uint32_t msg_bound = c->small ? c->small_msgs : c->opt.max_msgs, sms = c->n_sms;
-    auto grid = [&](uint32_t items, uint32_t per_block, uint32_t most) { const uint32_t g = (items + per_block - 1) / per_block; return g < 1 ? 1u : g < most ? g : most; };
+    const uint32_t msg_bound = c->small ? c->sm.msgs : c->opt.max_msgs, sms = c->n_sms;
     CU(cudaMemsetAsync(S.cnts, 0, 4 * (16 + 2 * (size_t)S.cap), s));          // counters | cnt | fill
     CU(cudaEventRecord(c->st_ev[0], s));
     k_stream_route<<<grid(msg_bound, 256, sms * 4), 256, 0, s>>>(B, S); CU(cudaEventRecord(c->st_ev[1], s));
@@ -563,10 +570,15 @@ static int launch_pipeline(b2_ctx* c) {
     return B2_OK;
 }
 
+// b2_batch_execute / _execute_many / b2_batch_launch replay the uploaded batch, without its stream pass
+static bool replay_refused(const b2_ctx* c) {
+    if (!c || !c->uploaded) { set_err("no batch uploaded"); return true; }
+    if (c->stream_armed) { set_err("a submitted batch of a context with a stream table must be collected first: this entry point replays a batch and does not run the stream pass"); return true; }
+    return false;
+}
 extern "C" int b2_batch_execute(b2_ctx* c, float* kernel_ms, uint32_t* n_launches) {
-    if (!c || !c->uploaded) { set_err("no batch uploaded"); return B2_E_INVAL; }
+    if (replay_refused(c)) return B2_E_INVAL;
     CU(cudaSetDevice(c->opt.device));
-    if (c->stream_armed) { set_err("a submitted batch of a context with a stream table must be collected first: this entry point replays a batch and does not run the stream pass"); return B2_E_INVAL; }
     c->profile_stages = true;
     int rc = launch_pipeline(c);
     c->profile_stages = false;
@@ -581,12 +593,12 @@ extern "C" int b2_batch_execute(b2_ctx* c, float* kernel_ms, uint32_t* n_launche
 }
 
 extern "C" int b2_batch_execute_many(b2_ctx* c, uint32_t steps, float* total_ms, uint32_t* n_launches) {
-    if (!c || !c->uploaded || steps == 0) { set_err("no batch uploaded"); return B2_E_INVAL; }
+    if (steps == 0) { set_err("no batch uploaded"); return B2_E_INVAL; }
+    if (replay_refused(c)) return B2_E_INVAL;
     CU(cudaSetDevice(c->opt.device));
     cudaEvent_t e0, e1;
     CU(cudaEventCreate(&e0)); CU(cudaEventCreate(&e1));
     CU(cudaEventRecord(e0, c->stream));
-    if (c->stream_armed) { set_err("a submitted batch of a context with a stream table must be collected first: this entry point replays a batch and does not run the stream pass"); return B2_E_INVAL; }
     uint32_t launches = 0;
     for (uint32_t i = 0; i < steps; i++) {
         int rc = launch_pipeline(c);
@@ -606,10 +618,9 @@ extern "C" int b2_batch_execute_many(b2_ctx* c, uint32_t steps, float* total_ms,
 }
 
 extern "C" int b2_batch_launch(b2_ctx* c) {
-    if (!c || !c->uploaded) { set_err("no batch uploaded"); return B2_E_INVAL; }
+    if (replay_refused(c)) return B2_E_INVAL;
     CU(cudaSetDevice(c->opt.device));
     if (c->first_pending) { CU(cudaEventRecord(c->ev_first, c->stream)); c->first_pending = false; }
-    if (c->stream_armed) { set_err("a submitted batch of a context with a stream table must be collected first: this entry point replays a batch and does not run the stream pass"); return B2_E_INVAL; }
     int rc = launch_pipeline(c);
     if (rc != B2_OK) return rc;
     CU(cudaEventRecord(c->ev_last, c->stream));
@@ -686,12 +697,16 @@ static int download_normal(b2_ctx* c, b2_batch_result* out) {
     return B2_OK;
 }
 
+// the running average message size, from which the next upload picks its tiles and pack kernel
+static void note_avg_frame(b2_ctx* c, uint64_t bytes, uint32_t n_msgs) {
+    if (n_msgs) { const uint32_t now = (uint32_t)(bytes / n_msgs); c->avg_frame = c->avg_frame ? (uint32_t)(((uint64_t)c->avg_frame * 3 + now) / 4) : now; }
+}
 extern "C" int b2_batch_download(b2_ctx* c, b2_batch_result* out) {
     if (!c || !out || !c->executed) { set_err("no executed batch"); return B2_E_INVAL; }
     CU(cudaSetDevice(c->opt.device));
     memset(out, 0, sizeof *out);
     if (c->small) {
-        if (!c->small_copy_queued) CU(cudaMemcpyAsync(c->h_small, c->d_small, c->small_total, cudaMemcpyDeviceToHost, c->stream));
+        if (!c->small_copy_queued) CU(cudaMemcpyAsync(c->h_small, c->d_small, c->sm.total, cudaMemcpyDeviceToHost, c->stream));
         c->small_copy_queued = false;
         CU(cudaStreamSynchronize(c->stream));
         const uint32_t* tot = reinterpret_cast<const uint32_t*>(c->h_small);
@@ -703,10 +718,10 @@ extern "C" int b2_batch_download(b2_ctx* c, b2_batch_result* out) {
             rc = download_normal(c, out);
             if (rc != B2_OK) return rc;
         } else {
-            out->runs = reinterpret_cast<const b2_run_status*>(c->h_small + c->small_off_rs); out->n_runs = c->n_runs;
-            out->msgs = reinterpret_cast<const b2_msg_desc*>(c->h_small + c->small_off_msgs); out->n_msgs = tot[0];
-            out->resp = c->h_small + c->small_off_resp; out->resp_bytes = tot[1];
-            out->refs = c->cfg.by_ref ? reinterpret_cast<const b2_resp_ref*>(c->h_small + c->small_off_refs) : nullptr;
+            out->runs = reinterpret_cast<const b2_run_status*>(c->h_small + c->sm.off_rs); out->n_runs = c->n_runs;
+            out->msgs = reinterpret_cast<const b2_msg_desc*>(c->h_small + c->sm.off_msgs); out->n_msgs = tot[0];
+            out->resp = c->h_small + c->sm.off_resp; out->resp_bytes = tot[1];
+            out->refs = c->cfg.by_ref ? reinterpret_cast<const b2_resp_ref*>(c->h_small + c->sm.off_refs) : nullptr;
             if (c->resp_mode == B2_RESP_IOVEC) refs_to_iov(c, out, c->host_bytes);
             if (c->stream_ran && c->h_st_cnts[2]) {          // multi-frame messages completed: their bytes follow
                 CU(cudaMemcpyAsync(c->h_st_out, c->sp.out, c->h_st_cnts[2], cudaMemcpyDeviceToHost, c->stream));
@@ -717,7 +732,7 @@ extern "C" int b2_batch_download(b2_ctx* c, b2_batch_result* out) {
         int rc = download_normal(c, out);
         if (rc != B2_OK) return rc;
     }
-    if (out->n_msgs) { const uint32_t now = (uint32_t)(c->covered / out->n_msgs); c->avg_frame = c->avg_frame ? (uint32_t)(((uint64_t)c->avg_frame * 3 + now) / 4) : now; }
+    note_avg_frame(c, c->covered, out->n_msgs);
     out->kernel_ms = c->last_kernel_ms; out->n_launches = c->last_launches;
     c->stream_valid = c->stream_armed; c->stream_armed = false;
     return B2_OK;
@@ -730,7 +745,7 @@ extern "C" int b2_batch_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, co
     rc = launch_pipeline(c);
     if (rc != B2_OK) return rc;
     c->executed = true;
-    if (c->small) { CU(cudaMemcpyAsync(c->h_small, c->d_small, c->small_total, cudaMemcpyDeviceToHost, c->stream)); c->small_copy_queued = true; }
+    if (c->small) { CU(cudaMemcpyAsync(c->h_small, c->d_small, c->sm.total, cudaMemcpyDeviceToHost, c->stream)); c->small_copy_queued = true; }
     return B2_OK;
 }
 
@@ -813,9 +828,9 @@ static int stream_configure(b2_ctx* c, uint32_t max_streams, uint32_t pending_by
 
 // a ring ticket of a context whose ring runs the stream pass is submitted and not collected: the table belongs to k_ring
 static bool ring_owns_table(const b2_ctx* c) {
-    if (!c->st_ring) return false;
-    for (uint32_t k = 0; k < kRingSlots; k++) if (!c->ring_collected[k]) { set_err("a ring ticket is outstanding: b2_ring_wait it first, the stream table belongs to it"); return true; }
-    return false;
+    if (!c->st_ring || !ring_busy(c)) return false;
+    set_err("a ring ticket is outstanding: b2_ring_wait it first, the stream table belongs to it");
+    return true;
 }
 
 static uint32_t stream_find(const b2_ctx* c, int64_t id) {
@@ -1019,7 +1034,6 @@ extern "C" int b2_stream_write(b2_ctx* c, const void* bytes, uint32_t nbytes, co
     P.out = static_cast<uint8_t*>(c->d_sw[1]);
     cudaStream_t s = c->stream;
     const uint32_t sms = c->n_sms, streams = n < c->st_max ? n : c->st_max;
-    auto grid = [&](uint32_t items, uint32_t per_block, uint32_t most) { const uint32_t g = (items + per_block - 1) / per_block; return g < 1 ? 1u : g < most ? g : most; };
     CU(cudaMemcpyAsync(blk, c->h_sw_recs, sizeof(SwRec) * (size_t)n, cudaMemcpyHostToDevice, s));
     if (nbytes) CU(cudaMemcpyAsync(c->d_sw[0], bytes, nbytes, cudaMemcpyHostToDevice, s));
     CU(cudaMemsetAsync(per_slot, 0, 64 + 8 * cap, s));                 // counters | cnt | fill
@@ -1139,8 +1153,9 @@ static unsigned long long ring_stage(b2_ctx* c, uint8_t* slot, const void* bytes
     if (!dev) { memcpy(slot + c->ring_off_in, bytes, nbytes); dev = (unsigned long long)(uintptr_t)(slot + c->ring_off_in); }
     return dev;
 }
-// rings the doorbell of ticket t in its slot (everything else the host stores there first) and relaunches the kernel if it idled out
-static int ring_ring(b2_ctx* c, RingSlotHdr* h, uint32_t t, uint32_t* ticket) {
+// marks ticket t outstanding, rings its doorbell (everything else the host stores in the slot first) and relaunches the kernel if it idled out
+static int ring_ring(b2_ctx* c, RingSlotHdr* h, uint32_t t, const void* bytes, uint32_t* ticket) {
+    c->ring_bytes[t % kRingSlots] = bytes; c->ring_collected[t % kRingSlots] = false;
     __sync_synchronize();
     h->submit = t;
     __sync_synchronize();
@@ -1165,6 +1180,12 @@ static int ring_spin(b2_ctx* c, const RingSlotHdr* h, uint32_t ticket) {
     __sync_synchronize();
     return B2_OK;
 }
+// the slot of `ticket` while it is submitted and not collected; else null, with the error set (args_ok: the caller's own checks)
+static uint8_t* ring_ticket_slot(b2_ctx* c, bool args_ok, uint32_t ticket, const char* bad_ticket) {
+    if (!args_ok || !c->ring_slots || ticket == 0 || ticket >= c->ring_next || ticket + kRingSlots < c->ring_next) { set_err(bad_ticket); return nullptr; }
+    if (c->ring_collected[ticket % kRingSlots]) { set_err("ticket already collected"); return nullptr; }
+    return c->ring_slots + (size_t)(ticket % kRingSlots) * c->ring_stride;
+}
 extern "C" int b2_ring_stop(b2_ctx* c) { if (!c) return B2_E_INVAL; cudaSetDevice(c->opt.device); ring_halt(c); return B2_OK; }
 
 extern "C" int b2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs, uint32_t* ticket) {
@@ -1177,24 +1198,22 @@ extern "C" int b2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, con
     if (!c->ring_collected[si]) { set_err("submit ring full: b2_ring_wait the oldest ticket first"); return B2_E_CAPACITY; }
     for (uint32_t r = 0; r < n_runs; r++)
         if ((runs[r].offset & 15u) || (uint64_t)runs[r].offset + runs[r].length > nbytes) { set_err("run offset must be 16-aligned and inside the batch"); return B2_E_INVAL; }
+    overwrites(c, kDevInput | kDevBatch);           // k_ring pulls the ticket into d_bytes / d_meta and runs it over the batch scratch
     uint8_t* slot = c->ring_slots + (size_t)si * c->ring_stride;
     RingSlotHdr* h = reinterpret_cast<RingSlotHdr*>(slot);
     const unsigned long long dev = ring_stage(c, slot, bytes, nbytes);
     memcpy(slot + c->ring_off_runs, runs, sizeof(b2_run) * (size_t)n_runs);
-    uint32_t mb = nbytes / 12 + 1; if (mb > kSmallMsgs) mb = kSmallMsgs; if (mb > c->opt.max_msgs) mb = c->opt.max_msgs;
-    h->n_runs = n_runs; h->nbytes = nbytes; h->small_msgs = mb; h->small_resp = nbytes + mb * 80 + 2048;
-    h->off_rs = 64; h->off_msgs = 64 + n_runs * 32; h->off_refs = h->off_msgs + mb * 64; h->off_resp = (h->off_refs + mb * 16 + 255u) & ~255u;
-    h->total = h->off_resp + h->small_resp; h->by_ref = c->cfg.by_ref; h->bytes_dev = dev;
-    c->ring_bytes[si] = bytes; c->ring_collected[si] = false;
-    return ring_ring(c, h, t, ticket);
+    const SmallLayout L = small_layout(nbytes, n_runs, c->opt.max_msgs);
+    h->n_runs = n_runs; h->nbytes = nbytes; h->small_msgs = L.msgs; h->small_resp = L.resp; h->off_rs = L.off_rs; h->off_msgs = L.off_msgs;
+    h->off_refs = L.off_refs; h->off_resp = L.off_resp; h->total = L.total; h->by_ref = c->cfg.by_ref; h->bytes_dev = dev;
+    return ring_ring(c, h, t, bytes, ticket);
 }
 
 extern "C" int b2_ring_wait(b2_ctx* c, uint32_t ticket, b2_batch_result* out) {
-    if (!c || !out || !c->ring_slots || ticket == 0 || ticket >= c->ring_next || ticket + kRingSlots < c->ring_next) { set_err("bad ring ticket"); return B2_E_INVAL; }
+    uint8_t* slot = ring_ticket_slot(c, c && out, ticket, "bad ring ticket");
+    if (!slot) return B2_E_INVAL;
     const uint32_t si = ticket % kRingSlots;
-    uint8_t* slot = c->ring_slots + (size_t)si * c->ring_stride;
     RingSlotHdr* h = reinterpret_cast<RingSlotHdr*>(slot);
-    if (c->ring_collected[si]) { set_err("ticket already collected"); return B2_E_INVAL; }
     if (c->st_ring && ticket != c->ring_next_wait) { set_err("a context whose ring runs the stream pass collects its tickets in ticket order"); return B2_E_INVAL; }
     if (c->h2_ring) { set_err("this context's ring serves h2: use b2_h2_ring_wait"); return B2_E_INVAL; }
     { int rc = ring_spin(c, h, ticket); if (rc != B2_OK) return rc; }
@@ -1203,24 +1222,16 @@ extern "C" int b2_ring_wait(b2_ctx* c, uint32_t ticket, b2_batch_result* out) {
     memset(out, 0, sizeof *out);
     const uint8_t* ob = slot + c->ring_off_out;
     const uint32_t* tot = reinterpret_cast<const uint32_t*>(ob);
-    if ((tot[2] & 3u) && c->st_ring) {
-        // k_ring ran no stream pass for this ticket and parks before the next one's pull: the big pipeline serves the ticket (its own
-        // stream pass included) while the kernel waits, then ctl[3] releases it — the table sees the tickets in ticket order
-        const bool allow = c->allow_small; c->allow_small = false;
-        const int rc = b2_process_batch(c, c->ring_bytes[si], h->nbytes, reinterpret_cast<const b2_run*>(slot + c->ring_off_runs), h->n_runs, out);
-        c->allow_small = allow;
-        __sync_synchronize();
-        c->ring_ctl[3] = ticket;
-        __sync_synchronize();
-        return rc;
-    }
     if (tot[2] & 3u) {
-        // more messages / reply bytes than the compact block holds: the big pipeline serves this batch (after the ring is quiet)
-        for (uint32_t k = 0; k < kRingSlots; k++) if (!c->ring_collected[k]) { set_err("ring overflow fallback needs the other tickets collected first"); return B2_E_CAPACITY; }
-        ring_halt(c);
+        // more messages / reply bytes than the compact block holds: the big pipeline serves the ticket.  With the stream pass on the ring,
+        // k_ring ran no pass for it (the pipeline runs its own) and parks before the next one's pull until ctl[3] releases it, so that the
+        // table sees the tickets in ticket order; otherwise the ring must be quiet first
+        if (!c->st_ring && ring_busy(c)) { set_err("ring overflow fallback needs the other tickets collected first"); return B2_E_CAPACITY; }
+        if (!c->st_ring) ring_halt(c);
         const bool allow = c->allow_small; c->allow_small = false;
         const int rc = b2_process_batch(c, c->ring_bytes[si], h->nbytes, reinterpret_cast<const b2_run*>(slot + c->ring_off_runs), h->n_runs, out);
         c->allow_small = allow;
+        if (c->st_ring) { __sync_synchronize(); c->ring_ctl[3] = ticket; __sync_synchronize(); }
         return rc;
     }
     out->runs = reinterpret_cast<const b2_run_status*>(ob + h->off_rs); out->n_runs = h->n_runs;
@@ -1230,7 +1241,7 @@ extern "C" int b2_ring_wait(b2_ctx* c, uint32_t ticket, b2_batch_result* out) {
     if (c->resp_mode == B2_RESP_IOVEC) refs_to_iov(c, out, c->ring_bytes[si]);
     out->n_launches = 0; out->kernel_ms = 0.f;
     if (c->st_ring) { c->stream_valid = true; c->st_view_ticket = ticket; c->st_input = c->d_bytes; }
-    if (out->n_msgs) { const uint32_t now = h->nbytes / out->n_msgs; c->avg_frame = c->avg_frame ? (uint32_t)(((uint64_t)c->avg_frame * 3 + now) / 4) : now; }
+    note_avg_frame(c, h->nbytes, out->n_msgs);
     return B2_OK;
 }
 extern "C" uint64_t b2_ring_launches(b2_ctx* c) { return c ? c->ring_launches : 0; }
@@ -1327,6 +1338,8 @@ __global__ void k_crc32c_batch(const uint8_t* bytes, const uint32_t* offs, const
     }
 }
 
+// the outputs of a batch call lie back to back in `out`, 16-byte aligned: the next one, `need` bytes, at *off; false once past out_cap
+static bool out_place(uint64_t& total, uint64_t need, uint32_t out_cap, uint32_t* off) { *off = (uint32_t)total; total += (need + 15) & ~15ull; return total <= out_cap; }
 extern "C" int b2_crc32c_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const uint32_t* offs, const uint32_t* lens,
                                uint32_t n, uint32_t* out) {
     if (!c || !bytes || !offs || !lens || !out) { set_err("null argument"); return B2_E_INVAL; }
@@ -1334,14 +1347,13 @@ extern "C" int b2_crc32c_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, co
     if (nbytes > c->opt.max_batch_bytes || n > c->opt.max_msgs) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     for (uint32_t i = 0; i < n; i++) if ((uint64_t)offs[i] + lens[i] > nbytes) { set_err("slice outside buffer"); return B2_E_INVAL; }
     CU(cudaSetDevice(c->opt.device));
-    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);       // the device copies of the last h2 batch are about to be overwritten
+    overwrites(c, kDevInput | kDevBatch);
     CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(c->d_frame_off, offs, 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(c->d_slot, lens, 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
     if (n) k_crc32c_batch<<<c->n_sms * 8, 256, 0, c->stream>>>(c->d_bytes, c->d_frame_off, c->d_slot, n, (uint32_t*)c->d_aux, c->d_crc_adv);
     CU(cudaMemcpyAsync(out, c->d_aux, 4 * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
-    c->uploaded = false; c->executed = false;
     return B2_OK;
 }
 
@@ -1370,16 +1382,14 @@ extern "C" int b2_snappy_uncompress_batch(b2_ctx* c, const void* bytes, uint32_t
         const uint8_t* p = (const uint8_t*)bytes + offs[i];
         uint32_t v = 0, shift = 0, k = 0; bool ok = false;
         while (k < lens[i] && shift < 32) { const uint32_t b = p[k++]; v |= (b & 0x7f) << shift; if (b < 128) { ok = true; break; } shift += 7; }
-        out_offs[i] = (uint32_t)total;
-        if (!ok || (uint64_t)v > 32ull * lens[i] + 64ull) { caps[i] = 0xffffffffu; continue; }   // cannot be a valid stream
-        caps[i] = v;
-        total += ((uint64_t)v + 15) & ~15ull;
-        if (total > out_cap) { set_err("output exceeds out_cap"); return B2_E_CAPACITY; }
+        const bool valid = ok && (uint64_t)v <= 32ull * lens[i] + 64ull;       // else it cannot be a valid stream: no output
+        caps[i] = valid ? v : 0xffffffffu;
+        if (!out_place(total, valid ? v : 0, out_cap, &out_offs[i])) { set_err("output exceeds out_cap"); return B2_E_CAPACITY; }
     }
     CU(cudaSetDevice(c->opt.device));
     uint32_t* d_offs = c->d_frame_off; uint32_t* d_lens = c->d_slot; uint32_t* d_ooffs = c->d_frame_run;
     uint32_t* d_caps = (uint32_t*)c->d_jobs; int32_t* d_olens = (int32_t*)c->d_aux;
-    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);       // the device copies of the last h2 batch are about to be overwritten
+    overwrites(c, kDevInput | kDevBatch);
     CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_offs, offs, 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_lens, lens, 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
@@ -1389,7 +1399,6 @@ extern "C" int b2_snappy_uncompress_batch(b2_ctx* c, const void* bytes, uint32_t
     CU(cudaMemcpyAsync(out_lens, d_olens, 4 * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
     if (total) CU(cudaMemcpyAsync(out, c->d_unz, total, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
-    c->uploaded = false; c->executed = false;
     return B2_OK;
 }
 
@@ -1411,13 +1420,11 @@ extern "C" int b2_snappy_compress_batch(b2_ctx* c, const void* bytes, uint32_t n
     uint64_t total = 0;
     for (uint32_t i = 0; i < n; i++) {
         if ((uint64_t)offs[i] + lens[i] > nbytes) { set_err("slice outside buffer"); return B2_E_INVAL; }
-        out_offs[i] = (uint32_t)total;
-        total += ((uint64_t)snappy_max_compressed_length(lens[i]) + 15) & ~15ull;
-        if (total > out_cap) { set_err("output exceeds out_cap"); return B2_E_CAPACITY; }
+        if (!out_place(total, snappy_max_compressed_length(lens[i]), out_cap, &out_offs[i])) { set_err("output exceeds out_cap"); return B2_E_CAPACITY; }
     }
     CU(cudaSetDevice(c->opt.device));
     uint32_t* d_offs = c->d_frame_off; uint32_t* d_lens = c->d_slot; uint32_t* d_ooffs = c->d_frame_run; uint32_t* d_olens = (uint32_t*)c->d_aux;
-    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);       // the device copies of the last h2 batch are about to be overwritten
+    overwrites(c, kDevInput | kDevBatch);
     CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_offs, offs, 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_lens, lens, 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
@@ -1426,7 +1433,6 @@ extern "C" int b2_snappy_compress_batch(b2_ctx* c, const void* bytes, uint32_t n
     CU(cudaMemcpyAsync(out_lens, d_olens, 4 * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
     if (total) CU(cudaMemcpyAsync(out, c->d_unz, total, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
-    c->uploaded = false; c->executed = false;
     return B2_OK;
 }
 
@@ -1454,13 +1460,13 @@ extern "C" uint32_t b2_crc32c_extend(uint32_t init_crc, const char* data, size_t
     if (!c || n > c->opt.max_batch_bytes) return 0;
     cudaSetDevice(c->opt.device);
     const uint32_t off = 0, len = (uint32_t)n; uint32_t out = 0;
+    overwrites(c, kDevBatch);                       // (the private leaf context has no h2 batch or stream pass that could read its input)
     if (cudaMemcpyAsync(c->d_bytes, data, n, cudaMemcpyHostToDevice, c->stream) != cudaSuccess) return 0;
     cudaMemcpyAsync(c->d_frame_off, &off, 4, cudaMemcpyHostToDevice, c->stream);
     cudaMemcpyAsync(c->d_slot, &len, 4, cudaMemcpyHostToDevice, c->stream);
     k_crc32c_batch<<<1, 32, 0, c->stream>>>(c->d_bytes, c->d_frame_off, c->d_slot, 1, (uint32_t*)c->d_aux, c->d_crc_adv, init_crc);
     cudaMemcpyAsync(&out, c->d_aux, 4, cudaMemcpyDeviceToHost, c->stream);
     cudaStreamSynchronize(c->stream);
-    c->uploaded = false; c->executed = false;
     return out;
 }
 // butil::snappy::MaxCompressedLength / RawCompress / GetUncompressedLength / RawUncompress (third_party/snappy/snappy.h:112-141)
@@ -1507,6 +1513,13 @@ extern "C" int b2_hpack_reset(b2_ctx* c, uint32_t conn, uint32_t max_table_size)
     return B2_OK;
 }
 
+// the items of a call on connection state, grouped by connection: the first item of every group, then n; false when a connection has two
+template <class Conn> static bool conn_groups(uint32_t n, Conn conn, std::vector<uint32_t>& first) {
+    for (uint32_t i = 0; i < n; i++) if (i == 0 || conn(i) != conn(i - 1)) first.push_back(i);
+    first.push_back(n);
+    for (size_t g = 0; g + 1 < first.size(); g++) for (size_t g2 = g + 1; g2 + 1 < first.size(); g2++) if (conn(first[g]) == conn(first[g2])) return false;
+    return true;
+}
 extern "C" int b2_hpack_decode_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_hpack_block* blocks, uint32_t n,
                                      void* out, uint32_t per_block_cap, uint32_t* out_lens, int32_t* status, uint32_t* n_headers) {
     if (!c || !bytes || !blocks || !out || !out_lens || !status || !n_headers) { set_err("null argument"); return B2_E_INVAL; }
@@ -1516,16 +1529,13 @@ extern "C" int b2_hpack_decode_batch(b2_ctx* c, const void* bytes, uint32_t nbyt
     for (uint32_t i = 0; i < n; i++) {
         if (blocks[i].conn >= B2_HPACK_MAX_CONNS || (uint64_t)blocks[i].offset + blocks[i].length > nbytes) { set_err("bad block"); return B2_E_INVAL; }
         conn[i] = blocks[i].conn; off[i] = blocks[i].offset; len[i] = blocks[i].length;
-        if (i == 0 || conn[i] != conn[i - 1]) first.push_back(i);
     }
-    const uint32_t n_groups = (uint32_t)first.size();
-    first.push_back(n);
-    for (uint32_t g = 0; g < n_groups; g++)                       // a connection may appear in one group only
-        for (uint32_t g2 = g + 1; g2 < n_groups; g2++) if (conn[first[g]] == conn[first[g2]]) { set_err("blocks of one connection must be adjacent"); return B2_E_INVAL; }
+    if (!conn_groups(n, [&](uint32_t i) { return conn[i]; }, first)) { set_err("blocks of one connection must be adjacent"); return B2_E_INVAL; }
+    const uint32_t n_groups = (uint32_t)first.size() - 1;
     CU(cudaSetDevice(c->opt.device));
     uint32_t* d_conn = c->d_frame_off; uint32_t* d_off = c->d_frame_run; uint32_t* d_len = c->d_slot;
     uint32_t* d_first = (uint32_t*)c->d_jobs; uint32_t* d_olens = (uint32_t*)c->d_aux; int32_t* d_st = (int32_t*)c->d_aux + n; uint32_t* d_nh = (uint32_t*)c->d_aux + 2 * (size_t)n;
-    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);       // the device copies of the last h2 batch are about to be overwritten
+    overwrites(c, kDevInput | kDevBatch);
     CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_conn, conn.data(), 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_off, off.data(), 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
@@ -1537,7 +1547,6 @@ extern "C" int b2_hpack_decode_batch(b2_ctx* c, const void* bytes, uint32_t nbyt
     CU(cudaMemcpyAsync(n_headers, d_nh, 4 * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
     if (n) CU(cudaMemcpyAsync(out, c->d_unz, (size_t)n * per_block_cap, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
-    c->uploaded = false; c->executed = false;
     return B2_OK;
 }
 
@@ -1550,7 +1559,7 @@ extern "C" int b2_h2_scan_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, c
     CU(cudaSetDevice(c->opt.device));
     static_assert(sizeof(b2_h2_frame) == sizeof(H2Frame), "frame layout");
     uint32_t* d_n = c->d_frame_off; uint32_t* d_cons = c->d_frame_run; uint32_t* d_err = c->d_slot;
-    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);       // the device copies of the last h2 batch are about to be overwritten
+    overwrites(c, kDevInput | kDevBatch);
     CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(c->d_meta, runs, sizeof(b2_run) * (size_t)n_runs, cudaMemcpyHostToDevice, c->stream));
     if (n_runs) k_h2_scan<<<(n_runs + 63) / 64, 64, 0, c->stream>>>(c->d_bytes, (const b2_run*)c->d_meta, n_runs, max_frame_size, (H2Frame*)c->d_unz, cap_per_run, d_n, d_cons, d_err);
@@ -1559,7 +1568,6 @@ extern "C" int b2_h2_scan_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, c
     CU(cudaMemcpyAsync(err, d_err, 4 * (size_t)n_runs, cudaMemcpyDeviceToHost, c->stream));
     if (n_runs) CU(cudaMemcpyAsync(frames, c->d_unz, (size_t)n_runs * cap_per_run * sizeof(b2_h2_frame), cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
-    c->uploaded = false; c->executed = false;
     return B2_OK;
 }
 
@@ -1577,6 +1585,9 @@ static int h2_ensure(b2_ctx* c) {
     CU(cudaMemset(c->d_h2_streams, 0xff, sizeof(H2Stream) * n_streams));           // id = -1: free
     return B2_OK;
 }
+// the second half of d_unz: input scratch of the h2 calls that must leave the first half alone, where the last h2 batch's out region
+// stays for b2_h2_pack_responses' zero-copy sources (B2_H2_RESP_BODY_IN_OUT / _CT_IN_OUT)
+static uint8_t* unz_upper(const b2_ctx* c) { return c->d_unz + c->opt.max_resp_bytes; }
 static H2Pool h2_pool(const b2_ctx* c) { H2Pool p; p.streams = c->d_h2_streams; p.slots = c->d_h2_slots; p.pending = c->h2_pending; p.stream_bytes = c->h2_stream_bytes; return p; }
 extern "C" int b2_h2_configure(b2_ctx* c, uint32_t max_conns, uint32_t max_pending, uint32_t stream_bytes) {
     if (!c || c->d_h2) { set_err("b2_h2_configure must precede the first h2 call on the context"); return B2_E_INVAL; }   // (b2_h2_ring_enable is an h2 call)
@@ -1630,15 +1641,18 @@ static void h2_gz_launch(b2_ctx* c, uint32_t n_runs, b2_h2_run_status* d_rs, M* 
 // k_h2_pack reads in d_aux / d_slot, its lengths in d_frame_off (free once the gunzip passes ran), group_first in d_run_tile_base,
 // the spans in d_refs, the packed replies in d_resp.
 struct H2Serve { void* replies; uint32_t replies_cap; b2_h2_reply_span* spans; };
+// the settings of the answering passes (b2_h2_serve_batch and k_h2_ring): the registered methods and the server identity
+static H2ServeCfg h2_serve_cfg(const b2_ctx* c) {
+    static_assert(sizeof(H2ServeCfg::identity) == sizeof(DevConfig::identity), "identity buffer");
+    H2ServeCfg g; g.n_methods = c->cfg.n_methods; g.identity_len = c->cfg.identity_len; memcpy(g.identity, c->cfg.identity, sizeof g.identity); return g;
+}
 static void h2_serve_launch(b2_ctx* c, uint32_t n_runs, b2_h2_run_status* d_rs, b2_h2_msg* d_msgs, uint32_t per_run, uint32_t region, uint32_t reply_region) {
     static_assert(kHeadBytes >= sizeof(b2_h2_response) && sizeof(MsgAux) >= sizeof(b2_h2_response) && sizeof(uint4) == sizeof(b2_h2_reply_span), "serve scratch");
     b2_h2_response* d_strided = reinterpret_cast<b2_h2_response*>(c->d_heads);
     b2_h2_response* d_list = reinterpret_cast<b2_h2_response*>(c->d_aux);
     b2_h2_reply_span* d_spans = reinterpret_cast<b2_h2_reply_span*>(c->d_refs);
     uint32_t* d_first = c->d_run_tile_base;
-    static_assert(sizeof(H2ServeCfg::identity) == sizeof(DevConfig::identity), "identity buffer");
-    H2ServeCfg cfg; cfg.n_methods = c->cfg.n_methods; cfg.identity_len = c->cfg.identity_len; memcpy(cfg.identity, c->cfg.identity, sizeof cfg.identity);
-    k_h2_serve<<<(n_runs + 31) / 32, 32, 0, c->stream>>>(c->d_bytes, (const b2_run*)c->d_meta, n_runs, c->d_methods, cfg, d_rs, d_msgs, per_run, c->d_unz, region,
+    k_h2_serve<<<(n_runs + 31) / 32, 32, 0, c->stream>>>(c->d_bytes, (const b2_run*)c->d_meta, n_runs, c->d_methods, h2_serve_cfg(c), d_rs, d_msgs, per_run, c->d_unz, region,
                                                          d_strided, c->d_frame_run, reply_region, d_spans);
     k_h2_serve_scan<<<1, 32, 0, c->stream>>>(n_runs, d_spans, d_first);
     k_h2_serve_compact<<<(n_runs * per_run + 255) / 256, 256, 0, c->stream>>>(n_runs, per_run, d_spans, d_first, d_strided, c->d_frame_run, d_list, c->d_slot);
@@ -1646,10 +1660,25 @@ static void h2_serve_launch(b2_ctx* c, uint32_t n_runs, b2_h2_run_status* d_rs, 
                                                                                              c->d_resp, c->d_slot, c->d_frame_off);
     k_h2_serve_gather<<<(n_runs + kH2PackWarps - 1) / kH2PackWarps, kH2PackWarps * 32, 0, c->stream>>>(n_runs, d_first, c->d_slot, c->d_frame_off, c->d_resp, d_spans);
 }
+// the runs of an h2 batch or ring ticket: inside the buffer, one per connection, on a connection the context has
+static bool h2_runs_ok(const b2_ctx* c, const b2_run* runs, uint32_t n_runs, uint32_t nbytes) {
+    for (uint32_t r = 0; r < n_runs; r++) {
+        if ((uint64_t)runs[r].offset + runs[r].length > nbytes) { set_err("run outside buffer"); return false; }
+        if (runs[r].socket_id >= c->h2_max_conns) { set_err("connection index out of range"); return false; }
+        for (uint32_t q = 0; q < r; q++) if (runs[q].socket_id == runs[r].socket_id) { set_err("one run per connection and batch"); return false; }
+    }
+    return true;
+}
+// each run of an h2 batch or ring ticket owns `region` bytes of out (acks from its start, records / bodies from region / 4), per_run
+// descriptors and reply_region bytes of the replies; fits: the least a run needs
+struct H2Split { uint32_t region, per_run, reply_region; bool fits; };
+static H2Split h2_split(uint32_t out_cap, uint32_t msg_cap, uint32_t replies_cap, uint32_t n_runs) {
+    const uint32_t region = (out_cap / n_runs) & ~63u, per_run = msg_cap / n_runs;
+    return { region, per_run, (replies_cap / n_runs) & ~63u, region >= 256 && per_run != 0 };
+}
 // ParseH2Message over a batch, server (b2_h2_msg) or client (b2_h2_call) connections: upload, the side's consume kernel (then the
-// gunzip passes, and for b2_h2_serve_batch the answering passes), and a fetch of only what was produced.  Every run owns `region` bytes
-// (acks from its start, records/bodies from region/4) and per_run descriptors: three strided copies, then the descriptors are compacted
-// into one list (run order).
+// gunzip passes, and for b2_h2_serve_batch the answering passes), and a fetch of only what was produced.  The runs' parts of out and
+// the descriptors (h2_split) come back in three strided copies, then the descriptors are compacted into one list (run order).
 template <class M>
 static int h2_parse_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
                           b2_h2_run_status* rs, M* descs, uint32_t cap, uint32_t* n_descs, void* out, uint32_t out_cap, const H2Serve* serve = nullptr) {
@@ -1661,18 +1690,14 @@ static int h2_parse_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b
     if (h2_ring_refuses(c, true)) return B2_E_INVAL;
     *n_descs = 0;
     if (n_runs == 0) return B2_OK;
-    for (uint32_t r = 0; r < n_runs; r++) {
-        if ((uint64_t)runs[r].offset + runs[r].length > nbytes) { set_err("run outside buffer"); return B2_E_INVAL; }
-        if (runs[r].socket_id >= c->h2_max_conns) { set_err("connection index out of range"); return B2_E_INVAL; }
-        for (uint32_t q = 0; q < r; q++) if (runs[q].socket_id == runs[r].socket_id) { set_err("one run per connection and batch"); return B2_E_INVAL; }
-    }
-    const uint32_t region = (out_cap / n_runs) & ~63u, per_run = cap / n_runs;
-    if (region < 256 || per_run == 0) { set_err(kClient ? "out_cap / call_cap too small for the number of runs" : "out_cap / msg_cap too small for the number of runs"); return B2_E_CAPACITY; }
+    if (!h2_runs_ok(c, runs, n_runs, nbytes)) return B2_E_INVAL;
+    const auto [region, per_run, reply_region, fits] = h2_split(out_cap, cap, serve ? serve->replies_cap : 0, n_runs);
+    if (!fits) { set_err(kClient ? "out_cap / call_cap too small for the number of runs" : "out_cap / msg_cap too small for the number of runs"); return B2_E_CAPACITY; }
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     CU(cudaSetDevice(c->opt.device));
     b2_h2_run_status* d_rs = reinterpret_cast<b2_h2_run_status*>(c->d_run_status);      // 32 B each, like b2_run_status
     M* d_descs = reinterpret_cast<M*>(c->d_msgs);                                        // 64 B each, like b2_msg_desc
-    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);       // the device copies of the last h2 batch are about to be overwritten
+    overwrites(c, kDevInput | kDevBatch);
     CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(c->d_meta, runs, sizeof(b2_run) * (size_t)n_runs, cudaMemcpyHostToDevice, c->stream));
     if constexpr (kClient) k_h2_client_consume<<<(n_runs + 31) / 32, 32, 0, c->stream>>>(c->d_bytes, (const b2_run*)c->d_meta, n_runs, c->d_h2, c->d_hpack,
@@ -1680,7 +1705,6 @@ static int h2_parse_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b
     else k_h2_consume<<<(n_runs + 31) / 32, 32, 0, c->stream>>>(c->d_bytes, (const b2_run*)c->d_meta, n_runs, c->d_h2, c->d_hpack, c->d_methods, c->cfg.n_methods,
                                                                  d_rs, d_descs, per_run, c->d_unz, region, h2_pool(c));
     if (h2_gz_wanted(c, runs, n_runs)) h2_gz_launch(c, n_runs, d_rs, d_descs, per_run, region);
-    const uint32_t reply_region = serve ? (serve->replies_cap / n_runs) & ~63u : 0;
     if constexpr (!kClient) {
         if (serve) {
             h2_serve_launch(c, n_runs, d_rs, d_descs, per_run, region, reply_region);
@@ -1712,7 +1736,6 @@ static int h2_parse_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b
     // a server batch stays readable by b2_h2_pack_responses; a client batch leaves h2_last_in / h2_last_out at 0, so that it may not
     if constexpr (!kClient) { c->h2_last_in = nbytes; c->h2_last_out = (uint64_t)region * n_runs; }
     *n_descs = total;
-    c->uploaded = false; c->executed = false;
     return B2_OK;
 }
 extern "C" int b2_h2_process_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
@@ -1744,21 +1767,17 @@ extern "C" int b2_h2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbyte
         if (r.conn >= c->h2_max_conns || (uint64_t)r.body_off + r.body_len > body_lim || (uint64_t)r.content_type_off + r.content_type_len > ct_lim ||
             (uint64_t)r.grpc_message_off + r.grpc_message_len > nbytes || r.content_type_len > 256 || r.grpc_message_len > 512) { set_err("bad response descriptor"); return B2_E_INVAL; }
         if ((r.flags & (B2_H2_RESP_BODY_IN_OUT | B2_H2_RESP_CT_IN_OUT)) && c->h2_last_out > c->opt.max_resp_bytes) { set_err("last h2 out buffer too large to stay resident"); return B2_E_CAPACITY; }
-        if (i == 0 || r.conn != resps[i - 1].conn) first.push_back(i);
         const uint64_t need = h2_reply_bound(r.body_len, r.content_type_len, r.grpc_message_len);
-        out_offs[i] = (uint32_t)total;
-        total = (total + need + 15) & ~15ull;
-        if (total > out_cap) { set_err("out_cap too small"); return B2_E_CAPACITY; }
+        if (!out_place(total, need, out_cap, &out_offs[i])) { set_err("out_cap too small"); return B2_E_CAPACITY; }
     }
-    const uint32_t n_groups = (uint32_t)first.size();
-    first.push_back(n);
-    for (uint32_t g = 0; g < n_groups; g++)
-        for (uint32_t g2 = g + 1; g2 < n_groups; g2++) if (resps[first[g]].conn == resps[first[g2]].conn) { set_err("responses of one connection must be adjacent"); return B2_E_INVAL; }
+    if (!conn_groups(n, [&](uint32_t i) { return resps[i].conn; }, first)) { set_err("responses of one connection must be adjacent"); return B2_E_INVAL; }
+    const uint32_t n_groups = (uint32_t)first.size() - 1;
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     CU(cudaSetDevice(c->opt.device));
     b2_h2_response* d_resps = reinterpret_cast<b2_h2_response*>(c->d_msgs);       // 48 B <= 64 B per entry
     uint32_t* d_first = c->d_frame_off; uint32_t* d_offs = c->d_frame_run; uint32_t* d_lens = c->d_slot;
-    uint8_t* d_aux = c->d_unz + c->opt.max_resp_bytes;            // second half of the scratch: the first half may hold the last h2 out buffer
+    uint8_t* d_aux = unz_upper(c);
+    overwrites(c, kDevBatch);
     if (nbytes) CU(cudaMemcpyAsync(d_aux, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_resps, resps, sizeof(b2_h2_response) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_first, first.data(), 4 * first.size(), cudaMemcpyHostToDevice, c->stream));
@@ -1767,7 +1786,6 @@ extern "C" int b2_h2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbyte
     CU(cudaMemcpyAsync(out_lens, d_lens, 4 * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaMemcpyAsync(out, c->d_resp, (size_t)total, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
-    c->uploaded = false; c->executed = false;
     return B2_OK;
 }
 
@@ -1796,24 +1814,21 @@ extern "C" int b2_h2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes
             hdr += nl + vl + 8; n_extra++; at += 4 + nl + vl;
         }
         if (hdr > kH2ReqFragCap || r.path_len + 16 > kH2ReqFragCap / 2 || r.authority_len + 16 > kH2ReqFragCap / 2 || r.content_type_len + 16 > kH2ReqFragCap / 2) { set_err("header block too long"); return B2_E_INVAL; }
-        if (i == 0 || r.conn != reqs[i - 1].conn) first.push_back(i);
         const uint64_t data = (uint64_t)r.body_len + 5;
         const uint64_t need = 58 + hdr + 9 + data + 9 * (data / 16384 + 4) + 13 + 16;
-        results[i].status = 0; results[i].stream_id = 0; results[i].out_off = (uint32_t)total; results[i].out_len = 0;
-        total = (total + need + 15) & ~15ull;
-        if (total > out_cap) { set_err("out_cap too small"); return B2_E_CAPACITY; }
+        results[i].status = 0; results[i].stream_id = 0; results[i].out_len = 0;
+        if (!out_place(total, need, out_cap, &results[i].out_off)) { set_err("out_cap too small"); return B2_E_CAPACITY; }
     }
-    const uint32_t n_groups = (uint32_t)first.size();
-    first.push_back(n);
-    for (uint32_t g = 0; g < n_groups; g++)
-        for (uint32_t g2 = g + 1; g2 < n_groups; g2++) if (reqs[first[g]].conn == reqs[first[g2]].conn) { set_err("requests of one connection must be adjacent"); return B2_E_INVAL; }
+    if (!conn_groups(n, [&](uint32_t i) { return reqs[i].conn; }, first)) { set_err("requests of one connection must be adjacent"); return B2_E_INVAL; }
+    const uint32_t n_groups = (uint32_t)first.size() - 1;
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     CU(cudaSetDevice(c->opt.device));
     b2_h2_request* d_reqs = reinterpret_cast<b2_h2_request*>(c->d_msgs);          // 48 B <= 64 B per entry
     b2_h2_request_result* d_res = reinterpret_cast<b2_h2_request_result*>(c->d_aux);
     static_assert(sizeof(MsgAux) >= sizeof(b2_h2_request_result), "results live in the aux array");
     uint32_t* d_first = c->d_frame_off;
-    uint8_t* d_in = c->d_unz + c->opt.max_resp_bytes;             // second half of the scratch (as b2_h2_pack_responses)
+    uint8_t* d_in = unz_upper(c);
+    overwrites(c, kDevBatch);
     CU(cudaMemcpyAsync(d_in, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_reqs, reqs, sizeof(b2_h2_request) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_res, results, sizeof(b2_h2_request_result) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
@@ -1822,7 +1837,6 @@ extern "C" int b2_h2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes
     CU(cudaMemcpyAsync(results, d_res, sizeof(b2_h2_request_result) * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaMemcpyAsync(out, c->d_resp, (size_t)total, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
-    c->uploaded = false; c->executed = false;
     return B2_OK;
 }
 extern "C" int b2_h2_conn_peer_update(b2_ctx* c, uint32_t conn, const b2_h2_peer_update* u) {
@@ -1867,11 +1881,11 @@ extern "C" int b2_h2_client_abandon_streams(b2_ctx* c, uint32_t conn, const uint
     if (!c || (!stream_ids && n)) { set_err("null argument"); return B2_E_INVAL; }
     if (h2_ring_refuses(c, true)) return B2_E_INVAL;
     if (conn >= c->h2_max_conns) { set_err("bad connection index"); return B2_E_INVAL; }
-    if ((uint64_t)n * 4 > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }   // (the ids go to the second half of the scratch)
+    if ((uint64_t)n * 4 > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }   // (the ids go to unz_upper)
     if (n == 0) return B2_OK;
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     CU(cudaSetDevice(c->opt.device));
-    uint32_t* d_ids = reinterpret_cast<uint32_t*>(c->d_unz + c->opt.max_resp_bytes);   // second half of the scratch (as b2_h2_pack_requests)
+    uint32_t* d_ids = reinterpret_cast<uint32_t*>(unz_upper(c));
     CU(cudaMemcpyAsync(d_ids, stream_ids, 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
     k_h2_client_abandon<<<1, 1, 0, c->stream>>>(c->d_h2, conn, d_ids, n, h2_pool(c));
     CU(cudaStreamSynchronize(c->stream));
@@ -1896,14 +1910,12 @@ extern "C" int b2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes, c
         if ((uint64_t)r.payload_off + r.payload_len > nbytes || (uint64_t)r.attachment_off + r.attachment_len > nbytes) { set_err("payload outside buffer"); return B2_E_INVAL; }
         const uint64_t pb = 6ull + r.payload_len;
         const uint64_t need = 12 + 512 + (r.compress_type == B2_COMPRESS_TYPE_SNAPPY ? snappy_max_compressed_length((uint32_t)pb) : pb) + r.attachment_len;
-        out_offs[i] = (uint32_t)total;
-        total = (total + need + 15) & ~15ull;
-        if (total > out_cap) { set_err("out_cap too small"); return B2_E_CAPACITY; }
+        if (!out_place(total, need, out_cap, &out_offs[i])) { set_err("out_cap too small"); return B2_E_CAPACITY; }
     }
     CU(cudaSetDevice(c->opt.device));
     ReqDesc* d_reqs = reinterpret_cast<ReqDesc*>(c->d_msgs);
     uint32_t* d_offs = c->d_frame_off; uint32_t* d_lens = c->d_slot;
-    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);       // the device copies of the last h2 batch are about to be overwritten
+    overwrites(c, kDevInput | kDevBatch);
     if (nbytes) CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_reqs, reqs, sizeof(b2_request) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_offs, out_offs, 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
@@ -1911,7 +1923,6 @@ extern "C" int b2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes, c
     CU(cudaMemcpyAsync(out_lens, d_lens, 4 * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaMemcpyAsync(out, c->d_resp, (size_t)total, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
-    c->uploaded = false; c->executed = false;
     return B2_OK;
 }
 
@@ -1938,14 +1949,12 @@ extern "C" int b2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbytes, 
         }
         const uint64_t body = r.compress_type == B2_COMPRESS_TYPE_SNAPPY ? snappy_max_compressed_length(r.body_len) : r.body_len;
         const uint64_t need = 12 + 128 + r.error_text_len + r.checksum_value_len + 11ull * r.n_extra_streams + uf + body + r.attachment_len;
-        out_offs[i] = (uint32_t)total;
-        total = (total + need + 15) & ~15ull;
-        if (total > out_cap) { set_err("out_cap too small"); return B2_E_CAPACITY; }
+        if (!out_place(total, need, out_cap, &out_offs[i])) { set_err("out_cap too small"); return B2_E_CAPACITY; }
     }
     CU(cudaSetDevice(c->opt.device));
     ReplyDesc* d_reps = reinterpret_cast<ReplyDesc*>(c->d_msgs);
     uint32_t* d_offs = c->d_frame_off; uint32_t* d_lens = c->d_slot;
-    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);
+    overwrites(c, kDevInput | kDevBatch);
     if (nbytes) CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_reps, reps, sizeof(b2_reply) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(d_offs, out_offs, 4 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
@@ -1953,7 +1962,6 @@ extern "C" int b2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbytes, 
     CU(cudaMemcpyAsync(out_lens, d_lens, 4 * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaMemcpyAsync(out, c->d_resp, (size_t)total, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
-    c->uploaded = false; c->executed = false;
     return B2_OK;
 }
 
@@ -1963,7 +1971,7 @@ static H2RingDev h2_ring_dev(const b2_ctx* c) {
     H.off_args = c->h2r_off_args; H.off_rs = c->h2r_off_rs; H.off_msgs = c->h2r_off_msgs; H.off_spans = c->h2r_off_spans;
     H.off_out = c->h2r_off_out; H.off_replies = c->h2r_off_replies;
     H.conns = c->d_h2; H.hps = c->d_hpack; H.methods = c->d_methods; H.n_methods = c->cfg.n_methods; H.pool = h2_pool(c);
-    H.cfg.n_methods = c->cfg.n_methods; H.cfg.identity_len = c->cfg.identity_len; memcpy(H.cfg.identity, c->cfg.identity, sizeof H.cfg.identity);
+    H.cfg = h2_serve_cfg(c);
     // the scratch of b2_h2_serve_batch (h2_parse_batch, h2_gz_launch, h2_serve_launch)
     H.rs = reinterpret_cast<b2_h2_run_status*>(c->d_run_status); H.msgs = reinterpret_cast<b2_h2_msg*>(c->d_msgs); H.out = c->d_unz;
     H.merge = c->d_h2_gz_merge; H.gz = c->d_frame_off;
@@ -2003,37 +2011,28 @@ extern "C" int b2_h2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, 
     // the argument checks of b2_h2_serve_batch (h2_parse_batch) with the caps of b2_h2_ring_enable, and the slot's staging size
     if (nbytes > c->h2r_max_bytes) { set_err("batch larger than b2_h2_ring_enable's max_bytes: use b2_h2_serve_batch"); return B2_E_CAPACITY; }
     if (n_runs > c->opt.max_runs) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
-    for (uint32_t r = 0; r < n_runs; r++) {
-        if ((uint64_t)runs[r].offset + runs[r].length > nbytes) { set_err("run outside buffer"); return B2_E_INVAL; }
-        if (runs[r].socket_id >= c->h2_max_conns) { set_err("connection index out of range"); return B2_E_INVAL; }
-        for (uint32_t q = 0; q < r; q++) if (runs[q].socket_id == runs[r].socket_id) { set_err("one run per connection and batch"); return B2_E_INVAL; }
-    }
-    H2RingArgs a;
-    a.region = (c->h2r_out_cap / n_runs) & ~63u; a.per_run = c->h2r_msg_cap / n_runs; a.reply_region = (c->h2r_replies_cap / n_runs) & ~63u;
-    if (a.region < 256 || a.per_run == 0) { set_err("out_cap / msg_cap too small for the number of runs"); return B2_E_CAPACITY; }
-    a.gunzip = h2_gz_wanted(c, runs, n_runs) ? 1u : 0u;
+    if (!h2_runs_ok(c, runs, n_runs, nbytes)) return B2_E_INVAL;
+    const H2Split sp = h2_split(c->h2r_out_cap, c->h2r_msg_cap, c->h2r_replies_cap, n_runs);
+    if (!sp.fits) { set_err("out_cap / msg_cap too small for the number of runs"); return B2_E_CAPACITY; }
+    const H2RingArgs a = { sp.per_run, sp.region, sp.reply_region, h2_gz_wanted(c, runs, n_runs) ? 1u : 0u };
     const uint32_t t = c->ring_next, si = t % kRingSlots;
     if (!c->ring_collected[si]) { set_err("submit ring full: b2_h2_ring_wait the oldest ticket first"); return B2_E_CAPACITY; }
-    c->h2_last_in = 0; c->h2_last_out = 0; input_overwritten(c);       // the device copies of the last h2 batch are about to be overwritten
-    c->uploaded = false; c->executed = false;
+    overwrites(c, kDevInput | kDevBatch);
     uint8_t* slot = c->ring_slots + (size_t)si * c->ring_stride;
     RingSlotHdr* h = reinterpret_cast<RingSlotHdr*>(slot);
     h->bytes_dev = ring_stage(c, slot, bytes, nbytes);
     memcpy(slot + c->ring_off_runs, runs, sizeof(b2_run) * (size_t)n_runs);
     memcpy(slot + c->h2r_off_args, &a, sizeof a);
     h->n_runs = n_runs; h->nbytes = nbytes;
-    c->ring_bytes[si] = bytes; c->ring_collected[si] = false;
-    return ring_ring(c, h, t, ticket);
+    return ring_ring(c, h, t, bytes, ticket);
 }
 extern "C" int b2_h2_ring_wait(b2_ctx* c, uint32_t ticket, b2_h2_ring_result* out) {
-    if (!c || !out || !c->h2_ring || !c->ring_slots || ticket == 0 || ticket >= c->ring_next || ticket + kRingSlots < c->ring_next) { set_err("bad h2 ring ticket"); return B2_E_INVAL; }
     static_assert(sizeof(b2_h2_ring_result) == 64, "h2 ring result ABI layout");
-    const uint32_t si = ticket % kRingSlots;
-    const uint8_t* slot = c->ring_slots + (size_t)si * c->ring_stride;
+    const uint8_t* slot = ring_ticket_slot(c, c && out && c->h2_ring, ticket, "bad h2 ring ticket");
+    if (!slot) return B2_E_INVAL;
     const RingSlotHdr* h = reinterpret_cast<const RingSlotHdr*>(slot);
-    if (c->ring_collected[si]) { set_err("ticket already collected"); return B2_E_INVAL; }
     { int rc = ring_spin(c, h, ticket); if (rc != B2_OK) return rc; }
-    c->ring_collected[si] = true;
+    c->ring_collected[ticket % kRingSlots] = true;
     const uint32_t n_runs = h->n_runs;
     const b2_h2_run_status* rs = reinterpret_cast<const b2_h2_run_status*>(slot + c->h2r_off_rs);
     uint32_t n_msgs = 0;
@@ -2041,7 +2040,7 @@ extern "C" int b2_h2_ring_wait(b2_ctx* c, uint32_t ticket, b2_h2_ring_result* ou
     memset(out, 0, sizeof *out);
     out->runs = rs; out->n_runs = n_runs; out->n_msgs = n_msgs;
     out->msgs = reinterpret_cast<const b2_h2_msg*>(slot + c->h2r_off_msgs);
-    out->out = slot + c->h2r_off_out; out->region = (c->h2r_out_cap / n_runs) & ~63u;
+    out->out = slot + c->h2r_off_out; out->region = h2_split(c->h2r_out_cap, c->h2r_msg_cap, c->h2r_replies_cap, n_runs).region;
     out->replies = slot + c->h2r_off_replies; out->spans = reinterpret_cast<const b2_h2_reply_span*>(slot + c->h2r_off_spans);
     if (n_msgs > c->h2r_msg_cap) { out->n_msgs = 0; out->status = B2_E_CAPACITY; }
     // the most recent ticket's input and out regions stay on the device: b2_h2_pack_responses may take bodies and content-types from them

@@ -574,7 +574,9 @@ int  b2_h2_process_batch(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const 
  * Response i's bytes land at out + out_offs[i] (filled by the call), out_lens[i] long.  User-defined response headers
  * are not covered.  bytes may be NULL (nbytes 0) when every field uses a zero-copy source. */
 #define B2_H2_RESP_GRPC 1u
-/* zero-copy sources: the buffers of the LAST b2_h2_process_batch on this context are still on the device */
+/* zero-copy sources: the buffers of the LAST b2_h2_process_batch on this context are still on the device.  A later call that
+ * overwrites the context's device input ends that, b2_ring_submit included (k_ring pulls every ticket there): the flags are then
+ * refused with B2_E_INVAL. */
 #define B2_H2_RESP_BODY_IN_INPUT 2u   /* body_off indexes that call's input bytes (e.g. an echoed B2_H2_FLAG_BODY_IN_INPUT message) */
 #define B2_H2_RESP_BODY_IN_OUT   4u   /* body_off indexes that call's out buffer */
 #define B2_H2_RESP_CT_IN_OUT     8u   /* content_type_off indexes that call's out buffer (the request's own content-type value) */
