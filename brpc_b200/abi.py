@@ -1,5 +1,7 @@
 """ctypes binding of include/b2rpc.h (brpc_b200/libb2rpc.so)."""
+import atexit
 import ctypes as C
+import gc
 import os
 
 import numpy as np
@@ -97,6 +99,15 @@ class H2RingResult(C.Structure):
 assert C.sizeof(H2RingResult) == 64
 
 
+class H2ClientRingResult(C.Structure):
+    _fields_ = [("runs", C.c_void_p), ("n_runs", C.c_uint32), ("n_calls", C.c_uint32), ("calls", C.c_void_p), ("out", C.c_void_p),
+                ("region", C.c_uint32), ("n_reqs", C.c_uint32), ("reqs", C.c_void_p), ("req_out", C.c_void_p), ("status", C.c_int32),
+                ("reserved", C.c_uint32)]
+
+
+assert C.sizeof(H2ClientRingResult) == 64
+
+
 class StreamState(C.Structure):
     _fields_ = [("local_consumed", C.c_uint64), ("remote_consumed", C.c_uint64), ("pending_bytes", C.c_uint32), ("flags", C.c_uint32),
                 ("error_code", C.c_int32), ("reserved", C.c_uint32)]
@@ -187,6 +198,9 @@ def _load():
     l.b2_h2_ring_enable.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]
     l.b2_h2_ring_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
     l.b2_h2_ring_wait.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(H2RingResult)]
+    l.b2_h2_client_ring_enable.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]
+    l.b2_h2_client_ring_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
+    l.b2_h2_client_ring_wait.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(H2ClientRingResult)]
     l.b2_h2_pack_responses.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     l.b2_pack_requests.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     l.b2_pack_responses.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
@@ -215,7 +229,7 @@ ABI_SYMBOLS = ["b2_ctx_create", "b2_ctx_destroy", "b2_last_error", "b2_version",
                "b2_h2_client_conn_reset", "b2_h2_client_process_batch", "b2_h2_client_abandon_streams", "b2_h2_conn_set_gunzip",
                "b2_h2_serve_batch", "b2_stream_configure", "b2_stream_open", "b2_stream_set_connected", "b2_stream_close", "b2_stream_query",
                "b2_stream_take_pending", "b2_stream_results", "b2_stream_write", "b2_stream_ring_enable", "b2_h2_ring_enable", "b2_h2_ring_submit",
-               "b2_h2_ring_wait"]
+               "b2_h2_ring_wait", "b2_h2_client_ring_enable", "b2_h2_client_ring_submit", "b2_h2_client_ring_wait"]
 
 ECHO_METHOD = dict(service_full_name=b"example.EchoService", service_name=b"EchoService", method_name=b"Echo",
                    request_type_name=b"example.EchoRequest", handler=1, echo_attachment=1,
@@ -226,6 +240,30 @@ def _check(rc):
     if rc < 0:
         raise B2Error(rc, (lib.b2_last_error() or b"").decode("utf-8", "replace"))
     return rc
+
+
+# The cyclic garbage collector runs at whatever allocation crosses its threshold — inside a latency loop as well — and b2_ctx_destroy waits
+# for the whole device, including another context's resident ring kernel until that one idles out (B2_RING_IDLE_MS).  A Context the
+# collector reclaims is therefore destroyed at the next safe point instead: the next Context creation or close(), or exit.
+_in_gc = [False]
+_reclaimed = []
+
+
+def _gc_phase(phase, info):
+    _in_gc[0] = phase == "start"
+
+
+def _destroy_reclaimed():
+    hs = _reclaimed[:]
+    del _reclaimed[:]
+    for h in hs:
+        lib.b2_ring_stop(h)          # every resident kernel among them leaves first: each destroy waits for the device
+    for h in hs:
+        lib.b2_ctx_destroy(h)
+
+
+gc.callbacks.append(_gc_phase)
+atexit.register(_destroy_reclaimed)
 
 
 class PinnedBuffer:
@@ -255,6 +293,7 @@ class Context:
 
     def __init__(self, device=0, max_batch_bytes=64 << 20, max_msgs=1 << 20, max_runs=4096, max_resp_bytes=0,
                  tile_bytes=0, max_body_size=0, methods=(ECHO_METHOD,), server_identity=None, stream_handler=0):
+        _destroy_reclaimed()
         opt = Options(device, max_batch_bytes, max_msgs, max_runs, max_resp_bytes, tile_bytes, max_body_size)
         h = C.c_void_p()
         _check(lib.b2_ctx_create(C.byref(opt), C.byref(h)))
@@ -271,10 +310,15 @@ class Context:
         if getattr(self, "_h", None):
             lib.b2_ctx_destroy(self._h)
             self._h = None
+        _destroy_reclaimed()
 
     def __del__(self):
         try:
-            self.close()
+            if _in_gc[0] and getattr(self, "_h", None):
+                _reclaimed.append(self._h)
+                self._h = None
+            else:
+                self.close()
         except Exception:
             pass
 
@@ -697,6 +741,41 @@ class Context:
         rep_end = int((spans["off"].astype(np.int64) + spans["len"]).max()) if n else 0
         return (view(res.runs, 32 * n, H2_RUN_STATUS_DT), view(res.msgs, 64 * res.n_msgs, H2_MSG_DT), view(res.out, res.region * n),
                 view(res.replies, rep_end), spans)
+
+    # ---- h2/gRPC client connections on the latency path (b2_h2_client_ring_*) ----
+    def h2_client_ring_enable(self, max_bytes, call_cap, out_cap, max_reqs, req_out_cap):
+        """Run client connections on the resident k_h2_client_ring with these per-ticket caps (b2_h2_client_ring_enable): after
+        h2_configure, before the first ring call."""
+        _check(lib.b2_h2_client_ring_enable(self._h, max_bytes, call_cap, out_cap, max_reqs, req_out_cap))
+
+    def h2_client_ring_submit(self, data, runs, reqs, ptr=None, nbytes=None):
+        """One turn of a client's event loop: the server's bytes of client connections (runs[i].socket_id = connection) are parsed as by
+        h2_client_process_batch, then reqs (H2_REQUEST_DT, offsets into the same data) are packed as by h2_pack_requests.  Either list may
+        be empty, not both.  Returns the ticket."""
+        runs = np.ascontiguousarray(runs, dtype=RUN_DT); reqs = np.ascontiguousarray(reqs, dtype=H2_REQUEST_DT)
+        if ptr is None:
+            data = np.ascontiguousarray(data, dtype=np.uint8); ptr, nbytes = data.ctypes.data, data.nbytes
+            self._ring_keep = data
+        t = C.c_uint32(0)
+        _check(lib.b2_h2_client_ring_submit(self._h, ptr, nbytes, runs.ctypes.data if len(runs) else None, len(runs),
+                                            reqs.ctypes.data if len(reqs) else None, len(reqs), C.byref(t)))
+        return t.value
+
+    def h2_client_ring_wait(self, ticket):
+        """(run_status, calls, out, req_results, [frames per request]) of the ticket, as h2_client_process_batch and h2_pack_requests return
+        them: views of the ticket's pinned slot, valid until the slot is reused by the 8th later submission (the frames are copies)."""
+        res = H2ClientRingResult()
+        _check(lib.b2_h2_client_ring_wait(self._h, ticket, C.byref(res)))
+        if res.status < 0:
+            raise B2Error(res.status, "h2 client ring ticket %d" % ticket)
+
+        def view(ptr, nbytes, dt=np.uint8):
+            return np.ctypeslib.as_array((C.c_uint8 * nbytes).from_address(ptr)).view(dt) if nbytes else np.zeros(0, dt)
+        reqs = view(res.reqs, 16 * res.n_reqs, H2_REQUEST_RESULT_DT)
+        end = int((reqs["out_off"].astype(np.int64) + reqs["out_len"]).max()) if res.n_reqs else 0
+        frames = view(res.req_out, end)
+        return (view(res.runs, 32 * res.n_runs, H2_RUN_STATUS_DT), view(res.calls, 64 * res.n_calls, H2_CALL_DT), view(res.out, res.region * res.n_runs),
+                reqs, [frames[int(r["out_off"]):int(r["out_off"]) + int(r["out_len"])].tobytes() for r in reqs])
 
     def pack_requests(self, data, reqs, out_cap=None):
         """reqs: REQUEST_DT array (offsets into data).  Returns the packed frame of every request (b"" = rejected)."""

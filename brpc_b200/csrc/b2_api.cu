@@ -70,6 +70,9 @@ struct b2_ctx {
     // parts of a slot behind its header, runs and staged input
     bool h2_ring = false; uint32_t h2r_max_bytes = 0, h2r_msg_cap = 0, h2r_out_cap = 0, h2r_replies_cap = 0;
     uint32_t h2r_off_args = 0, h2r_off_rs = 0, h2r_off_msgs = 0, h2r_off_spans = 0, h2r_off_out = 0, h2r_off_replies = 0;
+    // h2/gRPC client connections on the ring (b2_h2_client_ring_enable): the context runs k_h2_client_ring.  Its caps and slot parts
+    bool h2c_ring = false; uint32_t h2c_max_bytes = 0, h2c_call_cap = 0, h2c_out_cap = 0, h2c_max_reqs = 0, h2c_req_out_cap = 0;
+    uint32_t h2c_off_args = 0, h2c_off_reqs = 0, h2c_off_rs = 0, h2c_off_calls = 0, h2c_off_out = 0, h2c_off_req_res = 0, h2c_off_req_out = 0;
     ulonglong2* d_iov = nullptr; b2_iovec* h_iov = nullptr; const void* host_bytes = nullptr;      // B2_RESP_IOVEC
     uint4* d_refs = nullptr; b2_resp_ref* h_refs = nullptr; int input_mode = B2_INPUT_COPY, resp_mode = B2_RESP_COPY; const uint8_t* pull_bytes = nullptr;
     uint32_t* d_crc_adv = nullptr; unsigned long long* d_counters = nullptr; uint32_t* d_totals = nullptr; DevMethod* d_methods = nullptr;
@@ -179,12 +182,13 @@ extern "C" uint64_t b2_block_pool_host_allocs(void) { std::lock_guard<std::mutex
 static void ring_halt(b2_ctx* c);
 static void stream_free(b2_ctx* c);
 static bool ring_busy(const b2_ctx* c) { for (uint32_t k = 0; k < kRingSlots; k++) if (!c->ring_collected[k]) return true; return false; }
-// Every call that uploads to the context or touches h2 state is refused while an h2 ring ticket is outstanding: the ticket uses the same
-// device scratch and connection state.  A call that writes h2 connection state also retires k_h2_ring first: the resident CTA reads that
-// state through L1, and a launch boundary is where L1 is known not to hold lines another kernel wrote since.
+// Every call that uploads to the context or touches h2 state is refused while a ticket of an h2 ring (k_h2_ring or k_h2_client_ring) is
+// outstanding: the ticket uses the same device scratch and connection state.  A call that writes h2 connection state also retires the
+// resident kernel first: the resident CTA reads that state through L1, and a launch boundary is where L1 is known not to hold lines
+// another kernel wrote since.
 static bool h2_ring_refuses(b2_ctx* c, bool writes_h2_state) {
-    if (!c->h2_ring) return false;
-    if (ring_busy(c)) { set_err("an h2 ring ticket is outstanding: b2_h2_ring_wait it first"); return true; }
+    if (!c->h2_ring && !c->h2c_ring) return false;
+    if (ring_busy(c)) { set_err(c->h2_ring ? "an h2 ring ticket is outstanding: b2_h2_ring_wait it first" : "an h2 client ring ticket is outstanding: b2_h2_client_ring_wait it first"); return true; }
     if (writes_h2_state) ring_halt(c);
     return false;
 }
@@ -1059,7 +1063,7 @@ extern "C" int b2_stream_write(b2_ctx* c, const void* bytes, uint32_t nbytes, co
 
 extern "C" int b2_stream_ring_enable(b2_ctx* c, uint32_t out_bytes) {
     if (!c || !c->has_streams) { set_err("no stream table (b2_stream_configure)"); return B2_E_INVAL; }
-    if (c->st_ring || c->ring_slots || c->h2_ring) { set_err("b2_stream_ring_enable: once, before the context's first ring call"); return B2_E_INVAL; }
+    if (c->st_ring || c->ring_slots || c->h2_ring || c->h2c_ring) { set_err("b2_stream_ring_enable: once, before the context's first ring call"); return B2_E_INVAL; }
     if (out_bytes > (256u << 20)) { set_err("out_bytes above 256 MiB"); return B2_E_CAPACITY; }
     CU(cudaSetDevice(c->opt.device));
     CU(cudaStreamSynchronize(c->stream));
@@ -1082,7 +1086,8 @@ static void ring_halt(b2_ctx* c) {
     c->ring_ctl[0] = 0; c->ring_ctl[1] = 0; __sync_synchronize();
 }
 static H2RingDev h2_ring_dev(const b2_ctx* c);
-// (re)launches the context's resident kernel: k_h2_ring after b2_h2_ring_enable, else k_ring
+static H2ClientRingDev h2_client_ring_dev(const b2_ctx* c);
+// (re)launches the context's resident kernel: k_h2_ring after b2_h2_ring_enable, k_h2_client_ring after b2_h2_client_ring_enable, else k_ring
 static int ring_launch(b2_ctx* c) {
     RingDev R;
     R.slots = c->ring_slots; R.slot_stride = c->ring_stride; R.off_runs = c->ring_off_runs; R.off_in = c->ring_off_in; R.off_out = c->ring_off_out;
@@ -1094,6 +1099,14 @@ static int ring_launch(b2_ctx* c) {
         const H2RingDev H = h2_ring_dev(c);
         c->ring_ctl[1] = 1; __sync_synchronize();
         k_h2_ring<<<1, kSmallThreads, kH2RingSmem, c->ring_stream>>>(R, H);
+        c->ring_launches++;
+        CU(cudaGetLastError());
+        return B2_OK;
+    }
+    if (c->h2c_ring) {
+        const H2ClientRingDev H = h2_client_ring_dev(c);
+        c->ring_ctl[1] = 1; __sync_synchronize();
+        k_h2_client_ring<<<1, kSmallThreads, kH2ClientRingSmem, c->ring_stream>>>(R, H);
         c->ring_launches++;
         CU(cudaGetLastError());
         return B2_OK;
@@ -1192,6 +1205,7 @@ extern "C" int b2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, con
     if (!c || !bytes || !runs || !ticket || n_runs == 0) { set_err("null argument"); return B2_E_INVAL; }
     if (c->has_streams && !c->st_ring) { set_err("the ring path runs the stream pass only after b2_stream_ring_enable: use b2_batch_submit on a context with a stream table"); return B2_E_INVAL; }
     if (c->h2_ring) { set_err("this context's ring serves h2 (b2_h2_ring_enable): use b2_h2_ring_submit"); return B2_E_INVAL; }
+    if (c->h2c_ring) { set_err("this context's ring serves h2 client connections (b2_h2_client_ring_enable): use b2_h2_client_ring_submit"); return B2_E_INVAL; }
     if (nbytes > kSmallBytes || n_runs > kSmallRuns) { set_err("b2_ring_submit serves batches up to 128 KiB / 512 runs: use b2_batch_submit"); return B2_E_CAPACITY; }
     if (!c->ring_slots) { int rc = b2_ring_start(c); if (rc != B2_OK) return rc; }
     const uint32_t t = c->ring_next, si = t % kRingSlots;
@@ -1216,6 +1230,7 @@ extern "C" int b2_ring_wait(b2_ctx* c, uint32_t ticket, b2_batch_result* out) {
     RingSlotHdr* h = reinterpret_cast<RingSlotHdr*>(slot);
     if (c->st_ring && ticket != c->ring_next_wait) { set_err("a context whose ring runs the stream pass collects its tickets in ticket order"); return B2_E_INVAL; }
     if (c->h2_ring) { set_err("this context's ring serves h2: use b2_h2_ring_wait"); return B2_E_INVAL; }
+    if (c->h2c_ring) { set_err("this context's ring serves h2 client connections: use b2_h2_client_ring_wait"); return B2_E_INVAL; }
     { int rc = ring_spin(c, h, ticket); if (rc != B2_OK) return rc; }
     c->ring_collected[si] = true;
     if (c->st_ring) c->ring_next_wait = ticket + 1;
@@ -1789,16 +1804,11 @@ extern "C" int b2_h2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbyte
     return B2_OK;
 }
 
-// client side of h2: see include/b2rpc.h
-extern "C" int b2_h2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_h2_request* reqs, uint32_t n,
-                                   void* out, uint32_t out_cap, b2_h2_request_result* results) {
-    if (!c || !bytes || !reqs || !out || !results) { set_err("null argument"); return B2_E_INVAL; }
-    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
-    static_assert(sizeof(b2_h2_request) == 48 && sizeof(b2_h2_request_result) == 16, "h2 request ABI layout");
-    if (nbytes > c->opt.max_resp_bytes || n > c->opt.max_msgs || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
-    if (n == 0) return B2_OK;
-    std::vector<uint32_t> first;
-    uint64_t total = 0;
+// the requests of b2_h2_pack_requests or of a client ring ticket: every descriptor inside bytes, header blocks that fit the kernel's
+// fragment (kH2ReqFragCap), requests of one connection adjacent (first: the connection groups), and each request's room in out placed
+// (results[i].out_off, the rest of results[i] zeroed; total: the bytes placed)
+static int h2_place_requests(const b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_h2_request* reqs, uint32_t n, uint32_t out_cap,
+                             b2_h2_request_result* results, std::vector<uint32_t>& first, uint64_t& total) {
     for (uint32_t i = 0; i < n; i++) {
         const b2_h2_request& r = reqs[i];
         if (r.conn >= c->h2_max_conns || (uint64_t)r.path_off + r.path_len > nbytes || (uint64_t)r.authority_off + r.authority_len > nbytes ||
@@ -1820,6 +1830,19 @@ extern "C" int b2_h2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes
         if (!out_place(total, need, out_cap, &results[i].out_off)) { set_err("out_cap too small"); return B2_E_CAPACITY; }
     }
     if (!conn_groups(n, [&](uint32_t i) { return reqs[i].conn; }, first)) { set_err("requests of one connection must be adjacent"); return B2_E_INVAL; }
+    return B2_OK;
+}
+// client side of h2: see include/b2rpc.h
+extern "C" int b2_h2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_h2_request* reqs, uint32_t n,
+                                   void* out, uint32_t out_cap, b2_h2_request_result* results) {
+    if (!c || !bytes || !reqs || !out || !results) { set_err("null argument"); return B2_E_INVAL; }
+    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
+    static_assert(sizeof(b2_h2_request) == 48 && sizeof(b2_h2_request_result) == 16, "h2 request ABI layout");
+    if (nbytes > c->opt.max_resp_bytes || n > c->opt.max_msgs || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    if (n == 0) return B2_OK;
+    std::vector<uint32_t> first;
+    uint64_t total = 0;
+    { int rc = h2_place_requests(c, bytes, nbytes, reqs, n, out_cap, results, first, total); if (rc != B2_OK) return rc; }
     const uint32_t n_groups = (uint32_t)first.size() - 1;
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     CU(cudaSetDevice(c->opt.device));
@@ -2045,5 +2068,105 @@ extern "C" int b2_h2_ring_wait(b2_ctx* c, uint32_t ticket, b2_h2_ring_result* ou
     if (n_msgs > c->h2r_msg_cap) { out->n_msgs = 0; out->status = B2_E_CAPACITY; }
     // the most recent ticket's input and out regions stay on the device: b2_h2_pack_responses may take bodies and content-types from them
     if (ticket + 1 == c->ring_next) { c->h2_last_in = h->nbytes; c->h2_last_out = (uint64_t)out->region * n_runs; }
+    return B2_OK;
+}
+
+// ---- h2/gRPC client connections on the latency path: k_h2_client_ring on the same submit ring (include/b2rpc.h, b2_h2_client_ring_enable)
+static H2ClientRingDev h2_client_ring_dev(const b2_ctx* c) {
+    H2ClientRingDev H;
+    H.off_args = c->h2c_off_args; H.off_reqs = c->h2c_off_reqs; H.off_rs = c->h2c_off_rs; H.off_calls = c->h2c_off_calls; H.off_out = c->h2c_off_out;
+    H.off_req_res = c->h2c_off_req_res; H.off_req_out = c->h2c_off_req_out;
+    H.conns = c->d_h2; H.hps = c->d_hpack; H.pool = h2_pool(c);
+    // the scratch of b2_h2_client_process_batch (h2_parse_batch, h2_gz_launch); the request block in the head rows, which the client parse
+    // leaves alone (b2_h2_pack_requests' own d_msgs / d_aux / d_frame_off would overlap the calls and gz words), the frames in d_resp
+    static_assert(kHeadBytes >= sizeof(b2_h2_request) + sizeof(b2_h2_request_result) + 4, "request block in the head rows");
+    H.rs = reinterpret_cast<b2_h2_run_status*>(c->d_run_status); H.calls = reinterpret_cast<b2_h2_call*>(c->d_msgs); H.out = c->d_unz;
+    H.merge = c->d_h2_gz_merge; H.gz = c->d_frame_off; H.first = c->d_run_tile_base;
+    H.reqs = c->d_heads; H.req_out = c->d_resp;
+    return H;
+}
+extern "C" int b2_h2_client_ring_enable(b2_ctx* c, uint32_t max_bytes, uint32_t call_cap, uint32_t out_cap, uint32_t max_reqs, uint32_t req_out_cap) {
+    if (!c) { set_err("null argument"); return B2_E_INVAL; }
+    if (c->h2_ring || c->h2c_ring || c->ring_slots || c->st_ring) { set_err("b2_h2_client_ring_enable: once, before the context's first ring call, and not with another ring kind"); return B2_E_INVAL; }
+    if (max_bytes == 0 || call_cap == 0 || out_cap == 0 || max_reqs == 0 || req_out_cap == 0) { set_err("capacities must be non-zero"); return B2_E_INVAL; }
+    // the limits of b2_h2_client_process_batch and b2_h2_pack_requests, both of which read the ticket's bytes
+    if (max_bytes > c->opt.max_batch_bytes || max_bytes > c->opt.max_resp_bytes || call_cap > c->opt.max_msgs || out_cap > 2ull * c->opt.max_resp_bytes ||
+        max_reqs > c->opt.max_msgs || req_out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    int rc = h2_ensure(c); if (rc != B2_OK) return rc;
+    CU(cudaSetDevice(c->opt.device));
+    static_assert(sizeof(RingSlotHdr) + sizeof(H2ClientRingArgs) <= 256, "h2 client ring slot header");
+    // [RingSlotHdr | args | runs | staged input | requests + placed results + group_first | statuses | calls | out | request results | frames]
+    auto up = [](uint64_t v) { return (uint32_t)((v + 255u) & ~255ull); };
+    const uint64_t runs = (uint64_t)c->opt.max_runs;
+    c->h2c_off_args = sizeof(RingSlotHdr);
+    c->ring_off_runs = 256;
+    c->ring_off_in = up(c->ring_off_runs + runs * sizeof(b2_run));
+    c->h2c_off_reqs = up((uint64_t)c->ring_off_in + max_bytes + 16);
+    c->h2c_off_rs = up((uint64_t)c->h2c_off_reqs + h2c_ring_block(max_reqs, max_reqs));
+    c->h2c_off_calls = up(c->h2c_off_rs + runs * sizeof(b2_h2_run_status));
+    c->h2c_off_out = up(c->h2c_off_calls + (uint64_t)call_cap * sizeof(b2_h2_call));
+    c->h2c_off_req_res = up((uint64_t)c->h2c_off_out + out_cap + 16);
+    c->h2c_off_req_out = up(c->h2c_off_req_res + (uint64_t)max_reqs * sizeof(b2_h2_request_result));
+    rc = ring_alloc(c, (uint64_t)c->h2c_off_req_out + req_out_cap + 16); if (rc != B2_OK) return rc;
+    CU(cudaFuncSetAttribute(k_h2_client_ring, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kH2ClientRingSmem));
+    c->h2c_max_bytes = max_bytes; c->h2c_call_cap = call_cap; c->h2c_out_cap = out_cap; c->h2c_max_reqs = max_reqs; c->h2c_req_out_cap = req_out_cap;
+    c->h2c_ring = true;
+    return B2_OK;
+}
+extern "C" int b2_h2_client_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
+                                        const b2_h2_request* reqs, uint32_t n_reqs, uint32_t* ticket) {
+    if (!c || !bytes || !ticket || (!runs && n_runs) || (!reqs && n_reqs)) { set_err("null argument"); return B2_E_INVAL; }
+    if (n_runs == 0 && n_reqs == 0) { set_err("a ticket carries runs, requests or both"); return B2_E_INVAL; }
+    if (!c->h2c_ring) { set_err("b2_h2_client_ring_enable first"); return B2_E_INVAL; }
+    // the argument checks of b2_h2_client_process_batch and b2_h2_pack_requests with the caps of b2_h2_client_ring_enable
+    if (nbytes > c->h2c_max_bytes) { set_err("ticket larger than b2_h2_client_ring_enable's max_bytes: use the batch calls"); return B2_E_CAPACITY; }
+    if (n_runs > c->opt.max_runs || n_reqs > c->h2c_max_reqs) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    H2Split sp = { 0, 0, 0, true };
+    if (n_runs) {
+        if (!h2_runs_ok(c, runs, n_runs, nbytes)) return B2_E_INVAL;
+        sp = h2_split(c->h2c_out_cap, c->h2c_call_cap, 0, n_runs);
+        if (!sp.fits) { set_err("out_cap / call_cap too small for the number of runs"); return B2_E_CAPACITY; }
+    }
+    const uint32_t t = c->ring_next, si = t % kRingSlots;
+    if (!c->ring_collected[si]) { set_err("submit ring full: b2_h2_client_ring_wait the oldest ticket first"); return B2_E_CAPACITY; }
+    std::vector<uint32_t> first;
+    std::vector<b2_h2_request_result> placed(n_reqs);
+    uint64_t total = 0;
+    if (n_reqs) { int rc = h2_place_requests(c, bytes, nbytes, reqs, n_reqs, c->h2c_req_out_cap, placed.data(), first, total); if (rc != B2_OK) return rc; }
+    const H2ClientRingArgs a = { sp.per_run, sp.region, n_runs && h2_gz_wanted(c, runs, n_runs) ? 1u : 0u, n_reqs, n_reqs ? (uint32_t)first.size() - 1 : 0u, { 0, 0, 0 } };
+    overwrites(c, kDevInput | kDevBatch);
+    uint8_t* slot = c->ring_slots + (size_t)si * c->ring_stride;
+    uint8_t* block = slot + c->h2c_off_reqs;                     // the request block the kernel pulls: requests, placed results, group_first
+    if (n_reqs) {
+        memcpy(block, reqs, sizeof(b2_h2_request) * (size_t)n_reqs);
+        memcpy(block + h2c_ring_res_off(n_reqs), placed.data(), sizeof(b2_h2_request_result) * (size_t)n_reqs);
+        memcpy(block + h2c_ring_first_off(n_reqs), first.data(), 4 * first.size());
+    }
+    RingSlotHdr* h = reinterpret_cast<RingSlotHdr*>(slot);
+    h->bytes_dev = ring_stage(c, slot, bytes, nbytes);
+    if (n_runs) memcpy(slot + c->ring_off_runs, runs, sizeof(b2_run) * (size_t)n_runs);
+    memcpy(slot + c->h2c_off_args, &a, sizeof a);
+    h->n_runs = n_runs; h->nbytes = nbytes;
+    return ring_ring(c, h, t, bytes, ticket);
+}
+extern "C" int b2_h2_client_ring_wait(b2_ctx* c, uint32_t ticket, b2_h2_client_ring_result* out) {
+    static_assert(sizeof(b2_h2_client_ring_result) == 64, "h2 client ring result ABI layout");
+    const uint8_t* slot = ring_ticket_slot(c, c && out && c->h2c_ring, ticket, "bad h2 client ring ticket");
+    if (!slot) return B2_E_INVAL;
+    const RingSlotHdr* h = reinterpret_cast<const RingSlotHdr*>(slot);
+    { int rc = ring_spin(c, h, ticket); if (rc != B2_OK) return rc; }
+    c->ring_collected[ticket % kRingSlots] = true;
+    const H2ClientRingArgs* a = reinterpret_cast<const H2ClientRingArgs*>(slot + c->h2c_off_args);
+    const uint32_t n_runs = h->n_runs;
+    const b2_h2_run_status* rs = reinterpret_cast<const b2_h2_run_status*>(slot + c->h2c_off_rs);
+    uint32_t n_calls = 0;
+    for (uint32_t r = 0; r < n_runs; r++) n_calls += rs[r].n_msgs;
+    memset(out, 0, sizeof *out);
+    out->runs = rs; out->n_runs = n_runs; out->n_calls = n_calls;
+    out->calls = reinterpret_cast<const b2_h2_call*>(slot + c->h2c_off_calls);
+    out->out = slot + c->h2c_off_out; out->region = a->region;
+    out->n_reqs = a->n_reqs;
+    out->reqs = reinterpret_cast<const b2_h2_request_result*>(slot + c->h2c_off_req_res);
+    out->req_out = slot + c->h2c_off_req_out;
     return B2_OK;
 }

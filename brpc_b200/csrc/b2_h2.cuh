@@ -692,13 +692,11 @@ constexpr uint32_t kH2ClientMode = 1u;                            // H2Conn::pad
 // The same split as k_h2_pack: one warp per connection, lane 0 runs the serial part (stream id, windows, HPACK encode against the
 // connection's table) into shared memory, the warp writes the frames.
 constexpr uint32_t kH2ReqFragCap = 2048;
-__global__ void __launch_bounds__(kH2PackWarps * 32) k_h2_pack_req(const uint8_t* bytes, const b2_h2_request* reqs, const uint32_t* group_first, uint32_t n_groups,
-                                                                   H2Conn* conns, uint8_t* out, b2_h2_request_result* results, H2Pool pool) {
-    __shared__ __align__(16) uint8_t s_buf[kH2PackWarps][2][kH2ReqFragCap];
-    const uint32_t lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    const uint32_t g = blockIdx.x * kH2PackWarps + w;
-    if (g >= n_groups) return;
-    uint8_t* frag = s_buf[w][0]; uint8_t* tmp = s_buf[w][1];
+// Connection group g, by one warp; buf: the warp's 2 * kH2ReqFragCap bytes of shared scratch; results[i].out_off placed by the host.
+// k_h2_pack_req and k_h2_client_ring call it.
+__device__ __forceinline__ void h2_pack_req_group(uint32_t g, uint32_t lane, uint8_t* buf, const uint8_t* bytes, const b2_h2_request* reqs,
+                                                  const uint32_t* group_first, H2Conn* conns, uint8_t* out, b2_h2_request_result* results, H2Pool pool) {
+    uint8_t* frag = buf; uint8_t* tmp = buf + kH2ReqFragCap;
     for (uint32_t i = group_first[g]; i < group_first[g + 1]; i++) {
         const b2_h2_request R = reqs[i];
         uint8_t* o0 = out + results[i].out_off; uint8_t* o = o0;
@@ -800,6 +798,14 @@ __global__ void __launch_bounds__(kH2PackWarps * 32) k_h2_pack_req(const uint8_t
         if (lane == 0) { results[i].status = B2_H2_REQ_OK; results[i].stream_id = sid; results[i].out_len = (uint32_t)(o - o0); }
         __syncwarp();                                                // the shared buffers are reused by the next request
     }
+}
+__global__ void __launch_bounds__(kH2PackWarps * 32) k_h2_pack_req(const uint8_t* bytes, const b2_h2_request* reqs, const uint32_t* group_first, uint32_t n_groups,
+                                                                   H2Conn* conns, uint8_t* out, b2_h2_request_result* results, H2Pool pool) {
+    __shared__ __align__(16) uint8_t s_buf[kH2PackWarps][2][kH2ReqFragCap];
+    const uint32_t lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const uint32_t g = blockIdx.x * kH2PackWarps + w;
+    if (g >= n_groups) return;
+    h2_pack_req_group(g, lane, s_buf[w][0], bytes, reqs, group_first, conns, out, results, pool);
 }
 // b2_h2_conn_peer_update: OnSettings' effect on _remote_settings (:848-915) and OnWindowUpdate on stream 0 (:1006-1041), mirrored by the host
 __global__ void k_h2_peer_update(H2Conn* conns, uint32_t conn, b2_h2_peer_update u, int* rc) {
@@ -1709,6 +1715,35 @@ __global__ void __launch_bounds__(kH2PackWarps * 32) k_h2_serve_gather(uint32_t 
 
 #if defined(B2_KERNELS_RING)
 // ---------------------------------------------------------------------------------------------------------
+// The block phases k_h2_ring and k_h2_client_ring share.  The four gunzip passes over the ticket's parse (the whole CTA, __syncthreads()
+// where the batch call has kernel boundaries).
+template <class M>
+__device__ __forceinline__ void h2_ring_gunzip(uint32_t n_runs, uint32_t per_run, uint32_t region, const uint8_t* bytes, const b2_run* runs,
+                                               const H2Conn* conns, b2_h2_run_status* rs, M* msgs, uint8_t* out, uint8_t* merge, uint32_t* gz) {
+    const uint32_t tid = threadIdx.x, n_slots = n_runs * per_run;
+    for (uint32_t r = tid; r < n_runs; r += kSmallThreads) h2_gz_select_run(r, bytes, runs, conns, rs, msgs, per_run, out, merge, gz);
+    __syncthreads();
+    for (uint32_t i = tid; i < n_slots; i += kSmallThreads) h2_gz_size_one(i, bytes, rs, msgs, per_run, out, gz);
+    __syncthreads();
+    for (uint32_t r = tid; r < n_runs; r += kSmallThreads) h2_gz_place_run(r, rs, msgs, per_run, region, gz);
+    __syncthreads();
+    for (uint32_t i = tid; i < n_slots; i += kSmallThreads) h2_gz_inflate_one(i, bytes, rs, msgs, per_run, out, gz);
+    __syncthreads();
+}
+// The push of run r, by one warp: its descriptors into the list at first[r] (the batch call compacts them on the host), its control
+// bytes and blob (whose length the status reports in first_msg) at the offsets the batch call uses, then the status with first_msg =
+// the list index.
+template <class M>
+__device__ __forceinline__ void h2_ring_push_run(uint32_t r, uint32_t lane, uint8_t* slot, uint32_t off_rs, uint32_t off_descs, uint32_t off_out,
+                                                 const b2_h2_run_status* rs, const M* descs, uint32_t per_run, const uint8_t* out, uint32_t region,
+                                                 const uint32_t* first) {
+    b2_h2_run_status st = rs[r];
+    const uint32_t f = first[r], base = r * region;
+    ring_push(slot + off_descs + (size_t)f * sizeof(M), reinterpret_cast<const uint8_t*>(descs + (size_t)r * per_run), st.n_msgs * (uint32_t)sizeof(M), lane, 32);
+    ring_push(slot + off_out + base, out + base, st.ctrl_len, lane, 32);
+    ring_push(slot + off_out + base + region / 4, out + base + region / 4, st.first_msg, lane, 32);
+    if (lane == 0) { st.first_msg = f; reinterpret_cast<b2_h2_run_status*>(slot + off_rs)[r] = st; }
+}
 // k_h2_ring: b2_h2_serve_batch on the latency path (b2_h2_ring_*).  One resident CTA, fed through the same submit ring as k_ring
 // (ring_doorbell / ring_pull / ring_push / ring_stamp / ring_release of b2_kernels.cuh): per ticket the passes of the batch call, as block phases with
 // __syncthreads() where the batch call has kernel boundaries, on the same device scratch, then only the used parts are pushed into the
@@ -1752,16 +1787,7 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_h2_ring(RingDev R, H2RingD
         for (uint32_t r = tid; r < n_runs; r += kSmallThreads)
             h2_consume_run<false>(r, bytes, runs, H.conns, H.hps, H.methods, H.n_methods, H.rs, H.msgs, per_run, H.out, region, H.pool);
         __syncthreads();
-        if (s_args.gunzip) {                                          // a run's connection opted in (b2_h2_conn_set_gunzip)
-            for (uint32_t r = tid; r < n_runs; r += kSmallThreads) h2_gz_select_run(r, bytes, runs, H.conns, H.rs, H.msgs, per_run, H.out, H.merge, H.gz);
-            __syncthreads();
-            for (uint32_t i = tid; i < n_slots; i += kSmallThreads) h2_gz_size_one(i, bytes, H.rs, H.msgs, per_run, H.out, H.gz);
-            __syncthreads();
-            for (uint32_t r = tid; r < n_runs; r += kSmallThreads) h2_gz_place_run(r, H.rs, H.msgs, per_run, region, H.gz);
-            __syncthreads();
-            for (uint32_t i = tid; i < n_slots; i += kSmallThreads) h2_gz_inflate_one(i, bytes, H.rs, H.msgs, per_run, H.out, H.gz);
-            __syncthreads();
-        }
+        if (s_args.gunzip) h2_ring_gunzip(n_runs, per_run, region, bytes, runs, H.conns, H.rs, H.msgs, H.out, H.merge, H.gz);   // a run's connection opted in
         for (uint32_t r = tid; r < n_runs; r += kSmallThreads)
             h2_serve_run(r, bytes, runs, H.methods, H.cfg, H.rs, H.msgs, per_run, H.out, region, H.strided, H.strided_offs, reply_region, H.spans);
         __syncthreads();
@@ -1778,21 +1804,91 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_h2_ring(RingDev R, H2RingD
         // the descriptors become one list in run order (the batch call compacts them on the host): first[r] = run r's first list index
         if (wid == 0) h2_warp_scan_runs(n_runs, lane, [&](uint32_t r) { return H.rs[r].n_msgs; }, H.first);
         __syncthreads();
-        // push, a warp per run: its descriptors into the list, its control bytes and blob (whose length the status reports in first_msg)
-        // at the offsets the batch call uses, its replies, then the status with first_msg = the list index, and the span
+        // push, a warp per run: h2_ring_push_run, then its replies and span
         for (uint32_t r = wid; r < n_runs; r += kSmallWarps) {
-            b2_h2_run_status st = H.rs[r];
             const b2_h2_reply_span sp = H.spans[r];
-            const uint32_t f = H.first[r], base = r * region;
-            ring_push(slot + H.off_msgs + (size_t)f * sizeof(b2_h2_msg), reinterpret_cast<const uint8_t*>(H.msgs + (size_t)r * per_run), st.n_msgs * (uint32_t)sizeof(b2_h2_msg), lane, 32);
-            ring_push(slot + H.off_out + base, H.out + base, st.ctrl_len, lane, 32);
-            ring_push(slot + H.off_out + base + region / 4, H.out + base + region / 4, st.first_msg, lane, 32);
+            h2_ring_push_run(r, lane, slot, H.off_rs, H.off_msgs, H.off_out, H.rs, H.msgs, per_run, H.out, region, H.first);
             ring_push(slot + H.off_replies + sp.off, H.replies + sp.off, sp.len, lane, 32);
-            if (lane == 0) {
-                st.first_msg = f;
-                reinterpret_cast<b2_h2_run_status*>(slot + H.off_rs)[r] = st;
-                reinterpret_cast<b2_h2_reply_span*>(slot + H.off_spans)[r] = sp;
-            }
+            if (lane == 0) reinterpret_cast<b2_h2_reply_span*>(slot + H.off_spans)[r] = sp;
+        }
+        if (tid == 0) ring_stamp(hdr, t);
+        __threadfence_system();
+        __syncthreads();
+        if (tid == 0) ring_release(R, hdr, ticket);
+        ticket++;
+    }
+    if (tid == 0) R.next_ticket[0] = ticket;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// k_h2_client_ring: one turn of a client's event loop on the latency path (b2_h2_client_ring_*): b2_h2_client_process_batch over the
+// ticket's runs, then b2_h2_pack_requests over its requests, as block phases on the same device scratch, so that what the runs change
+// (SETTINGS, WINDOW_UPDATE, GOAWAY, ended calls) governs the requests of the same ticket.  The requests, their placed results and
+// group_first are pulled from the slot into scratch the parse does not use, and their fields index the pulled input; frames go to
+// the offsets the host placed, and only out_len bytes of each are pushed.  Connection state is read through L1, as in k_h2_ring.
+struct H2ClientRingArgs { uint32_t per_run, region, gunzip, n_reqs, n_groups, pad[3]; };   // per ticket, from the host, at the slot's off_args
+struct H2ClientRingDev {
+    // the slot's parts behind RingSlotHdr (runs, staged input: RingDev); off_reqs: [requests | placed results | group_first] of the ticket
+    uint32_t off_args, off_reqs, off_rs, off_calls, off_out, off_req_res, off_req_out;
+    H2Conn* conns; HpackState* hps; H2Pool pool;
+    // the scratch of b2_h2_client_process_batch (statuses, per_run-strided calls, out regions, gunzip merge scratch and words, then the
+    // first list index of every run's calls), the pulled request block, and the frames of b2_h2_pack_requests
+    b2_h2_run_status* rs; b2_h2_call* calls; uint8_t* out; uint8_t* merge; uint32_t* gz; uint32_t* first;
+    uint8_t* reqs; uint8_t* req_out;
+};
+// the request block of a ticket: n requests, their results (out_off placed), then group_first (n_groups + 1 words); all parts 16-byte aligned
+B2_HD uint32_t h2c_ring_res_off(uint32_t n) { return n * (uint32_t)sizeof(b2_h2_request); }
+B2_HD uint32_t h2c_ring_first_off(uint32_t n) { return h2c_ring_res_off(n) + n * (uint32_t)sizeof(b2_h2_request_result); }
+B2_HD uint32_t h2c_ring_block(uint32_t n, uint32_t n_groups) { return h2c_ring_first_off(n) + (((n_groups + 1) * 4 + 15u) & ~15u); }
+constexpr uint32_t kH2ClientRingSmem = kSmallWarps * 2 * kH2ReqFragCap;  // k_h2_pack_req's scratch for each warp
+__global__ void __launch_bounds__(kSmallThreads, 1) k_h2_client_ring(RingDev R, H2ClientRingDev H) {
+    extern __shared__ __align__(16) uint8_t h2c_ring_raw[];
+    __shared__ uint32_t s_go;
+    __shared__ RingSlotHdr s_hdr;
+    __shared__ H2ClientRingArgs s_args;
+    const uint32_t tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const uint8_t* bytes = R.d_bytes;
+    const b2_run* runs = reinterpret_cast<const b2_run*>(R.d_meta);
+    uint32_t ticket = R.next_ticket[0];
+    for (;;) {
+        uint8_t* slot = R.slots + (size_t)(ticket % kRingSlots) * R.slot_stride;
+        RingSlotHdr* hdr = reinterpret_cast<RingSlotHdr*>(slot);
+        if (tid == 0) s_go = ring_doorbell(R, hdr, ticket);
+        __syncthreads();
+        if (!s_go) break;
+        unsigned long long t[4] = { 0, 0, 0, 0 };                    // doorbell seen, header read, bytes pulled, requests packed
+        if (tid == 0) t[0] = globaltimer_ns();
+        ring_pull(R, slot, s_hdr, R.d_meta, t[1]);
+        if (tid < sizeof(H2ClientRingArgs) / 4) reinterpret_cast<uint32_t*>(&s_args)[tid] = ld_sys_u32(reinterpret_cast<const volatile uint32_t*>(slot + H.off_args) + tid);
+        __threadfence();
+        __syncthreads();
+        if (tid == 0) t[2] = globaltimer_ns();
+        const uint32_t n_runs = s_hdr.n_runs, per_run = s_args.per_run, region = s_args.region, n_reqs = s_args.n_reqs, n_groups = s_args.n_groups;
+        const b2_h2_request* reqs = reinterpret_cast<const b2_h2_request*>(H.reqs);
+        b2_h2_request_result* res = reinterpret_cast<b2_h2_request_result*>(H.reqs + h2c_ring_res_off(n_reqs));
+        const uint32_t* group_first = reinterpret_cast<const uint32_t*>(H.reqs + h2c_ring_first_off(n_reqs));
+        {   // the request block, while the parse below has not yet run (nothing reads it before the pack phase)
+            const uint4* src = reinterpret_cast<const uint4*>(slot + H.off_reqs);
+            uint4* dst = reinterpret_cast<uint4*>(H.reqs);
+            for (uint32_t k = tid; k < h2c_ring_block(n_reqs, n_groups) / 16u; k += kSmallThreads) dst[k] = src[k];
+        }
+        for (uint32_t r = tid; r < n_runs; r += kSmallThreads)
+            h2_consume_run<true>(r, bytes, runs, H.conns, H.hps, nullptr, 0, H.rs, H.calls, per_run, H.out, region, H.pool);
+        __syncthreads();
+        if (s_args.gunzip) h2_ring_gunzip(n_runs, per_run, region, bytes, runs, H.conns, H.rs, H.calls, H.out, H.merge, H.gz);   // a run's connection opted in
+        for (uint32_t g = wid; g < n_groups; g += kSmallWarps)
+            h2_pack_req_group(g, lane, h2c_ring_raw + wid * 2 * kH2ReqFragCap, bytes, reqs, group_first, H.conns, H.req_out, res, H.pool);
+        __syncthreads();
+        if (tid == 0) t[3] = globaltimer_ns();
+        if (wid == 0) h2_warp_scan_runs(n_runs, lane, [&](uint32_t r) { return H.rs[r].n_msgs; }, H.first);
+        __syncthreads();
+        // push: a warp per run (h2_ring_push_run), the request results, then a warp per request its frames
+        for (uint32_t r = wid; r < n_runs; r += kSmallWarps)
+            h2_ring_push_run(r, lane, slot, H.off_rs, H.off_calls, H.off_out, H.rs, H.calls, per_run, H.out, region, H.first);
+        ring_push(slot + H.off_req_res, reinterpret_cast<const uint8_t*>(res), n_reqs * (uint32_t)sizeof(b2_h2_request_result), tid, kSmallThreads);
+        for (uint32_t i = wid; i < n_reqs; i += kSmallWarps) {
+            const b2_h2_request_result q = res[i];
+            ring_push(slot + H.off_req_out + q.out_off, H.req_out + q.out_off, q.out_len, lane, 32);
         }
         if (tid == 0) ring_stamp(hdr, t);
         __threadfence_system();

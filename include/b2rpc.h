@@ -804,6 +804,42 @@ typedef struct b2_h2_ring_result {    /* views into the ticket's pinned slot, va
 int  b2_h2_ring_enable(b2_ctx* ctx, uint32_t max_bytes, uint32_t msg_cap, uint32_t out_cap, uint32_t replies_cap);
 int  b2_h2_ring_submit(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs, uint32_t* ticket);
 int  b2_h2_ring_wait(b2_ctx* ctx, uint32_t ticket, b2_h2_ring_result* out);
+/* h2/gRPC CLIENT connections on the latency path: b2_h2_client_process_batch followed by b2_h2_pack_requests inside a resident kernel
+ * (k_h2_client_ring) fed through the same submit ring.  A ticket is one turn of a client's event loop: read what arrived, then send what
+ * is queued.  The runs (the bytes read from client sockets, socket_id = connection) are parsed as by b2_h2_client_process_batch, then the
+ * requests are packed as by b2_h2_pack_requests; their fields index the same `bytes` as the runs.  So within one ticket a SETTINGS or
+ * WINDOW_UPDATE in the runs governs how its requests are framed and charged, a GOAWAY in the runs makes its later stream ids
+ * B2_H2_REQ_LOGOFF, and calls that end in the runs free their stream records before the requests take records (B2_H2_REQ_NO_ROOM).
+ * For each connection write its run's control bytes (ctrl_off / ctrl_len) first, then its request frames in request order.
+ * A context runs exactly one of k_ring, k_h2_ring and k_h2_client_ring: b2_ring_submit / _wait, b2_h2_ring_* and b2_stream_ring_enable
+ * refuse a context that runs this one, and b2_h2_client_ring_enable refuses a context that ran another.
+ * b2_h2_client_ring_enable: once, after b2_h2_configure and before the context's first ring call (else B2_E_INVAL).  The caps are per
+ * ticket and play the roles of the batch calls' nbytes bound (both), call_cap and out_cap (b2_h2_client_process_batch), and the number
+ * of requests and out_cap (b2_h2_pack_requests); they are checked against the context limits those calls check and fix the slot layout.
+ * b2_ring_stop, b2_ring_launches, b2_ring_phase_ns ([2]: requests packed) and B2_RING_IDLE_MS apply as to k_h2_ring.
+ * b2_h2_client_ring_submit: every check of both batch calls with the enable-time caps; n_runs or n_reqs may be 0, not both.  Bytes in
+ * b2_block_alloc memory are pulled in place, others staged into the slot.
+ * b2_h2_client_ring_wait: tickets may be waited in any order.  For any sequence of tickets the results equal, byte for byte, what a context
+ * returns for the same sequence of b2_h2_client_process_batch(bytes, runs, call_cap, out_cap) + b2_h2_pack_requests(bytes, reqs,
+ * req_out_cap) (a call whose list is empty skipped): run statuses and calls, the defined bytes of out, request results and each request's
+ * frames — and so does the connection state left behind (HPACK tables, windows, deferred WINDOW_UPDATEs, the pending map, stream ids,
+ * GOAWAY).  A client ticket leaves nothing for b2_h2_pack_responses to read zero-copy, as the client batch call.
+ * While a ticket is outstanding the calls b2_h2_ring_wait lists above fail with B2_E_INVAL, and the calls that write h2 connection state
+ * (b2_h2_client_conn_reset / _abandon_streams, b2_h2_conn_set_gunzip / _peer_update / _set_next_stream_id, ...) retire the kernel between
+ * tickets; the next submission relaunches it (b2_ring_launches counts it). */
+typedef struct b2_h2_client_ring_result {       /* views into the ticket's pinned slot, valid until the 8th later submission */
+    const b2_h2_run_status* runs; uint32_t n_runs, n_calls;
+    const b2_h2_call* calls;                    /* compacted: runs[i].first_msg is a list index */
+    const uint8_t* out; uint32_t region;        /* run i's control bytes and blob at out + i * region, as in the batch call */
+    uint32_t n_reqs;
+    const b2_h2_request_result* reqs;           /* status, stream_id, out_off, out_len */
+    const uint8_t* req_out;                     /* request i's frames at req_out + reqs[i].out_off */
+    int32_t status; uint32_t reserved;
+} b2_h2_client_ring_result;                     /* 64 bytes */
+int  b2_h2_client_ring_enable(b2_ctx* ctx, uint32_t max_bytes, uint32_t call_cap, uint32_t out_cap, uint32_t max_reqs, uint32_t req_out_cap);
+int  b2_h2_client_ring_submit(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
+                              const b2_h2_request* reqs, uint32_t n_reqs, uint32_t* ticket);
+int  b2_h2_client_ring_wait(b2_ctx* ctx, uint32_t ticket, b2_h2_client_ring_result* out);
 
 /* ---- streaming_rpc, the receiving side of a Stream on the device ------------------------------------------------------------------
  * Without a stream table a STRM frame ends as a B2_MSG_STREAM_FRAME descriptor and the host rebuilds brpc's Stream from the list.  With
