@@ -242,6 +242,11 @@ def _check(rc):
     return rc
 
 
+def _view(ptr, nbytes, dtype=np.uint8):
+    """nbytes of context-owned memory at ptr as a dtype array (no copy)"""
+    return np.ctypeslib.as_array((C.c_uint8 * nbytes).from_address(ptr)).view(dtype) if nbytes else np.zeros(0, dtype)
+
+
 # The cyclic garbage collector runs at whatever allocation crosses its threshold — inside a latency loop as well — and b2_ctx_destroy waits
 # for the whole device, including another context's resident ring kernel until that one idles out (B2_RING_IDLE_MS).  A Context the
 # collector reclaims is therefore destroyed at the next safe point instead: the next Context creation or close(), or exit.
@@ -348,6 +353,13 @@ class Context:
         return {"kernel_ms": res.kernel_ms, "n_launches": res.n_launches, "refs": refs, "iov": iov}
 
     # ---- the persistent latency kernel (b2_ring_*) ----
+    def _ring_bytes(self, data, ptr, nbytes):
+        """a ticket's bytes: (ptr, nbytes) as given, else data's, which the context keeps referenced until the next submission"""
+        if ptr is None:
+            data = np.ascontiguousarray(data, dtype=np.uint8); ptr, nbytes = data.ctypes.data, data.nbytes
+            self._ring_keep = data
+        return ptr, nbytes
+
     def ring_start(self):
         _check(lib.b2_ring_start(self._h))
 
@@ -356,9 +368,7 @@ class Context:
 
     def ring_submit(self, data, runs, ptr=None, nbytes=None):
         runs = np.ascontiguousarray(runs, dtype=RUN_DT)
-        if ptr is None:
-            data = np.ascontiguousarray(data, dtype=np.uint8); ptr, nbytes = data.ctypes.data, data.nbytes
-            self._ring_keep = data
+        ptr, nbytes = self._ring_bytes(data, ptr, nbytes)
         t = C.c_uint32(0)
         _check(lib.b2_ring_submit(self._h, ptr, nbytes, runs.ctypes.data, len(runs), C.byref(t)))
         return t.value
@@ -498,11 +508,8 @@ class Context:
         next batch call (a ring ticket's: until its slot is reused)."""
         r = StreamBatchResult()
         _check(lib.b2_stream_results(self._h, C.byref(r)))
-
-        def view(ptr, nbytes, dt):
-            return np.ctypeslib.as_array((C.c_uint8 * nbytes).from_address(ptr)).view(dt) if nbytes else np.zeros(0, dt)
-        return (view(r.msgs, 32 * r.n_msgs, STREAM_MSG_DT), view(r.events, 80 * r.n_events, STREAM_EVENT_DT), view(r.out, r.out_bytes, np.uint8),
-                view(r.ctrl, r.ctrl_bytes, np.uint8), view(r.run_ctrl, 8 * r.n_runs, np.uint32).reshape(-1, 2))
+        return (_view(r.msgs, 32 * r.n_msgs, STREAM_MSG_DT), _view(r.events, 80 * r.n_events, STREAM_EVENT_DT), _view(r.out, r.out_bytes, np.uint8),
+                _view(r.ctrl, r.ctrl_bytes, np.uint8), _view(r.run_ctrl, 8 * r.n_runs, np.uint32).reshape(-1, 2))
 
     def stream_write(self, writes, data=None, max_segment_size=0, out_cap=None, out=None):
         """StreamWrite for a batch of writes (b2_stream_write).  writes: STREAM_WRITE_DT array or a list of (stream_id, flags, src_off,
@@ -719,9 +726,7 @@ class Context:
     def h2_ring_submit(self, data, runs, ptr=None, nbytes=None):
         """One batch of server connection runs (runs[i].socket_id = connection).  Returns the ticket."""
         runs = np.ascontiguousarray(runs, dtype=RUN_DT)
-        if ptr is None:
-            data = np.ascontiguousarray(data, dtype=np.uint8); ptr, nbytes = data.ctypes.data, data.nbytes
-            self._ring_keep = data
+        ptr, nbytes = self._ring_bytes(data, ptr, nbytes)
         t = C.c_uint32(0)
         _check(lib.b2_h2_ring_submit(self._h, ptr, nbytes, runs.ctypes.data, len(runs), C.byref(t)))
         return t.value
@@ -733,14 +738,11 @@ class Context:
         _check(lib.b2_h2_ring_wait(self._h, ticket, C.byref(res)))
         if res.status < 0:
             raise B2Error(res.status, "h2 ring ticket %d" % ticket)
-
-        def view(ptr, nbytes, dt=np.uint8):
-            return np.ctypeslib.as_array((C.c_uint8 * nbytes).from_address(ptr)).view(dt) if nbytes else np.zeros(0, dt)
         n = res.n_runs
-        spans = view(res.spans, 16 * n, H2_REPLY_SPAN_DT)
+        spans = _view(res.spans, 16 * n, H2_REPLY_SPAN_DT)
         rep_end = int((spans["off"].astype(np.int64) + spans["len"]).max()) if n else 0
-        return (view(res.runs, 32 * n, H2_RUN_STATUS_DT), view(res.msgs, 64 * res.n_msgs, H2_MSG_DT), view(res.out, res.region * n),
-                view(res.replies, rep_end), spans)
+        return (_view(res.runs, 32 * n, H2_RUN_STATUS_DT), _view(res.msgs, 64 * res.n_msgs, H2_MSG_DT), _view(res.out, res.region * n),
+                _view(res.replies, rep_end), spans)
 
     # ---- h2/gRPC client connections on the latency path (b2_h2_client_ring_*) ----
     def h2_client_ring_enable(self, max_bytes, call_cap, out_cap, max_reqs, req_out_cap):
@@ -753,9 +755,7 @@ class Context:
         h2_client_process_batch, then reqs (H2_REQUEST_DT, offsets into the same data) are packed as by h2_pack_requests.  Either list may
         be empty, not both.  Returns the ticket."""
         runs = np.ascontiguousarray(runs, dtype=RUN_DT); reqs = np.ascontiguousarray(reqs, dtype=H2_REQUEST_DT)
-        if ptr is None:
-            data = np.ascontiguousarray(data, dtype=np.uint8); ptr, nbytes = data.ctypes.data, data.nbytes
-            self._ring_keep = data
+        ptr, nbytes = self._ring_bytes(data, ptr, nbytes)
         t = C.c_uint32(0)
         _check(lib.b2_h2_client_ring_submit(self._h, ptr, nbytes, runs.ctypes.data if len(runs) else None, len(runs),
                                             reqs.ctypes.data if len(reqs) else None, len(reqs), C.byref(t)))
@@ -768,13 +768,10 @@ class Context:
         _check(lib.b2_h2_client_ring_wait(self._h, ticket, C.byref(res)))
         if res.status < 0:
             raise B2Error(res.status, "h2 client ring ticket %d" % ticket)
-
-        def view(ptr, nbytes, dt=np.uint8):
-            return np.ctypeslib.as_array((C.c_uint8 * nbytes).from_address(ptr)).view(dt) if nbytes else np.zeros(0, dt)
-        reqs = view(res.reqs, 16 * res.n_reqs, H2_REQUEST_RESULT_DT)
+        reqs = _view(res.reqs, 16 * res.n_reqs, H2_REQUEST_RESULT_DT)
         end = int((reqs["out_off"].astype(np.int64) + reqs["out_len"]).max()) if res.n_reqs else 0
-        frames = view(res.req_out, end)
-        return (view(res.runs, 32 * res.n_runs, H2_RUN_STATUS_DT), view(res.calls, 64 * res.n_calls, H2_CALL_DT), view(res.out, res.region * res.n_runs),
+        frames = _view(res.req_out, end)
+        return (_view(res.runs, 32 * res.n_runs, H2_RUN_STATUS_DT), _view(res.calls, 64 * res.n_calls, H2_CALL_DT), _view(res.out, res.region * res.n_runs),
                 reqs, [frames[int(r["out_off"]):int(r["out_off"]) + int(r["out_len"])].tobytes() for r in reqs])
 
     def pack_requests(self, data, reqs, out_cap=None):

@@ -45,6 +45,14 @@ SmallLayout small_layout(uint32_t nbytes, uint32_t n_runs, uint32_t max_msgs) {
 constexpr uint32_t kSecEvents = 64, kSecMsgs = kSecEvents + kSmallMsgs * 80, kSecCtrl = kSecMsgs + kSmallMsgs * 32,
                    kSecRunCtrl = kSecCtrl + 3 * kStreamCtrlMax * kSmallMsgs, kSecOut = kSecRunCtrl + kSmallRuns * 8;
 struct Stage { const char* name; cudaEvent_t ev; };
+// Which resident kernel a context's ring runs, fixed by its first ring call: k_ring (b2_ring_start / b2_ring_submit), k_ring with the
+// stream pass (b2_stream_ring_enable), k_h2_ring (b2_h2_ring_enable) or k_h2_client_ring (b2_h2_client_ring_enable)
+enum class RingKind { none, batch, batch_streams, h2_server, h2_client };
+// A slot's layout: the header (RingSlotHdr, then the kind's per-ticket args) in the first 256 bytes, then each part 256-byte aligned
+struct SlotLayout {
+    uint64_t end = 256;
+    uint32_t add(uint64_t bytes) { const uint64_t off = end; end = (end + bytes + 255u) & ~255ull; return (uint32_t)off; }
+};
 }
 
 struct b2_ctx {
@@ -58,21 +66,19 @@ struct b2_ctx {
     uint32_t* d_slot = nullptr; uint32_t* d_scan_tmp = nullptr; uint8_t* d_resp = nullptr; uint8_t* d_unz = nullptr; uint16_t* d_snappy_tab = nullptr; HpackState* d_hpack = nullptr; H2Conn* d_h2 = nullptr; H2Stream* d_h2_streams = nullptr; uint8_t* d_h2_slots = nullptr; uint32_t h2_max_conns = B2_H2_MAX_CONNS, h2_pending = B2_H2_MAX_PENDING, h2_stream_bytes = B2_H2_STREAM_BYTES; uint64_t h2_last_in = 0, h2_last_out = 0;   // sizes of the last h2 batch still on the device
     uint32_t* d_frame_row = nullptr; uint4* d_rows = nullptr;
     std::vector<uint8_t> h2_gunzip; uint8_t* d_h2_gz_merge = nullptr;     // host mirror of the kH2Gunzip bits; merge scratch, B2_H2_HEADER_BYTES per run
-    // persistent latency kernel (b2_ring_*): pinned + mapped submit ring, its own stream
+    // persistent latency kernel (b2_ring_*): pinned + mapped submit ring, its own stream.  ring_slots: allocated (by the first ring call
+    // that needs them); the slot parts of each kind live in that kind's kernel arguments (ring_dev: runs, staged input, output, stream section)
+    RingKind ring_kind = RingKind::none; RingDev ring_dev = {}; H2RingDev h2r_dev = {}; H2ClientRingDev h2c_dev = {};
     uint8_t* ring_slots = nullptr; volatile uint32_t* ring_ctl = nullptr; uint32_t* d_ring_ticket = nullptr; cudaStream_t ring_stream = nullptr;
-    uint32_t ring_next = 1, ring_stride = 0, ring_off_runs = 0, ring_off_in = 0, ring_off_out = 0; bool ring_collected[8] = { true, true, true, true, true, true, true, true };
+    uint32_t ring_next = 1, ring_stride = 0; bool ring_collected[8] = { true, true, true, true, true, true, true, true };
     const void* ring_bytes[8] = {}; const void* ring_pin_base = nullptr; unsigned long long ring_pin_dev = 0; uint64_t ring_launches = 0;
-    // the stream pass on the ring (b2_stream_ring_enable): the ring's StreamPass writes its results into d_st_ring, k_ring pushes them
-    // to the slot's section at ring_off_st; tickets are collected in order (ring_next_wait); st_view_ticket: the ticket b2_stream_results
-    // describes (0: the last batch call's pass)
-    bool st_ring = false; StreamPass sp_ring = {}; uint8_t* d_st_ring = nullptr; uint32_t ring_off_st = 0, ring_next_wait = 1, st_view_ticket = 0;
-    // h2/gRPC on the ring (b2_h2_ring_enable): the context runs k_h2_ring instead of k_ring.  The caps every ticket is served with, and the
-    // parts of a slot behind its header, runs and staged input
-    bool h2_ring = false; uint32_t h2r_max_bytes = 0, h2r_msg_cap = 0, h2r_out_cap = 0, h2r_replies_cap = 0;
-    uint32_t h2r_off_args = 0, h2r_off_rs = 0, h2r_off_msgs = 0, h2r_off_spans = 0, h2r_off_out = 0, h2r_off_replies = 0;
-    // h2/gRPC client connections on the ring (b2_h2_client_ring_enable): the context runs k_h2_client_ring.  Its caps and slot parts
-    bool h2c_ring = false; uint32_t h2c_max_bytes = 0, h2c_call_cap = 0, h2c_out_cap = 0, h2c_max_reqs = 0, h2c_req_out_cap = 0;
-    uint32_t h2c_off_args = 0, h2c_off_reqs = 0, h2c_off_rs = 0, h2c_off_calls = 0, h2c_off_out = 0, h2c_off_req_res = 0, h2c_off_req_out = 0;
+    // the stream pass on the ring (batch_streams): the ring's StreamPass writes its results into d_st_ring, k_ring pushes them to the
+    // slot's section; tickets are collected in order (ring_next_wait); st_view_ticket: the ticket b2_stream_results describes (0: the last
+    // batch call's pass)
+    StreamPass sp_ring = {}; uint8_t* d_st_ring = nullptr; uint32_t ring_next_wait = 1, st_view_ticket = 0;
+    // the caps every ticket of an h2 ring (k_h2_ring, k_h2_client_ring) is served with
+    uint32_t h2r_max_bytes = 0, h2r_msg_cap = 0, h2r_out_cap = 0, h2r_replies_cap = 0;
+    uint32_t h2c_max_bytes = 0, h2c_call_cap = 0, h2c_out_cap = 0, h2c_max_reqs = 0, h2c_req_out_cap = 0;
     ulonglong2* d_iov = nullptr; b2_iovec* h_iov = nullptr; const void* host_bytes = nullptr;      // B2_RESP_IOVEC
     uint4* d_refs = nullptr; b2_resp_ref* h_refs = nullptr; int input_mode = B2_INPUT_COPY, resp_mode = B2_RESP_COPY; const uint8_t* pull_bytes = nullptr;
     uint32_t* d_crc_adv = nullptr; unsigned long long* d_counters = nullptr; uint32_t* d_totals = nullptr; DevMethod* d_methods = nullptr;
@@ -182,13 +188,14 @@ extern "C" uint64_t b2_block_pool_host_allocs(void) { std::lock_guard<std::mutex
 static void ring_halt(b2_ctx* c);
 static void stream_free(b2_ctx* c);
 static bool ring_busy(const b2_ctx* c) { for (uint32_t k = 0; k < kRingSlots; k++) if (!c->ring_collected[k]) return true; return false; }
+static uint8_t* ring_slot(const b2_ctx* c, uint32_t ticket) { return c->ring_slots + (size_t)(ticket % kRingSlots) * c->ring_stride; }
 // Every call that uploads to the context or touches h2 state is refused while a ticket of an h2 ring (k_h2_ring or k_h2_client_ring) is
 // outstanding: the ticket uses the same device scratch and connection state.  A call that writes h2 connection state also retires the
 // resident kernel first: the resident CTA reads that state through L1, and a launch boundary is where L1 is known not to hold lines
 // another kernel wrote since.
 static bool h2_ring_refuses(b2_ctx* c, bool writes_h2_state) {
-    if (!c->h2_ring && !c->h2c_ring) return false;
-    if (ring_busy(c)) { set_err(c->h2_ring ? "an h2 ring ticket is outstanding: b2_h2_ring_wait it first" : "an h2 client ring ticket is outstanding: b2_h2_client_ring_wait it first"); return true; }
+    if (c->ring_kind != RingKind::h2_server && c->ring_kind != RingKind::h2_client) return false;
+    if (ring_busy(c)) { set_err(c->ring_kind == RingKind::h2_server ? "an h2 ring ticket is outstanding: b2_h2_ring_wait it first" : "an h2 client ring ticket is outstanding: b2_h2_client_ring_wait it first"); return true; }
     if (writes_h2_state) ring_halt(c);
     return false;
 }
@@ -490,7 +497,7 @@ static int launch_stream_pass(b2_ctx* c, const BatchPtrs& B, cudaStream_t s, uin
     k_stream_run<<<grid(c->st_max, 4, sms * 8), 128, 0, s>>>(B, S); CU(cudaEventRecord(c->st_ev[4], s));
     k_stream_rst<<<grid(c->n_runs, 4, sms * 4), 128, 0, s>>>(B, S); CU(cudaEventRecord(c->st_ev[5], s));
     CU(cudaMemcpyAsync(c->h_st_cnts, S.cnts, 64, cudaMemcpyDeviceToHost, s));
-    if (c->st_ring) CU(cudaMemsetAsync(S.cnt, 0, 8 * (size_t)S.cap, s));     // cnt | fill: zero when the ring's next ticket starts
+    if (c->ring_kind == RingKind::batch_streams) CU(cudaMemsetAsync(S.cnt, 0, 8 * (size_t)S.cap, s));     // cnt | fill: zero when the ring's next ticket starts
     launches += 5; c->stream_ran = true; c->st_input = B.bytes;
     return B2_OK;
 }
@@ -832,7 +839,7 @@ static int stream_configure(b2_ctx* c, uint32_t max_streams, uint32_t pending_by
 
 // a ring ticket of a context whose ring runs the stream pass is submitted and not collected: the table belongs to k_ring
 static bool ring_owns_table(const b2_ctx* c) {
-    if (!c->st_ring || !ring_busy(c)) return false;
+    if (c->ring_kind != RingKind::batch_streams || !ring_busy(c)) return false;
     set_err("a ring ticket is outstanding: b2_ring_wait it first, the stream table belongs to it");
     return true;
 }
@@ -944,7 +951,7 @@ extern "C" int b2_stream_results(b2_ctx* c, b2_stream_batch_result* out) {
     if (!c->stream_valid) { set_err("no collected batch of b2_process_batch / b2_batch_collect / b2_ring_wait"); return B2_E_INVAL; }
     memset(out, 0, sizeof *out);
     if (c->st_view_ticket) {                               // a ticket the ring served: the slot's stream section
-        const uint8_t* slot = c->ring_slots + (size_t)(c->st_view_ticket % kRingSlots) * c->ring_stride, *sec = slot + c->ring_off_st;
+        const uint8_t* slot = ring_slot(c, c->st_view_ticket), *sec = slot + c->ring_dev.off_st;
         const uint32_t* n = reinterpret_cast<const uint32_t*>(sec);
         out->msgs = reinterpret_cast<const b2_stream_msg*>(sec + kSecMsgs); out->n_msgs = n[0];
         out->events = reinterpret_cast<const b2_stream_event*>(sec + kSecEvents); out->n_events = n[1];
@@ -1063,7 +1070,7 @@ extern "C" int b2_stream_write(b2_ctx* c, const void* bytes, uint32_t nbytes, co
 
 extern "C" int b2_stream_ring_enable(b2_ctx* c, uint32_t out_bytes) {
     if (!c || !c->has_streams) { set_err("no stream table (b2_stream_configure)"); return B2_E_INVAL; }
-    if (c->st_ring || c->ring_slots || c->h2_ring || c->h2c_ring) { set_err("b2_stream_ring_enable: once, before the context's first ring call"); return B2_E_INVAL; }
+    if (c->ring_kind != RingKind::none) { set_err("b2_stream_ring_enable: once, before the context's first ring call"); return B2_E_INVAL; }
     if (out_bytes > (256u << 20)) { set_err("out_bytes above 256 MiB"); return B2_E_CAPACITY; }
     CU(cudaSetDevice(c->opt.device));
     CU(cudaStreamSynchronize(c->stream));
@@ -1074,11 +1081,11 @@ extern "C" int b2_stream_ring_enable(b2_ctx* c, uint32_t out_bytes) {
     R.events = reinterpret_cast<b2_stream_event*>(c->d_st_ring + kSecEvents); R.msgs = reinterpret_cast<b2_stream_msg*>(c->d_st_ring + kSecMsgs);
     R.ctrl = c->d_st_ring + kSecCtrl; R.run_ctrl = reinterpret_cast<uint32_t*>(c->d_st_ring + kSecRunCtrl);
     R.out = c->d_st_ring + kSecOut; R.out_cap = out_bytes;
-    c->sp_ring = R; c->st_ring = true;
+    c->sp_ring = R; c->ring_kind = RingKind::batch_streams;
     return B2_OK;
 }
 
-// ---- the persistent latency path: submit ring + resident kernel (k_ring) ---------------------------------------------------------
+// ---- the persistent latency path: submit ring + the resident kernel of the context's ring kind ------------------------------------
 static void ring_halt(b2_ctx* c) {
     if (!c->ring_ctl) return;
     c->ring_ctl[0] = 1; __sync_synchronize();
@@ -1087,38 +1094,26 @@ static void ring_halt(b2_ctx* c) {
 }
 static H2RingDev h2_ring_dev(const b2_ctx* c);
 static H2ClientRingDev h2_client_ring_dev(const b2_ctx* c);
-// (re)launches the context's resident kernel: k_h2_ring after b2_h2_ring_enable, k_h2_client_ring after b2_h2_client_ring_enable, else k_ring
+// (re)launches the resident kernel of the context's ring kind on ring_stream
 static int ring_launch(b2_ctx* c) {
-    RingDev R;
-    R.slots = c->ring_slots; R.slot_stride = c->ring_stride; R.off_runs = c->ring_off_runs; R.off_in = c->ring_off_in; R.off_out = c->ring_off_out;
-    R.ctl = c->ring_ctl; R.next_ticket = c->d_ring_ticket; R.off_st = c->ring_off_st;
+    RingDev R = c->ring_dev;                // (the slot parts)
+    R.slots = c->ring_slots; R.slot_stride = c->ring_stride; R.ctl = c->ring_ctl; R.next_ticket = c->d_ring_ticket;
     unsigned long long idle_ms = 20; if (const char* e = getenv("B2_RING_IDLE_MS")) idle_ms = (unsigned long long)atoi(e);
     R.idle_ns = idle_ms * 1000000ull;
     R.d_bytes = c->d_bytes; R.d_meta = c->d_meta; R.d_small = c->d_small;
-    if (c->h2_ring) {
-        const H2RingDev H = h2_ring_dev(c);
-        c->ring_ctl[1] = 1; __sync_synchronize();
-        k_h2_ring<<<1, kSmallThreads, kH2RingSmem, c->ring_stream>>>(R, H);
-        c->ring_launches++;
-        CU(cudaGetLastError());
-        return B2_OK;
-    }
-    if (c->h2c_ring) {
-        const H2ClientRingDev H = h2_client_ring_dev(c);
-        c->ring_ctl[1] = 1; __sync_synchronize();
-        k_h2_client_ring<<<1, kSmallThreads, kH2ClientRingSmem, c->ring_stream>>>(R, H);
-        c->ring_launches++;
-        CU(cudaGetLastError());
-        return B2_OK;
-    }
-    const bool was_small = c->small; c->small = false;
-    BatchPtrs B = make_ptrs(c);
-    c->small = was_small;
-    B.bytes = c->d_bytes;
     c->ring_ctl[1] = 1; __sync_synchronize();
-    StreamPass SP = {};                     // (tab null: the ring runs no stream pass)
-    if (c->st_ring) SP = c->sp_ring;
-    k_ring<<<1, kSmallThreads, sizeof(SmallSmem), c->ring_stream>>>(R, B, c->cfg, SP);
+    switch (c->ring_kind) {
+    case RingKind::h2_server: { const H2RingDev H = h2_ring_dev(c); k_h2_ring<<<1, kSmallThreads, kH2RingSmem, c->ring_stream>>>(R, H); break; }
+    case RingKind::h2_client: { const H2ClientRingDev H = h2_client_ring_dev(c); k_h2_client_ring<<<1, kSmallThreads, kH2ClientRingSmem, c->ring_stream>>>(R, H); break; }
+    default: {                              // batch, batch_streams
+        const bool was_small = c->small; c->small = false;
+        BatchPtrs B = make_ptrs(c);
+        c->small = was_small;
+        B.bytes = c->d_bytes;
+        const StreamPass SP = c->ring_kind == RingKind::batch_streams ? c->sp_ring : StreamPass{};   // (tab null: the ring runs no stream pass)
+        k_ring<<<1, kSmallThreads, sizeof(SmallSmem), c->ring_stream>>>(R, B, c->cfg, SP);
+    }
+    }
     c->ring_launches++;
     CU(cudaGetLastError());
     return B2_OK;
@@ -1140,20 +1135,22 @@ static int ring_alloc(b2_ctx* c, uint64_t end) {
 extern "C" int b2_ring_start(b2_ctx* c) {
     if (!c) return B2_E_INVAL;
     CU(cudaSetDevice(c->opt.device));
-    if (!c->ring_slots) {
-        c->ring_off_runs = sizeof(RingSlotHdr);
-        c->ring_off_in = (c->ring_off_runs + kSmallRuns * (uint32_t)sizeof(b2_run) + 255u) & ~255u;
-        c->ring_off_out = (c->ring_off_in + kSmallBytes + 1024u + 255u) & ~255u;
-        c->ring_off_st = (c->ring_off_out + kSmallBlock + 255u) & ~255u;
-        const uint64_t end = c->st_ring ? (uint64_t)c->ring_off_st + kSecOut + ((c->sp_ring.out_cap + 15u) & ~15u) : (uint64_t)c->ring_off_out + kSmallBlock;
-        int rc = ring_alloc(c, end); if (rc != B2_OK) return rc;
+    if (c->ring_kind == RingKind::none) c->ring_kind = RingKind::batch;
+    if (!c->ring_slots) {                   // k_ring's slot (the h2 kinds lay out theirs when enabled): [header | runs | staged input | output block | stream section]
+        SlotLayout L;
+        RingDev& R = c->ring_dev;
+        R.off_runs = L.add(kSmallRuns * sizeof(b2_run));
+        R.off_in = L.add(kSmallBytes + 1024u);
+        R.off_out = L.add(kSmallBlock);
+        if (c->ring_kind == RingKind::batch_streams) R.off_st = L.add(kSecOut + ((c->sp_ring.out_cap + 15u) & ~15u));
+        int rc = ring_alloc(c, L.end); if (rc != B2_OK) return rc;
         CU(cudaFuncSetAttribute(k_ring, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmallSmem)));
     }
     if (!c->ring_ctl[1]) return ring_launch(c);
     return B2_OK;
 }
 // the batch bytes as the kernel pulls them: in place when they already live in pinned + mapped memory (b2_block_alloc), else staged into
-// the slot at ring_off_in
+// the slot's off_in
 static unsigned long long ring_stage(b2_ctx* c, uint8_t* slot, const void* bytes, uint32_t nbytes) {
     unsigned long long dev = 0;
     if (bytes == c->ring_pin_base) dev = c->ring_pin_dev;
@@ -1163,11 +1160,28 @@ static unsigned long long ring_stage(b2_ctx* c, uint8_t* slot, const void* bytes
             dev = (unsigned long long)(uintptr_t)at.devicePointer; c->ring_pin_base = bytes; c->ring_pin_dev = dev;
         } else cudaGetLastError();
     }
-    if (!dev) { memcpy(slot + c->ring_off_in, bytes, nbytes); dev = (unsigned long long)(uintptr_t)(slot + c->ring_off_in); }
+    if (!dev) { memcpy(slot + c->ring_dev.off_in, bytes, nbytes); dev = (unsigned long long)(uintptr_t)(slot + c->ring_dev.off_in); }
     return dev;
 }
-// marks ticket t outstanding, rings its doorbell (everything else the host stores in the slot first) and relaunches the kernel if it idled out
-static int ring_ring(b2_ctx* c, RingSlotHdr* h, uint32_t t, const void* bytes, uint32_t* ticket) {
+// A submission in three steps, each kind's own parts in between.  ring_claim: the slot of the next ticket, or null when the ring is full
+// (wait_call: what frees a slot).  ring_fill: what every ticket carries — the batch bytes, the runs and their sizes in the header; the
+// resident kernel pulls them into d_bytes / d_meta and serves the ticket over the batch scratch.  ring_ring: the doorbell.
+static uint8_t* ring_claim(b2_ctx* c, const char* wait_call) {
+    if (!c->ring_collected[c->ring_next % kRingSlots]) { set_err("submit ring full: %s the oldest ticket first", wait_call); return nullptr; }
+    return ring_slot(c, c->ring_next);
+}
+static RingSlotHdr* ring_fill(b2_ctx* c, uint8_t* slot, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs) {
+    overwrites(c, kDevInput | kDevBatch);
+    RingSlotHdr* h = reinterpret_cast<RingSlotHdr*>(slot);
+    h->bytes_dev = ring_stage(c, slot, bytes, nbytes);
+    if (n_runs) memcpy(slot + c->ring_dev.off_runs, runs, sizeof(b2_run) * (size_t)n_runs);
+    h->n_runs = n_runs; h->nbytes = nbytes;
+    return h;
+}
+// marks the next ticket outstanding, rings its doorbell (everything else the host stores in the slot first) and relaunches the kernel if it
+// idled out
+static int ring_ring(b2_ctx* c, RingSlotHdr* h, const void* bytes, uint32_t* ticket) {
+    const uint32_t t = c->ring_next;
     c->ring_bytes[t % kRingSlots] = bytes; c->ring_collected[t % kRingSlots] = false;
     __sync_synchronize();
     h->submit = t;
@@ -1193,60 +1207,63 @@ static int ring_spin(b2_ctx* c, const RingSlotHdr* h, uint32_t ticket) {
     __sync_synchronize();
     return B2_OK;
 }
-// the slot of `ticket` while it is submitted and not collected; else null, with the error set (args_ok: the caller's own checks)
-static uint8_t* ring_ticket_slot(b2_ctx* c, bool args_ok, uint32_t ticket, const char* bad_ticket) {
+// The slot of `ticket` once the kernel released it, marked collected; else null, with the error set and rc the code.  args_ok: the
+// caller's own checks (bad_ticket: its text for them and for a ticket that is not outstanding).  A context whose ring runs the stream
+// pass collects in ticket order.
+static uint8_t* ring_collect(b2_ctx* c, bool args_ok, uint32_t ticket, const char* bad_ticket, int& rc) {
+    rc = B2_E_INVAL;
     if (!args_ok || !c->ring_slots || ticket == 0 || ticket >= c->ring_next || ticket + kRingSlots < c->ring_next) { set_err(bad_ticket); return nullptr; }
     if (c->ring_collected[ticket % kRingSlots]) { set_err("ticket already collected"); return nullptr; }
-    return c->ring_slots + (size_t)(ticket % kRingSlots) * c->ring_stride;
+    const bool in_order = c->ring_kind == RingKind::batch_streams;
+    if (in_order && ticket != c->ring_next_wait) { set_err("a context whose ring runs the stream pass collects its tickets in ticket order"); return nullptr; }
+    uint8_t* slot = ring_slot(c, ticket);
+    if ((rc = ring_spin(c, reinterpret_cast<const RingSlotHdr*>(slot), ticket)) != B2_OK) return nullptr;
+    c->ring_collected[ticket % kRingSlots] = true;
+    if (in_order) c->ring_next_wait = ticket + 1;
+    return slot;
 }
 extern "C" int b2_ring_stop(b2_ctx* c) { if (!c) return B2_E_INVAL; cudaSetDevice(c->opt.device); ring_halt(c); return B2_OK; }
 
 extern "C" int b2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs, uint32_t* ticket) {
     if (!c || !bytes || !runs || !ticket || n_runs == 0) { set_err("null argument"); return B2_E_INVAL; }
-    if (c->has_streams && !c->st_ring) { set_err("the ring path runs the stream pass only after b2_stream_ring_enable: use b2_batch_submit on a context with a stream table"); return B2_E_INVAL; }
-    if (c->h2_ring) { set_err("this context's ring serves h2 (b2_h2_ring_enable): use b2_h2_ring_submit"); return B2_E_INVAL; }
-    if (c->h2c_ring) { set_err("this context's ring serves h2 client connections (b2_h2_client_ring_enable): use b2_h2_client_ring_submit"); return B2_E_INVAL; }
+    if (c->has_streams && c->ring_kind != RingKind::batch_streams) { set_err("the ring path runs the stream pass only after b2_stream_ring_enable: use b2_batch_submit on a context with a stream table"); return B2_E_INVAL; }
+    if (c->ring_kind == RingKind::h2_server) { set_err("this context's ring serves h2 (b2_h2_ring_enable): use b2_h2_ring_submit"); return B2_E_INVAL; }
+    if (c->ring_kind == RingKind::h2_client) { set_err("this context's ring serves h2 client connections (b2_h2_client_ring_enable): use b2_h2_client_ring_submit"); return B2_E_INVAL; }
     if (nbytes > kSmallBytes || n_runs > kSmallRuns) { set_err("b2_ring_submit serves batches up to 128 KiB / 512 runs: use b2_batch_submit"); return B2_E_CAPACITY; }
     if (!c->ring_slots) { int rc = b2_ring_start(c); if (rc != B2_OK) return rc; }
-    const uint32_t t = c->ring_next, si = t % kRingSlots;
-    if (!c->ring_collected[si]) { set_err("submit ring full: b2_ring_wait the oldest ticket first"); return B2_E_CAPACITY; }
+    uint8_t* slot = ring_claim(c, "b2_ring_wait");
+    if (!slot) return B2_E_CAPACITY;
     for (uint32_t r = 0; r < n_runs; r++)
         if ((runs[r].offset & 15u) || (uint64_t)runs[r].offset + runs[r].length > nbytes) { set_err("run offset must be 16-aligned and inside the batch"); return B2_E_INVAL; }
-    overwrites(c, kDevInput | kDevBatch);           // k_ring pulls the ticket into d_bytes / d_meta and runs it over the batch scratch
-    uint8_t* slot = c->ring_slots + (size_t)si * c->ring_stride;
-    RingSlotHdr* h = reinterpret_cast<RingSlotHdr*>(slot);
-    const unsigned long long dev = ring_stage(c, slot, bytes, nbytes);
-    memcpy(slot + c->ring_off_runs, runs, sizeof(b2_run) * (size_t)n_runs);
+    RingSlotHdr* h = ring_fill(c, slot, bytes, nbytes, runs, n_runs);
     const SmallLayout L = small_layout(nbytes, n_runs, c->opt.max_msgs);
-    h->n_runs = n_runs; h->nbytes = nbytes; h->small_msgs = L.msgs; h->small_resp = L.resp; h->off_rs = L.off_rs; h->off_msgs = L.off_msgs;
-    h->off_refs = L.off_refs; h->off_resp = L.off_resp; h->total = L.total; h->by_ref = c->cfg.by_ref; h->bytes_dev = dev;
-    return ring_ring(c, h, t, bytes, ticket);
+    h->small_msgs = L.msgs; h->small_resp = L.resp; h->off_rs = L.off_rs; h->off_msgs = L.off_msgs;
+    h->off_refs = L.off_refs; h->off_resp = L.off_resp; h->total = L.total; h->by_ref = c->cfg.by_ref;
+    return ring_ring(c, h, bytes, ticket);
 }
 
 extern "C" int b2_ring_wait(b2_ctx* c, uint32_t ticket, b2_batch_result* out) {
-    uint8_t* slot = ring_ticket_slot(c, c && out, ticket, "bad ring ticket");
-    if (!slot) return B2_E_INVAL;
+    if (c && c->ring_kind == RingKind::h2_server) { set_err("this context's ring serves h2: use b2_h2_ring_wait"); return B2_E_INVAL; }
+    if (c && c->ring_kind == RingKind::h2_client) { set_err("this context's ring serves h2 client connections: use b2_h2_client_ring_wait"); return B2_E_INVAL; }
+    int rc;
+    uint8_t* slot = ring_collect(c, c && out, ticket, "bad ring ticket", rc);
+    if (!slot) return rc;
     const uint32_t si = ticket % kRingSlots;
+    const bool streams = c->ring_kind == RingKind::batch_streams;
     RingSlotHdr* h = reinterpret_cast<RingSlotHdr*>(slot);
-    if (c->st_ring && ticket != c->ring_next_wait) { set_err("a context whose ring runs the stream pass collects its tickets in ticket order"); return B2_E_INVAL; }
-    if (c->h2_ring) { set_err("this context's ring serves h2: use b2_h2_ring_wait"); return B2_E_INVAL; }
-    if (c->h2c_ring) { set_err("this context's ring serves h2 client connections: use b2_h2_client_ring_wait"); return B2_E_INVAL; }
-    { int rc = ring_spin(c, h, ticket); if (rc != B2_OK) return rc; }
-    c->ring_collected[si] = true;
-    if (c->st_ring) c->ring_next_wait = ticket + 1;
     memset(out, 0, sizeof *out);
-    const uint8_t* ob = slot + c->ring_off_out;
+    const uint8_t* ob = slot + c->ring_dev.off_out;
     const uint32_t* tot = reinterpret_cast<const uint32_t*>(ob);
     if (tot[2] & 3u) {
         // more messages / reply bytes than the compact block holds: the big pipeline serves the ticket.  With the stream pass on the ring,
         // k_ring ran no pass for it (the pipeline runs its own) and parks before the next one's pull until ctl[3] releases it, so that the
         // table sees the tickets in ticket order; otherwise the ring must be quiet first
-        if (!c->st_ring && ring_busy(c)) { set_err("ring overflow fallback needs the other tickets collected first"); return B2_E_CAPACITY; }
-        if (!c->st_ring) ring_halt(c);
+        if (!streams && ring_busy(c)) { set_err("ring overflow fallback needs the other tickets collected first"); return B2_E_CAPACITY; }
+        if (!streams) ring_halt(c);
         const bool allow = c->allow_small; c->allow_small = false;
-        const int rc = b2_process_batch(c, c->ring_bytes[si], h->nbytes, reinterpret_cast<const b2_run*>(slot + c->ring_off_runs), h->n_runs, out);
+        rc = b2_process_batch(c, c->ring_bytes[si], h->nbytes, reinterpret_cast<const b2_run*>(slot + c->ring_dev.off_runs), h->n_runs, out);
         c->allow_small = allow;
-        if (c->st_ring) { __sync_synchronize(); c->ring_ctl[3] = ticket; __sync_synchronize(); }
+        if (streams) { __sync_synchronize(); c->ring_ctl[3] = ticket; __sync_synchronize(); }
         return rc;
     }
     out->runs = reinterpret_cast<const b2_run_status*>(ob + h->off_rs); out->n_runs = h->n_runs;
@@ -1255,7 +1272,7 @@ extern "C" int b2_ring_wait(b2_ctx* c, uint32_t ticket, b2_batch_result* out) {
     out->refs = h->by_ref ? reinterpret_cast<const b2_resp_ref*>(ob + h->off_refs) : nullptr;
     if (c->resp_mode == B2_RESP_IOVEC) refs_to_iov(c, out, c->ring_bytes[si]);
     out->n_launches = 0; out->kernel_ms = 0.f;
-    if (c->st_ring) { c->stream_valid = true; c->st_view_ticket = ticket; c->st_input = c->d_bytes; }
+    if (streams) { c->stream_valid = true; c->st_view_ticket = ticket; c->st_input = c->d_bytes; }
     note_avg_frame(c, h->nbytes, out->n_msgs);
     return B2_OK;
 }
@@ -1263,7 +1280,7 @@ extern "C" uint64_t b2_ring_launches(b2_ctx* c) { return c ? c->ring_launches : 
 // device-side phase times of a collected ticket, ns since the kernel saw the doorbell: [0] header read [1] runs + bytes pulled [2] cut / decode / pack done [3] results pushed
 extern "C" int b2_ring_phase_ns(b2_ctx* c, uint32_t ticket, uint64_t out[4]) {
     if (!c || !c->ring_slots || !out) return B2_E_INVAL;
-    const RingSlotHdr* h = reinterpret_cast<const RingSlotHdr*>(c->ring_slots + (size_t)(ticket % kRingSlots) * c->ring_stride);
+    const RingSlotHdr* h = reinterpret_cast<const RingSlotHdr*>(ring_slot(c, ticket));
     for (int k = 0; k < 4; k++) out[k] = h->stamps[k + 1] - h->stamps[0];
     return B2_OK;
 }
@@ -1989,10 +2006,9 @@ extern "C" int b2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbytes, 
 }
 
 // ---- h2/gRPC on the latency path: k_h2_ring on the same submit ring (include/b2rpc.h, b2_h2_ring_enable) ---------------------------
+// the kernel arguments at each (re)launch: the slot parts of b2_h2_ring_enable, and the methods and identity as they are now
 static H2RingDev h2_ring_dev(const b2_ctx* c) {
-    H2RingDev H;
-    H.off_args = c->h2r_off_args; H.off_rs = c->h2r_off_rs; H.off_msgs = c->h2r_off_msgs; H.off_spans = c->h2r_off_spans;
-    H.off_out = c->h2r_off_out; H.off_replies = c->h2r_off_replies;
+    H2RingDev H = c->h2r_dev;
     H.conns = c->d_h2; H.hps = c->d_hpack; H.methods = c->d_methods; H.n_methods = c->cfg.n_methods; H.pool = h2_pool(c);
     H.cfg = h2_serve_cfg(c);
     // the scratch of b2_h2_serve_batch (h2_parse_batch, h2_gz_launch, h2_serve_launch)
@@ -2005,32 +2021,33 @@ static H2RingDev h2_ring_dev(const b2_ctx* c) {
 }
 extern "C" int b2_h2_ring_enable(b2_ctx* c, uint32_t max_bytes, uint32_t msg_cap, uint32_t out_cap, uint32_t replies_cap) {
     if (!c) { set_err("null argument"); return B2_E_INVAL; }
-    if (c->h2_ring || c->ring_slots || c->st_ring) { set_err("b2_h2_ring_enable: once, before the context's first ring call, and not with b2_stream_ring_enable"); return B2_E_INVAL; }
+    if (c->ring_kind != RingKind::none) { set_err("b2_h2_ring_enable: once, before the context's first ring call, and not with another ring kind"); return B2_E_INVAL; }
     if (max_bytes == 0 || msg_cap == 0 || out_cap == 0 || replies_cap == 0) { set_err("capacities must be non-zero"); return B2_E_INVAL; }
     if (max_bytes > c->opt.max_batch_bytes || out_cap > 2ull * c->opt.max_resp_bytes || msg_cap > c->opt.max_msgs || replies_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     CU(cudaSetDevice(c->opt.device));
     static_assert(sizeof(RingSlotHdr) + sizeof(H2RingArgs) <= 256, "h2 ring slot header");
     // [RingSlotHdr | args | runs | staged input | statuses | msgs | spans | out | replies]
-    auto up = [](uint64_t v) { return (uint32_t)((v + 255u) & ~255ull); };
     const uint64_t runs = (uint64_t)c->opt.max_runs;
-    c->h2r_off_args = sizeof(RingSlotHdr);
-    c->ring_off_runs = 256;
-    c->ring_off_in = up(c->ring_off_runs + runs * sizeof(b2_run));
-    c->h2r_off_rs = up((uint64_t)c->ring_off_in + max_bytes + 16);
-    c->h2r_off_msgs = up(c->h2r_off_rs + runs * sizeof(b2_h2_run_status));
-    c->h2r_off_spans = up(c->h2r_off_msgs + (uint64_t)msg_cap * sizeof(b2_h2_msg));
-    c->h2r_off_out = up(c->h2r_off_spans + runs * sizeof(b2_h2_reply_span));
-    c->h2r_off_replies = up((uint64_t)c->h2r_off_out + out_cap + 16);
-    rc = ring_alloc(c, (uint64_t)c->h2r_off_replies + replies_cap + 16); if (rc != B2_OK) return rc;
+    SlotLayout L;
+    H2RingDev& H = c->h2r_dev;
+    H.off_args = sizeof(RingSlotHdr);
+    c->ring_dev.off_runs = L.add(runs * sizeof(b2_run));
+    c->ring_dev.off_in = L.add((uint64_t)max_bytes + 16);
+    H.off_rs = L.add(runs * sizeof(b2_h2_run_status));
+    H.off_msgs = L.add((uint64_t)msg_cap * sizeof(b2_h2_msg));
+    H.off_spans = L.add(runs * sizeof(b2_h2_reply_span));
+    H.off_out = L.add((uint64_t)out_cap + 16);
+    H.off_replies = L.add((uint64_t)replies_cap + 16);
+    rc = ring_alloc(c, L.end); if (rc != B2_OK) return rc;
     CU(cudaFuncSetAttribute(k_h2_ring, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kH2RingSmem));
     c->h2r_max_bytes = max_bytes; c->h2r_msg_cap = msg_cap; c->h2r_out_cap = out_cap; c->h2r_replies_cap = replies_cap;
-    c->h2_ring = true;
+    c->ring_kind = RingKind::h2_server;
     return B2_OK;
 }
 extern "C" int b2_h2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs, uint32_t* ticket) {
     if (!c || !bytes || !runs || !ticket || n_runs == 0) { set_err("null argument"); return B2_E_INVAL; }
-    if (!c->h2_ring) { set_err("b2_h2_ring_enable first"); return B2_E_INVAL; }
+    if (c->ring_kind != RingKind::h2_server) { set_err("b2_h2_ring_enable first"); return B2_E_INVAL; }
     // the argument checks of b2_h2_serve_batch (h2_parse_batch) with the caps of b2_h2_ring_enable, and the slot's staging size
     if (nbytes > c->h2r_max_bytes) { set_err("batch larger than b2_h2_ring_enable's max_bytes: use b2_h2_serve_batch"); return B2_E_CAPACITY; }
     if (n_runs > c->opt.max_runs) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
@@ -2038,33 +2055,28 @@ extern "C" int b2_h2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, 
     const H2Split sp = h2_split(c->h2r_out_cap, c->h2r_msg_cap, c->h2r_replies_cap, n_runs);
     if (!sp.fits) { set_err("out_cap / msg_cap too small for the number of runs"); return B2_E_CAPACITY; }
     const H2RingArgs a = { sp.per_run, sp.region, sp.reply_region, h2_gz_wanted(c, runs, n_runs) ? 1u : 0u };
-    const uint32_t t = c->ring_next, si = t % kRingSlots;
-    if (!c->ring_collected[si]) { set_err("submit ring full: b2_h2_ring_wait the oldest ticket first"); return B2_E_CAPACITY; }
-    overwrites(c, kDevInput | kDevBatch);
-    uint8_t* slot = c->ring_slots + (size_t)si * c->ring_stride;
-    RingSlotHdr* h = reinterpret_cast<RingSlotHdr*>(slot);
-    h->bytes_dev = ring_stage(c, slot, bytes, nbytes);
-    memcpy(slot + c->ring_off_runs, runs, sizeof(b2_run) * (size_t)n_runs);
-    memcpy(slot + c->h2r_off_args, &a, sizeof a);
-    h->n_runs = n_runs; h->nbytes = nbytes;
-    return ring_ring(c, h, t, bytes, ticket);
+    uint8_t* slot = ring_claim(c, "b2_h2_ring_wait");
+    if (!slot) return B2_E_CAPACITY;
+    RingSlotHdr* h = ring_fill(c, slot, bytes, nbytes, runs, n_runs);
+    memcpy(slot + c->h2r_dev.off_args, &a, sizeof a);
+    return ring_ring(c, h, bytes, ticket);
 }
 extern "C" int b2_h2_ring_wait(b2_ctx* c, uint32_t ticket, b2_h2_ring_result* out) {
     static_assert(sizeof(b2_h2_ring_result) == 64, "h2 ring result ABI layout");
-    const uint8_t* slot = ring_ticket_slot(c, c && out && c->h2_ring, ticket, "bad h2 ring ticket");
-    if (!slot) return B2_E_INVAL;
+    int rc;
+    const uint8_t* slot = ring_collect(c, c && out && c->ring_kind == RingKind::h2_server, ticket, "bad h2 ring ticket", rc);
+    if (!slot) return rc;
     const RingSlotHdr* h = reinterpret_cast<const RingSlotHdr*>(slot);
-    { int rc = ring_spin(c, h, ticket); if (rc != B2_OK) return rc; }
-    c->ring_collected[ticket % kRingSlots] = true;
+    const H2RingDev& L = c->h2r_dev;
     const uint32_t n_runs = h->n_runs;
-    const b2_h2_run_status* rs = reinterpret_cast<const b2_h2_run_status*>(slot + c->h2r_off_rs);
+    const b2_h2_run_status* rs = reinterpret_cast<const b2_h2_run_status*>(slot + L.off_rs);
     uint32_t n_msgs = 0;
     for (uint32_t r = 0; r < n_runs; r++) n_msgs += rs[r].n_msgs;
     memset(out, 0, sizeof *out);
     out->runs = rs; out->n_runs = n_runs; out->n_msgs = n_msgs;
-    out->msgs = reinterpret_cast<const b2_h2_msg*>(slot + c->h2r_off_msgs);
-    out->out = slot + c->h2r_off_out; out->region = h2_split(c->h2r_out_cap, c->h2r_msg_cap, c->h2r_replies_cap, n_runs).region;
-    out->replies = slot + c->h2r_off_replies; out->spans = reinterpret_cast<const b2_h2_reply_span*>(slot + c->h2r_off_spans);
+    out->msgs = reinterpret_cast<const b2_h2_msg*>(slot + L.off_msgs);
+    out->out = slot + L.off_out; out->region = h2_split(c->h2r_out_cap, c->h2r_msg_cap, c->h2r_replies_cap, n_runs).region;
+    out->replies = slot + L.off_replies; out->spans = reinterpret_cast<const b2_h2_reply_span*>(slot + L.off_spans);
     if (n_msgs > c->h2r_msg_cap) { out->n_msgs = 0; out->status = B2_E_CAPACITY; }
     // the most recent ticket's input and out regions stay on the device: b2_h2_pack_responses may take bodies and content-types from them
     if (ticket + 1 == c->ring_next) { c->h2_last_in = h->nbytes; c->h2_last_out = (uint64_t)out->region * n_runs; }
@@ -2073,9 +2085,7 @@ extern "C" int b2_h2_ring_wait(b2_ctx* c, uint32_t ticket, b2_h2_ring_result* ou
 
 // ---- h2/gRPC client connections on the latency path: k_h2_client_ring on the same submit ring (include/b2rpc.h, b2_h2_client_ring_enable)
 static H2ClientRingDev h2_client_ring_dev(const b2_ctx* c) {
-    H2ClientRingDev H;
-    H.off_args = c->h2c_off_args; H.off_reqs = c->h2c_off_reqs; H.off_rs = c->h2c_off_rs; H.off_calls = c->h2c_off_calls; H.off_out = c->h2c_off_out;
-    H.off_req_res = c->h2c_off_req_res; H.off_req_out = c->h2c_off_req_out;
+    H2ClientRingDev H = c->h2c_dev;
     H.conns = c->d_h2; H.hps = c->d_hpack; H.pool = h2_pool(c);
     // the scratch of b2_h2_client_process_batch (h2_parse_batch, h2_gz_launch); the request block in the head rows, which the client parse
     // leaves alone (b2_h2_pack_requests' own d_msgs / d_aux / d_frame_off would overlap the calls and gz words), the frames in d_resp
@@ -2087,7 +2097,7 @@ static H2ClientRingDev h2_client_ring_dev(const b2_ctx* c) {
 }
 extern "C" int b2_h2_client_ring_enable(b2_ctx* c, uint32_t max_bytes, uint32_t call_cap, uint32_t out_cap, uint32_t max_reqs, uint32_t req_out_cap) {
     if (!c) { set_err("null argument"); return B2_E_INVAL; }
-    if (c->h2_ring || c->h2c_ring || c->ring_slots || c->st_ring) { set_err("b2_h2_client_ring_enable: once, before the context's first ring call, and not with another ring kind"); return B2_E_INVAL; }
+    if (c->ring_kind != RingKind::none) { set_err("b2_h2_client_ring_enable: once, before the context's first ring call, and not with another ring kind"); return B2_E_INVAL; }
     if (max_bytes == 0 || call_cap == 0 || out_cap == 0 || max_reqs == 0 || req_out_cap == 0) { set_err("capacities must be non-zero"); return B2_E_INVAL; }
     // the limits of b2_h2_client_process_batch and b2_h2_pack_requests, both of which read the ticket's bytes
     if (max_bytes > c->opt.max_batch_bytes || max_bytes > c->opt.max_resp_bytes || call_cap > c->opt.max_msgs || out_cap > 2ull * c->opt.max_resp_bytes ||
@@ -2096,28 +2106,29 @@ extern "C" int b2_h2_client_ring_enable(b2_ctx* c, uint32_t max_bytes, uint32_t 
     CU(cudaSetDevice(c->opt.device));
     static_assert(sizeof(RingSlotHdr) + sizeof(H2ClientRingArgs) <= 256, "h2 client ring slot header");
     // [RingSlotHdr | args | runs | staged input | requests + placed results + group_first | statuses | calls | out | request results | frames]
-    auto up = [](uint64_t v) { return (uint32_t)((v + 255u) & ~255ull); };
     const uint64_t runs = (uint64_t)c->opt.max_runs;
-    c->h2c_off_args = sizeof(RingSlotHdr);
-    c->ring_off_runs = 256;
-    c->ring_off_in = up(c->ring_off_runs + runs * sizeof(b2_run));
-    c->h2c_off_reqs = up((uint64_t)c->ring_off_in + max_bytes + 16);
-    c->h2c_off_rs = up((uint64_t)c->h2c_off_reqs + h2c_ring_block(max_reqs, max_reqs));
-    c->h2c_off_calls = up(c->h2c_off_rs + runs * sizeof(b2_h2_run_status));
-    c->h2c_off_out = up(c->h2c_off_calls + (uint64_t)call_cap * sizeof(b2_h2_call));
-    c->h2c_off_req_res = up((uint64_t)c->h2c_off_out + out_cap + 16);
-    c->h2c_off_req_out = up(c->h2c_off_req_res + (uint64_t)max_reqs * sizeof(b2_h2_request_result));
-    rc = ring_alloc(c, (uint64_t)c->h2c_off_req_out + req_out_cap + 16); if (rc != B2_OK) return rc;
+    SlotLayout L;
+    H2ClientRingDev& H = c->h2c_dev;
+    H.off_args = sizeof(RingSlotHdr);
+    c->ring_dev.off_runs = L.add(runs * sizeof(b2_run));
+    c->ring_dev.off_in = L.add((uint64_t)max_bytes + 16);
+    H.off_reqs = L.add(h2c_ring_block(max_reqs, max_reqs));
+    H.off_rs = L.add(runs * sizeof(b2_h2_run_status));
+    H.off_calls = L.add((uint64_t)call_cap * sizeof(b2_h2_call));
+    H.off_out = L.add((uint64_t)out_cap + 16);
+    H.off_req_res = L.add((uint64_t)max_reqs * sizeof(b2_h2_request_result));
+    H.off_req_out = L.add((uint64_t)req_out_cap + 16);
+    rc = ring_alloc(c, L.end); if (rc != B2_OK) return rc;
     CU(cudaFuncSetAttribute(k_h2_client_ring, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kH2ClientRingSmem));
     c->h2c_max_bytes = max_bytes; c->h2c_call_cap = call_cap; c->h2c_out_cap = out_cap; c->h2c_max_reqs = max_reqs; c->h2c_req_out_cap = req_out_cap;
-    c->h2c_ring = true;
+    c->ring_kind = RingKind::h2_client;
     return B2_OK;
 }
 extern "C" int b2_h2_client_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
                                         const b2_h2_request* reqs, uint32_t n_reqs, uint32_t* ticket) {
     if (!c || !bytes || !ticket || (!runs && n_runs) || (!reqs && n_reqs)) { set_err("null argument"); return B2_E_INVAL; }
     if (n_runs == 0 && n_reqs == 0) { set_err("a ticket carries runs, requests or both"); return B2_E_INVAL; }
-    if (!c->h2c_ring) { set_err("b2_h2_client_ring_enable first"); return B2_E_INVAL; }
+    if (c->ring_kind != RingKind::h2_client) { set_err("b2_h2_client_ring_enable first"); return B2_E_INVAL; }
     // the argument checks of b2_h2_client_process_batch and b2_h2_pack_requests with the caps of b2_h2_client_ring_enable
     if (nbytes > c->h2c_max_bytes) { set_err("ticket larger than b2_h2_client_ring_enable's max_bytes: use the batch calls"); return B2_E_CAPACITY; }
     if (n_runs > c->opt.max_runs || n_reqs > c->h2c_max_reqs) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
@@ -2127,46 +2138,41 @@ extern "C" int b2_h2_client_ring_submit(b2_ctx* c, const void* bytes, uint32_t n
         sp = h2_split(c->h2c_out_cap, c->h2c_call_cap, 0, n_runs);
         if (!sp.fits) { set_err("out_cap / call_cap too small for the number of runs"); return B2_E_CAPACITY; }
     }
-    const uint32_t t = c->ring_next, si = t % kRingSlots;
-    if (!c->ring_collected[si]) { set_err("submit ring full: b2_h2_client_ring_wait the oldest ticket first"); return B2_E_CAPACITY; }
+    uint8_t* slot = ring_claim(c, "b2_h2_client_ring_wait");
+    if (!slot) return B2_E_CAPACITY;
     std::vector<uint32_t> first;
     std::vector<b2_h2_request_result> placed(n_reqs);
     uint64_t total = 0;
     if (n_reqs) { int rc = h2_place_requests(c, bytes, nbytes, reqs, n_reqs, c->h2c_req_out_cap, placed.data(), first, total); if (rc != B2_OK) return rc; }
     const H2ClientRingArgs a = { sp.per_run, sp.region, n_runs && h2_gz_wanted(c, runs, n_runs) ? 1u : 0u, n_reqs, n_reqs ? (uint32_t)first.size() - 1 : 0u, { 0, 0, 0 } };
-    overwrites(c, kDevInput | kDevBatch);
-    uint8_t* slot = c->ring_slots + (size_t)si * c->ring_stride;
-    uint8_t* block = slot + c->h2c_off_reqs;                     // the request block the kernel pulls: requests, placed results, group_first
+    RingSlotHdr* h = ring_fill(c, slot, bytes, nbytes, runs, n_runs);
+    uint8_t* block = slot + c->h2c_dev.off_reqs;                 // the request block the kernel pulls: requests, placed results, group_first
     if (n_reqs) {
         memcpy(block, reqs, sizeof(b2_h2_request) * (size_t)n_reqs);
         memcpy(block + h2c_ring_res_off(n_reqs), placed.data(), sizeof(b2_h2_request_result) * (size_t)n_reqs);
         memcpy(block + h2c_ring_first_off(n_reqs), first.data(), 4 * first.size());
     }
-    RingSlotHdr* h = reinterpret_cast<RingSlotHdr*>(slot);
-    h->bytes_dev = ring_stage(c, slot, bytes, nbytes);
-    if (n_runs) memcpy(slot + c->ring_off_runs, runs, sizeof(b2_run) * (size_t)n_runs);
-    memcpy(slot + c->h2c_off_args, &a, sizeof a);
-    h->n_runs = n_runs; h->nbytes = nbytes;
-    return ring_ring(c, h, t, bytes, ticket);
+    memcpy(slot + c->h2c_dev.off_args, &a, sizeof a);
+    return ring_ring(c, h, bytes, ticket);
 }
 extern "C" int b2_h2_client_ring_wait(b2_ctx* c, uint32_t ticket, b2_h2_client_ring_result* out) {
     static_assert(sizeof(b2_h2_client_ring_result) == 64, "h2 client ring result ABI layout");
-    const uint8_t* slot = ring_ticket_slot(c, c && out && c->h2c_ring, ticket, "bad h2 client ring ticket");
-    if (!slot) return B2_E_INVAL;
+    int rc;
+    const uint8_t* slot = ring_collect(c, c && out && c->ring_kind == RingKind::h2_client, ticket, "bad h2 client ring ticket", rc);
+    if (!slot) return rc;
     const RingSlotHdr* h = reinterpret_cast<const RingSlotHdr*>(slot);
-    { int rc = ring_spin(c, h, ticket); if (rc != B2_OK) return rc; }
-    c->ring_collected[ticket % kRingSlots] = true;
-    const H2ClientRingArgs* a = reinterpret_cast<const H2ClientRingArgs*>(slot + c->h2c_off_args);
+    const H2ClientRingDev& L = c->h2c_dev;
+    const H2ClientRingArgs* a = reinterpret_cast<const H2ClientRingArgs*>(slot + L.off_args);
     const uint32_t n_runs = h->n_runs;
-    const b2_h2_run_status* rs = reinterpret_cast<const b2_h2_run_status*>(slot + c->h2c_off_rs);
+    const b2_h2_run_status* rs = reinterpret_cast<const b2_h2_run_status*>(slot + L.off_rs);
     uint32_t n_calls = 0;
     for (uint32_t r = 0; r < n_runs; r++) n_calls += rs[r].n_msgs;
     memset(out, 0, sizeof *out);
     out->runs = rs; out->n_runs = n_runs; out->n_calls = n_calls;
-    out->calls = reinterpret_cast<const b2_h2_call*>(slot + c->h2c_off_calls);
-    out->out = slot + c->h2c_off_out; out->region = a->region;
+    out->calls = reinterpret_cast<const b2_h2_call*>(slot + L.off_calls);
+    out->out = slot + L.off_out; out->region = a->region;
     out->n_reqs = a->n_reqs;
-    out->reqs = reinterpret_cast<const b2_h2_request_result*>(slot + c->h2c_off_req_res);
-    out->req_out = slot + c->h2c_off_req_out;
+    out->reqs = reinterpret_cast<const b2_h2_request_result*>(slot + L.off_req_res);
+    out->req_out = slot + L.off_req_out;
     return B2_OK;
 }

@@ -1745,7 +1745,7 @@ __device__ __forceinline__ void h2_ring_push_run(uint32_t r, uint32_t lane, uint
     if (lane == 0) { st.first_msg = f; reinterpret_cast<b2_h2_run_status*>(slot + off_rs)[r] = st; }
 }
 // k_h2_ring: b2_h2_serve_batch on the latency path (b2_h2_ring_*).  One resident CTA, fed through the same submit ring as k_ring
-// (ring_doorbell / ring_pull / ring_push / ring_stamp / ring_release of b2_kernels.cuh): per ticket the passes of the batch call, as block phases with
+// (the ticket loop ring_serve and ring_push of b2_kernels.cuh): per ticket the passes of the batch call, as block phases with
 // __syncthreads() where the batch call has kernel boundaries, on the same device scratch, then only the used parts are pushed into the
 // ticket's slot.  H2Conn, HpackState and the stream pool are read through L1: every call that writes them from another kernel retires
 // this one first (ring_halt), so a launch boundary lies between their writes and this CTA's loads.
@@ -1763,26 +1763,10 @@ struct H2RingDev {
 constexpr uint32_t kH2RingSmem = kSmallWarps * 3 * kH2FragCap;          // k_h2_pack's scratch for each warp
 __global__ void __launch_bounds__(kSmallThreads, 1) k_h2_ring(RingDev R, H2RingDev H) {
     extern __shared__ __align__(16) uint8_t h2_ring_raw[];
-    __shared__ uint32_t s_go;
-    __shared__ RingSlotHdr s_hdr;
-    __shared__ H2RingArgs s_args;
     const uint32_t tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const uint8_t* bytes = R.d_bytes;
     const b2_run* runs = reinterpret_cast<const b2_run*>(R.d_meta);
-    uint32_t ticket = R.next_ticket[0];
-    for (;;) {
-        uint8_t* slot = R.slots + (size_t)(ticket % kRingSlots) * R.slot_stride;
-        RingSlotHdr* hdr = reinterpret_cast<RingSlotHdr*>(slot);
-        if (tid == 0) s_go = ring_doorbell(R, hdr, ticket);
-        __syncthreads();
-        if (!s_go) break;
-        unsigned long long t[4] = { 0, 0, 0, 0 };                    // doorbell seen, header read, bytes pulled, replies packed
-        if (tid == 0) t[0] = globaltimer_ns();
-        ring_pull(R, slot, s_hdr, R.d_meta, t[1]);
-        if (tid < 4) reinterpret_cast<uint32_t*>(&s_args)[tid] = ld_sys_u32(reinterpret_cast<const volatile uint32_t*>(slot + H.off_args) + tid);
-        __threadfence();
-        __syncthreads();
-        if (tid == 0) t[2] = globaltimer_ns();
+    ring_serve<H2RingArgs>(R, H.off_args, [] {}, [&](uint8_t* slot, const RingSlotHdr& s_hdr, const H2RingArgs& s_args, unsigned long long (&t)[4]) __attribute__((always_inline)) {
         const uint32_t n_runs = s_hdr.n_runs, per_run = s_args.per_run, region = s_args.region, reply_region = s_args.reply_region, n_slots = n_runs * per_run;
         for (uint32_t r = tid; r < n_runs; r += kSmallThreads)
             h2_consume_run<false>(r, bytes, runs, H.conns, H.hps, H.methods, H.n_methods, H.rs, H.msgs, per_run, H.out, region, H.pool);
@@ -1800,7 +1784,7 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_h2_ring(RingDev R, H2RingD
         __syncthreads();
         for (uint32_t r = wid; r < n_runs; r += kSmallWarps) h2_gather_run(r, lane, H.first, H.list_offs, H.gz, H.replies, H.spans);
         __syncthreads();
-        if (tid == 0) t[3] = globaltimer_ns();
+        if (tid == 0) t[3] = globaltimer_ns();                          // replies packed
         // the descriptors become one list in run order (the batch call compacts them on the host): first[r] = run r's first list index
         if (wid == 0) h2_warp_scan_runs(n_runs, lane, [&](uint32_t r) { return H.rs[r].n_msgs; }, H.first);
         __syncthreads();
@@ -1811,13 +1795,8 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_h2_ring(RingDev R, H2RingD
             ring_push(slot + H.off_replies + sp.off, H.replies + sp.off, sp.len, lane, 32);
             if (lane == 0) reinterpret_cast<b2_h2_reply_span*>(slot + H.off_spans)[r] = sp;
         }
-        if (tid == 0) ring_stamp(hdr, t);
-        __threadfence_system();
-        __syncthreads();
-        if (tid == 0) ring_release(R, hdr, ticket);
-        ticket++;
-    }
-    if (tid == 0) R.next_ticket[0] = ticket;
+        return false;
+    });
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1843,26 +1822,10 @@ B2_HD uint32_t h2c_ring_block(uint32_t n, uint32_t n_groups) { return h2c_ring_f
 constexpr uint32_t kH2ClientRingSmem = kSmallWarps * 2 * kH2ReqFragCap;  // k_h2_pack_req's scratch for each warp
 __global__ void __launch_bounds__(kSmallThreads, 1) k_h2_client_ring(RingDev R, H2ClientRingDev H) {
     extern __shared__ __align__(16) uint8_t h2c_ring_raw[];
-    __shared__ uint32_t s_go;
-    __shared__ RingSlotHdr s_hdr;
-    __shared__ H2ClientRingArgs s_args;
     const uint32_t tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const uint8_t* bytes = R.d_bytes;
     const b2_run* runs = reinterpret_cast<const b2_run*>(R.d_meta);
-    uint32_t ticket = R.next_ticket[0];
-    for (;;) {
-        uint8_t* slot = R.slots + (size_t)(ticket % kRingSlots) * R.slot_stride;
-        RingSlotHdr* hdr = reinterpret_cast<RingSlotHdr*>(slot);
-        if (tid == 0) s_go = ring_doorbell(R, hdr, ticket);
-        __syncthreads();
-        if (!s_go) break;
-        unsigned long long t[4] = { 0, 0, 0, 0 };                    // doorbell seen, header read, bytes pulled, requests packed
-        if (tid == 0) t[0] = globaltimer_ns();
-        ring_pull(R, slot, s_hdr, R.d_meta, t[1]);
-        if (tid < sizeof(H2ClientRingArgs) / 4) reinterpret_cast<uint32_t*>(&s_args)[tid] = ld_sys_u32(reinterpret_cast<const volatile uint32_t*>(slot + H.off_args) + tid);
-        __threadfence();
-        __syncthreads();
-        if (tid == 0) t[2] = globaltimer_ns();
+    ring_serve<H2ClientRingArgs>(R, H.off_args, [] {}, [&](uint8_t* slot, const RingSlotHdr& s_hdr, const H2ClientRingArgs& s_args, unsigned long long (&t)[4]) __attribute__((always_inline)) {
         const uint32_t n_runs = s_hdr.n_runs, per_run = s_args.per_run, region = s_args.region, n_reqs = s_args.n_reqs, n_groups = s_args.n_groups;
         const b2_h2_request* reqs = reinterpret_cast<const b2_h2_request*>(H.reqs);
         b2_h2_request_result* res = reinterpret_cast<b2_h2_request_result*>(H.reqs + h2c_ring_res_off(n_reqs));
@@ -1879,7 +1842,7 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_h2_client_ring(RingDev R, 
         for (uint32_t g = wid; g < n_groups; g += kSmallWarps)
             h2_pack_req_group(g, lane, h2c_ring_raw + wid * 2 * kH2ReqFragCap, bytes, reqs, group_first, H.conns, H.req_out, res, H.pool);
         __syncthreads();
-        if (tid == 0) t[3] = globaltimer_ns();
+        if (tid == 0) t[3] = globaltimer_ns();                          // requests packed
         if (wid == 0) h2_warp_scan_runs(n_runs, lane, [&](uint32_t r) { return H.rs[r].n_msgs; }, H.first);
         __syncthreads();
         // push: a warp per run (h2_ring_push_run), the request results, then a warp per request its frames
@@ -1890,13 +1853,8 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_h2_client_ring(RingDev R, 
             const b2_h2_request_result q = res[i];
             ring_push(slot + H.off_req_out + q.out_off, H.req_out + q.out_off, q.out_len, lane, 32);
         }
-        if (tid == 0) ring_stamp(hdr, t);
-        __threadfence_system();
-        __syncthreads();
-        if (tid == 0) ring_release(R, hdr, ticket);
-        ticket++;
-    }
-    if (tid == 0) R.next_ticket[0] = ticket;
+        return false;
+    });
 }
 #endif
 #endif

@@ -2756,7 +2756,7 @@ struct RingSlotHdr {                 // in mapped host memory, one per slot; the
 };                                   // 128 bytes
 struct RingDev {
     uint8_t* slots;                  // mapped host memory: kRingSlots x slot_stride
-    uint32_t slot_stride, off_runs, off_in, off_out;     // layout of one slot: [RingSlotHdr | runs | staged input | output block]
+    uint32_t slot_stride, off_runs, off_in, off_out;     // layout of one slot: [RingSlotHdr | runs | staged input | output block (k_ring)]
     volatile uint32_t* ctl;          // mapped host memory: [0] stop  [1] running  [2] batches served  [3] parked ticket served (host)
     uint32_t* next_ticket;           // device memory: [0] ticket the kernel waits for next [1] ticket it parks behind (survive relaunches)
     uint32_t off_st;                 // with a stream table: the slot's stream section, behind the output block
@@ -2770,10 +2770,10 @@ __device__ __forceinline__ void st_sys_u32(volatile uint32_t* p, uint32_t v) {
     asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 __device__ __forceinline__ unsigned long long globaltimer_ns() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
-// The parts k_ring and k_h2_ring share.  Thread 0 waits for `ticket` in its slot: 1 when it came, 0 on `stop` or after idle_ns without
-// work.  A context whose ticket overflowed k_ring's compact block parks behind it (next_ticket[1]) until the host has served it through
-// the big pipeline and released it (ctl[3]): the stream table sees the tickets in ticket order, and the pull does not overwrite the device
-// input that pipeline reads.  k_h2_ring never parks (next_ticket[1] stays 0).
+// The parts of the ticket loop (ring_serve below) every resident kernel runs.  Thread 0 waits for `ticket` in its slot: 1 when it came, 0
+// on `stop` or after idle_ns without work.  A context whose ticket overflowed k_ring's compact block parks behind it (next_ticket[1]) until
+// the host has served it through the big pipeline and released it (ctl[3]): the stream table sees the tickets in ticket order, and the
+// pull does not overwrite the device input that pipeline reads.  k_h2_ring and k_h2_client_ring never park (next_ticket[1] stays 0).
 __device__ __forceinline__ uint32_t ring_doorbell(const RingDev& R, RingSlotHdr* hdr, uint32_t ticket) {
     const unsigned long long t0 = globaltimer_ns();
     const uint32_t park = R.next_ticket[1];
@@ -2827,7 +2827,47 @@ __device__ __forceinline__ void ring_stamp(RingSlotHdr* hdr, const unsigned long
 __device__ __forceinline__ void ring_release(const RingDev& R, RingSlotHdr* hdr, uint32_t ticket) {
     st_sys_u32(&hdr->done, ticket); st_sys_u32(R.ctl + 2, ticket + 1);
 }
-#define B2_KERNELS_RING 1                                             // b2_h2.cuh builds k_h2_ring on the parts above
+// The ticket loop of every resident kernel (k_ring, k_h2_ring, k_h2_client_ring), by the whole CTA.  Per ticket: the doorbell, the pull
+// of the header, runs and bytes and of the kind's per-ticket Args (at the slot's off_args; RingNoArgs: none), then prep(), the kernel's own
+// stores that the fence after the pull publishes with the pulled bytes, then body(slot, hdr, args, t): the ticket's work, which stamps
+// t[3] and pushes the results into the slot; it returns true when the kernel must park behind this ticket.  Then the stamps, the
+// system-wide fence and the release.  The next ticket is handed to the next launch when the kernel leaves.  off_args is a reference to
+// the kernel parameter, read where it is used, so that no register holds it across the body.
+struct RingNoArgs {};
+template <class Args, class Prep, class Body>
+__device__ __forceinline__ void ring_serve(const RingDev& R, const uint32_t& off_args, Prep prep, Body body) {
+    __shared__ uint32_t s_go;
+    __shared__ RingSlotHdr s_hdr;
+    __shared__ Args s_args;
+    const uint32_t tid = threadIdx.x;
+    uint32_t ticket = R.next_ticket[0];
+    for (;;) {
+        uint8_t* slot = R.slots + (size_t)(ticket % kRingSlots) * R.slot_stride;
+        RingSlotHdr* hdr = reinterpret_cast<RingSlotHdr*>(slot);
+        if (tid == 0) s_go = ring_doorbell(R, hdr, ticket);
+        __syncthreads();
+        if (!s_go) break;
+        unsigned long long t[4] = { 0, 0, 0, 0 };                    // doorbell seen, header read, bytes pulled, body done
+        if (tid == 0) t[0] = globaltimer_ns();
+        ring_pull(R, slot, s_hdr, R.d_meta, t[1]);
+        if constexpr (sizeof(Args) >= 4) { if (tid < sizeof(Args) / 4) reinterpret_cast<uint32_t*>(&s_args)[tid] = ld_sys_u32(reinterpret_cast<const volatile uint32_t*>(slot + off_args) + tid); }
+        prep();
+        __threadfence();
+        __syncthreads();
+        if (tid == 0) t[2] = globaltimer_ns();
+        const bool park = body(slot, s_hdr, s_args, t);
+        if (tid == 0) ring_stamp(hdr, t);
+        __threadfence_system();
+        __syncthreads();
+        if (tid == 0) {
+            if (park) R.next_ticket[1] = ticket;
+            ring_release(R, hdr, ticket);
+        }
+        ticket++;
+    }
+    if (tid == 0) R.next_ticket[0] = ticket;
+}
+#define B2_KERNELS_RING 1                                             // b2_h2.cuh builds k_h2_ring and k_h2_client_ring on ring_serve
 
 // ---------------------------------------------------------------------------------------------------------------------------------
 // streaming_rpc: the receiving side of a Stream on the device (b2_stream_*).  What brpc does with a STRM frame after the meta parse:
@@ -3158,35 +3198,23 @@ __device__ __forceinline__ void stream_pass_block(const BatchPtrs& B, const Stre
 __global__ void __launch_bounds__(kSmallThreads, 1) k_ring(RingDev R, BatchPtrs B0, DevConfig C, StreamPass SP) {
     extern __shared__ __align__(128) uint8_t small_raw[];
     SmallSmem& S = *reinterpret_cast<SmallSmem*>(small_raw);
-    __shared__ uint32_t s_go;
-    __shared__ RingSlotHdr s_hdr;
     const uint32_t tid = threadIdx.x;
     crc_tabs_to_smem(S.s_hot, B0.crc_adv);
-    uint32_t ticket = R.next_ticket[0];
     const bool streams = SP.tab != nullptr;
-    for (;;) {
-        uint8_t* slot = R.slots + (size_t)(ticket % kRingSlots) * R.slot_stride;
-        RingSlotHdr* hdr = reinterpret_cast<RingSlotHdr*>(slot);
-        if (tid == 0) s_go = ring_doorbell(R, hdr, ticket);
-        __syncthreads();
-        if (!s_go) break;
-        unsigned long long t[4] = { 0, 0, 0, 0 };                    // doorbell seen, header read, bytes pulled, body done
-        if (tid == 0) t[0] = globaltimer_ns();
-        ring_pull(R, slot, s_hdr, R.d_meta, t[1]);
+    DevConfig Cb = C; Cb.pull = 0;         // (copied once per launch: by_ref comes with each ticket)
+    // the totals of the compact block and the stream pass's counters start each ticket at zero
+    auto prep = [&] { if (tid < 16) { reinterpret_cast<uint32_t*>(R.d_small)[tid] = 0; if (streams) SP.cnts[tid] = 0; } };
+    ring_serve<RingNoArgs>(R, 0, prep, [&](uint8_t* slot, const RingSlotHdr& s_hdr, const RingNoArgs&, unsigned long long (&t)[4]) __attribute__((always_inline)) {
         const uint32_t n_runs = s_hdr.n_runs;
         BatchPtrs B = B0;
-        B.bytes = R.d_bytes; B.runs = reinterpret_cast<const b2_run*>(R.d_meta); B.n_runs = n_runs;
-        B.totals = reinterpret_cast<uint32_t*>(R.d_small);
+        B.bytes = R.d_bytes; B.runs = reinterpret_cast<const b2_run*>(R.d_meta); B.totals = reinterpret_cast<uint32_t*>(R.d_small);
+        B.n_runs = n_runs;
         B.run_status = reinterpret_cast<b2_run_status*>(R.d_small + s_hdr.off_rs);
         B.msgs = reinterpret_cast<b2_msg_desc*>(R.d_small + s_hdr.off_msgs);
         B.refs = reinterpret_cast<uint4*>(R.d_small + s_hdr.off_refs);
         B.resp = R.d_small + s_hdr.off_resp;
         B.max_msgs = s_hdr.small_msgs; B.max_resp = s_hdr.small_resp;
-        DevConfig Cb = C; Cb.by_ref = s_hdr.by_ref; Cb.pull = 0;
-        if (tid < 16) { B.totals[tid] = 0; if (streams) SP.cnts[tid] = 0; }
-        __threadfence();
-        __syncthreads();
-        if (tid == 0) t[2] = globaltimer_ns();
+        Cb.by_ref = s_hdr.by_ref;
         small_body(B, Cb, S);
         __threadfence();
         __syncthreads();
@@ -3207,16 +3235,8 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_ring(RingDev R, BatchPtrs 
             uint8_t* sec = slot + R.off_st;
             for (int q = 0; q < 6; q++) ring_push(sec + (from[q] - from[0]), from[q], len[q], tid, kSmallThreads);
         }
-        if (tid == 0) ring_stamp(hdr, t);
-        __threadfence_system();
-        __syncthreads();
-        if (tid == 0) {
-            if (streams && overflow) R.next_ticket[1] = ticket;
-            ring_release(R, hdr, ticket);
-        }
-        ticket++;
-    }
-    if (tid == 0) R.next_ticket[0] = ticket;
+        return streams && overflow;   // the host serves an overflowing ticket through the big pipeline: park behind it (ring_doorbell)
+    });
 }
 
 // b2_stream_close / b2_stream_set_connected: one stream between batch calls.  frame[0..] = the frame to write, *frame_len its length (0 = none).

@@ -771,7 +771,8 @@ int  b2_h2_serve_batch(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2
                        b2_h2_run_status* rs, b2_h2_msg* msgs, uint32_t msg_cap, uint32_t* n_msgs, void* out, uint32_t out_cap,
                        void* replies, uint32_t replies_cap, b2_h2_reply_span* spans);
 /* h2/gRPC on the latency path: b2_h2_serve_batch inside a resident kernel (k_h2_ring) fed through the submit ring of b2_ring_* — no
- * launch, copy or stream synchronisation per batch.  A context runs either k_ring or k_h2_ring, never both.
+ * launch, copy or stream synchronisation per batch.  A context runs either k_ring or k_h2_ring, never both: its first ring call (an enable
+ * call, b2_ring_start or b2_ring_submit) fixes which resident kernel it runs.
  * b2_h2_ring_enable: once, after b2_h2_configure and before the context's first ring call (after b2_ring_start / b2_ring_submit /
  * b2_stream_ring_enable, or twice: B2_E_INVAL; b2_ring_submit / b2_ring_wait then fail with B2_E_INVAL).  The four capacities are per
  * ticket and play the roles of b2_h2_serve_batch's nbytes bound, msg_cap, out_cap and replies_cap; they are checked against the context
