@@ -124,6 +124,10 @@ IOVEC_DT = np.dtype([("base", "<u8"), ("len", "<u8")])          # struct iovec
 INPUT_COPY, INPUT_PULL, RESP_COPY, RESP_BY_REF, RESP_IOVEC = 0, 1, 0, 1, 2
 
 
+class ResidentKernel(C.Structure):
+    _fields_ = [("name", C.c_char_p), ("regs", C.c_uint32), ("threads", C.c_uint32), ("smem_bytes", C.c_uint32), ("fits", C.c_uint32)]
+
+
 class B2Error(RuntimeError):
     def __init__(self, code, text):
         super().__init__("b2rpc error %d: %s" % (code, text))
@@ -164,6 +168,7 @@ def _load():
     l.b2_elapsed_ms.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_float)]
     l.b2_batch_download.argtypes = [C.c_void_p, C.POINTER(BatchResult)]
     l.b2_batch_info.argtypes = [C.c_void_p, C.c_void_p]
+    l.b2_resident_plan.argtypes = [C.c_void_p, C.POINTER(ResidentKernel), C.c_int]
     l.b2_device_pci_bus_id.argtypes = [C.c_int, C.c_char_p, C.c_int]
     l.b2_stage_times.argtypes = [C.c_void_p, C.POINTER(C.c_char_p), C.POINTER(C.c_float), C.c_int]
     l.b2_crc32c_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
@@ -224,7 +229,7 @@ lib = _load()
 ABI_SYMBOLS = ["b2_ctx_create", "b2_ctx_destroy", "b2_last_error", "b2_version", "b2_register_method",
                "b2_set_server_identity", "b2_set_stream_handler", "b2_set_protocols", "b2_block_alloc", "b2_block_free", "b2_block_pool_host_allocs", "b2_set_modes", "b2_ring_start", "b2_ring_stop", "b2_ring_submit", "b2_ring_wait", "b2_ring_launches", "b2_ring_phase_ns", "b2_latency_probe", "b2_process_batch", "b2_batch_submit", "b2_batch_collect", "b2_batch_upload",
                "b2_batch_execute", "b2_batch_execute_many", "b2_batch_download", "b2_batch_launch", "b2_batch_wait",
-               "b2_elapsed_ms", "b2_batch_info", "b2_device_pci_bus_id", "b2_stage_times", "b2_crc32c_batch", "b2_crc32c_extend", "b2_snappy_max_compressed_length", "b2_snappy_raw_compress", "b2_snappy_get_uncompressed_length", "b2_snappy_raw_uncompress", "b2_snappy_uncompress_batch", "b2_snappy_compress_batch", "b2_hpack_reset", "b2_hpack_decode_batch", "b2_pack_requests", "b2_pack_responses", "b2_h2_scan_batch", "b2_h2_conn_reset", "b2_h2_configure", "b2_h2_process_batch", "b2_h2_pack_responses", "b2_counters_read",
+               "b2_elapsed_ms", "b2_batch_info", "b2_resident_plan", "b2_device_pci_bus_id", "b2_stage_times", "b2_crc32c_batch", "b2_crc32c_extend", "b2_snappy_max_compressed_length", "b2_snappy_raw_compress", "b2_snappy_get_uncompressed_length", "b2_snappy_raw_uncompress", "b2_snappy_uncompress_batch", "b2_snappy_compress_batch", "b2_hpack_reset", "b2_hpack_decode_batch", "b2_pack_requests", "b2_pack_responses", "b2_h2_scan_batch", "b2_h2_conn_reset", "b2_h2_configure", "b2_h2_process_batch", "b2_h2_pack_responses", "b2_counters_read",
                "b2_counters_device_ptr", "b2_counters_allreduce", "b2_h2_pack_requests", "b2_h2_conn_set_next_stream_id", "b2_h2_conn_peer_update",
                "b2_h2_client_conn_reset", "b2_h2_client_process_batch", "b2_h2_client_abandon_streams", "b2_h2_conn_set_gunzip",
                "b2_h2_serve_batch", "b2_stream_configure", "b2_stream_open", "b2_stream_set_connected", "b2_stream_close", "b2_stream_query",
@@ -547,6 +552,14 @@ class Context:
         out = (C.c_uint32 * 4)()
         _check(lib.b2_batch_info(self._h, out))
         return {"tile_bytes": out[0], "n_tiles": out[1], "spec_k": out[2], "fused": bool(out[3])}
+
+    def resident_plan(self):
+        """k_fused in the uploaded batch's shape, then the kernels launched between two k_fused passes: registers, threads and shared
+        memory per block, and how many blocks of each start on an SM beside one k_fused CTA (b2_resident_plan)."""
+        out = (ResidentKernel * 8)()
+        n = _check(lib.b2_resident_plan(self._h, out, 8))
+        return [{"name": out[i].name.decode(), "regs": out[i].regs, "threads": out[i].threads, "smem_bytes": out[i].smem_bytes,
+                 "fits": out[i].fits} for i in range(min(n, 8))]
 
     def stage_times(self):
         names = (C.c_char_p * 16)()

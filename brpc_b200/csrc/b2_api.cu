@@ -55,6 +55,8 @@ struct SlotLayout {
 };
 }
 
+// The kernels of a fused pass in b2_resident_plan's order: k_fused, then the ones launched between two k_fused passes (DESIGN §3)
+enum : int { kPlanFused, kPlanSearch, kPlanWalk, kPlanResolve, kPlanSlow, kPlanKernels };
 struct b2_ctx {
     b2_options opt;
     DevConfig cfg;
@@ -112,6 +114,8 @@ struct b2_ctx {
     uint8_t* d_meta = nullptr; uint8_t* h_meta = nullptr;       // [runs | run_tile_base]
     uint8_t* d_small = nullptr; uint8_t* h_small = nullptr;     // [totals | run_status | msgs | resp]
     bool small = false, small_copy_queued = false, use_fused_small = true; SmallLayout sm = {};
+    // b2_resident_plan: the kernels of a fused pass as compiled (read at creation), and the SM they share
+    b2_resident_kernel plan[kPlanKernels] = {}; uint32_t sm_regs = 0, sm_smem = 0, sm_warps = 0, sm_blocks = 0, block_smem_reserve = 0;
 };
 
 // What a call overwrites on the device, and so which saved state it forgets; every call that writes the context's buffers says so first.
@@ -317,6 +321,25 @@ extern "C" int b2_ctx_create(const b2_options* o, b2_ctx** out) {
     if (const char* e = getenv("B2_FUSED")) c->use_fused = strcmp(e, "off") != 0;
     CU(cudaFuncSetAttribute(k_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(FusedWarpSmem) * (kFusedWarps > kFusedWarpsDense ? kFusedWarps : kFusedWarpsDense))));
     CU(cudaFuncSetAttribute(k_small, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmallSmem)));
+#if defined(__NVCC__)       // (the host build of this file on the CUDA emulator, tests/cpp, has no function attributes: its plan stays empty)
+    {
+        const void* fn[kPlanKernels] = { (const void*)k_fused, (const void*)k_tile_search, (const void*)k_tile_walk, (const void*)k_resolve, (const void*)k_pack_slow<true> };
+        const char* name[kPlanKernels] = { "k_fused", "k_tile_search", "k_tile_walk", "k_resolve", "k_pack_slow<true>" };
+        const uint32_t threads[kPlanKernels] = { 0, kSearchThreadsFused, 128, 256, kSlowLiteThreads };     // (k_fused: by the batch's shape)
+        for (int k = 0; k < kPlanKernels; k++) {
+            cudaFuncAttributes a;
+            CU(cudaFuncGetAttributes(&a, fn[k]));
+            c->plan[k].name = name[k]; c->plan[k].regs = (uint32_t)a.numRegs; c->plan[k].threads = threads[k]; c->plan[k].smem_bytes = (uint32_t)a.sharedSizeBytes;
+        }
+        int v[5] = {};
+        CU(cudaDeviceGetAttribute(&v[0], cudaDevAttrMaxRegistersPerMultiprocessor, o->device));
+        CU(cudaDeviceGetAttribute(&v[1], cudaDevAttrMaxSharedMemoryPerMultiprocessor, o->device));
+        CU(cudaDeviceGetAttribute(&v[2], cudaDevAttrMaxThreadsPerMultiProcessor, o->device));
+        CU(cudaDeviceGetAttribute(&v[3], cudaDevAttrMaxBlocksPerMultiprocessor, o->device));
+        CU(cudaDeviceGetAttribute(&v[4], cudaDevAttrReservedSharedMemoryPerBlock, o->device));
+        c->sm_regs = (uint32_t)v[0]; c->sm_smem = (uint32_t)v[1]; c->sm_warps = (uint32_t)v[2] / 32; c->sm_blocks = (uint32_t)v[3]; c->block_smem_reserve = (uint32_t)v[4];
+    }
+#endif
     *out = c;
     return B2_OK;
 }
@@ -427,6 +450,15 @@ extern "C" int b2_batch_upload(b2_ctx* c, const void* bytes, uint32_t nbytes, co
     c->stream_valid = false; c->st_view_ticket = 0;
     c->covered = covered;                           // (what the runs hold: with B2_INPUT_PULL nbytes spans the caller's whole arena)
     CU(cudaSetDevice(c->opt.device));
+    if (!c->avg_frame && n_runs && runs[0].length >= 12 && (uint64_t)runs[0].offset + 12 <= nbytes) {
+        // a context that has not finished a batch yet takes the frame size from the first baidu_std / streaming_rpc header of the batch, so
+        // that its tiles and k_fused's shape follow the traffic from the first batch on (a context whose passes are only launched and
+        // waited for never downloads a batch; its k_fused would keep the dense shape, which leaves no room for the other batch's kernels)
+        const uint8_t* f = static_cast<const uint8_t*>(bytes) + runs[0].offset;
+        uint32_t w[2]; memcpy(w, f, 8);
+        const uint32_t body = __builtin_bswap32(w[1]);
+        if ((w[0] == kMagicPRPC || w[0] == kMagicSTRM) && body <= c->cfg.max_body_size && body < (1u << 30)) c->avg_frame = 12 + body;
+    }
     if (c->adaptive_tile) {
         // like Socket::_avg_msg_size steering the read size (input_messenger.cpp:348-353): a tile should hold
         // 6-12 messages so the speculative entry search reads a small fraction of it
@@ -502,7 +534,17 @@ static int launch_stream_pass(b2_ctx* c, const BatchPtrs& B, cudaStream_t s, uin
     return B2_OK;
 }
 
-static int launch_pipeline(b2_ctx* c) {
+// k_fused's warps per CTA for the uploaded batch (B2_FUSED_WARPS: the shape that leaves room for the other batch's kernels; the dense
+// shape for small frames, or while the frame size is not known: a tile may then hold many frames to walk again)
+static uint32_t fused_warps(const b2_ctx* c) { return c->avg_frame && !c->dense ? kFusedWarps : kFusedWarpsDense; }
+// k_resolve's dynamic shared memory: every run's tile records, or none when some run does not fit (EVERY run of the launch then uses the
+// global scratch).  Ahead of k_fused none either: the SM a k_fused CTA holds is configured for it (132 KB of shared memory for its 129),
+// and a k_resolve block only starts beside it without records in shared memory.
+static size_t resolve_smem(const b2_ctx* c, bool fused) { const size_t b = (size_t)c->max_run_tiles * 12; return fused || b > 200 * 1024 ? 0 : b; }
+
+// timed: events around the pass (kernel_ms, b2_stage_times).  b2_batch_launch passes false: a record between two passes of a stream
+// sits on the path from one pass's last kernel to the next pass's first, which runs beside the other stream's k_fused.
+static int launch_pipeline(b2_ctx* c, bool timed = true) {
     const BatchPtrs B = make_ptrs(c);
     DevConfig C = c->cfg;
     // the fused decode+pack kernel serves batches whose bytes and replies both live in HBM
@@ -514,37 +556,42 @@ static int launch_pipeline(b2_ctx* c) {
     const bool prof = c->profile_stages;
     auto mark = [&](const char* name) { if (prof) { c->stage_names[st] = name; cudaEventRecord(c->ev[st + 1], s); st++; } };
     const uint32_t mask = c->stage_mask;
-    if (mask & 1) CU(cudaMemsetAsync(B.totals, 0, 48, s));
-    CU(cudaEventRecord(c->ev[0], s));
+    const bool small_launch = c->small && c->use_fused_small && !prof;
+    // the pass's totals start at zero: k_tile_search zeroes them when it runs (a launch of the other batch's pass then no longer waits
+    // for a memset and a second dependent launch behind it), a memset otherwise
+    const bool search_zeroes = (mask & 1) && c->n_runs && c->n_tiles && !small_launch;
+    if ((mask & 1) && !search_zeroes) CU(cudaMemsetAsync(B.totals, 0, 48, s));
+    if (timed) CU(cudaEventRecord(c->ev[0], s));
     c->stream_ran = false;
     if (c->n_runs == 0) { c->n_stages = 0; c->last_launches = 0; return B2_OK; }
-    if (c->small && c->use_fused_small && !prof) {
+    if (small_launch) {
         // latency path: the whole pipeline in one launch, one CTA
         k_small<<<1, kSmallThreads, sizeof(SmallSmem), s>>>(B, C);
         launches = 1;
         if (c->stream_armed) { int rc = launch_stream_pass(c, B, s, launches); if (rc != B2_OK) return rc; }
-        c->stage_names[0] = "fused_small"; cudaEventRecord(c->ev[1], s);
-        c->n_stages = 1; c->last_launches = launches;
+        c->stage_names[0] = "fused_small";
+        if (timed) cudaEventRecord(c->ev[1], s);
+        c->n_stages = timed ? 1 : 0; c->last_launches = launches;
         CU(cudaGetLastError());
         return B2_OK;
     }
     const uint32_t sms = c->n_sms;
     if (mask & 1) {
     if (c->n_tiles) {
-        k_tile_search<<<(c->n_tiles * 32 + 255) / 256, 256, 0, s>>>(B, C); launches++; mark("tile_search");
+        // (ahead of k_fused, in blocks that start beside the other batch's k_fused: b2_resident_plan)
+        const uint32_t search_threads = fused ? kSearchThreadsFused : 256u;
+        k_tile_search<<<(c->n_tiles * 32 + search_threads - 1) / search_threads, search_threads, 0, s>>>(B, C); launches++; mark("tile_search");
         if (C.pull) k_tile_walk_pull<<<(uint32_t)(((uint64_t)c->n_tiles * 8 + 127) / 128), 128, 0, s>>>(B, C);
         else k_tile_walk<<<(c->n_tiles + 127) / 128, 128, 0, s>>>(B, C);
         launches++; mark("tile_walk");
     }
     {
-        size_t smem = (size_t)c->max_run_tiles * 12;
-        if (smem > 200 * 1024) smem = 0;                 // some run does not fit: EVERY run of this launch uses the global scratch
+        const size_t smem = resolve_smem(c, fused);
         k_resolve<<<c->n_runs, 256, smem, s>>>(B, C, smem == 0 ? 1u : 0u); launches++; mark("resolve");
     }
     if (fused) {
         // one pass over the bytes: decode + echo + pack per live tile (k_frame_table / k_decode / k_scan / k_pack_tma are not needed)
-        // (before a context's first batch has told the average frame size, a tile may hold many frames to walk again: the many-warp shape)
-        const uint32_t fw = c->avg_frame && !c->dense ? kFusedWarps : kFusedWarpsDense;
+        const uint32_t fw = fused_warps(c);
         if (c->n_tiles) { k_fused<<<sms, fw * 32, sizeof(FusedWarpSmem) * fw, s>>>(B, C); launches++; mark("fused"); }
     } else {
     if (c->n_tiles) { k_frame_table<<<(uint32_t)(((uint64_t)c->n_tiles * C.spec_k + 255) / 256), 256, 0, s>>>(B, C); launches++; mark("frame_table"); }
@@ -556,7 +603,8 @@ static int launch_pipeline(b2_ctx* c) {
     }
     }
     if (fused) {
-        if (mask & 4) { k_pack_slow<true><<<sms * B2_SLOW_MIN_BLOCKS, 256, 0, s>>>(B, C); launches++; mark("pack_slow"); }
+        // (as many warps as k_pack_slow<false> gets, in blocks that start beside the other batch's k_fused)
+        if (mask & 4) { k_pack_slow<true><<<sms * B2_SLOW_MIN_BLOCKS * (256 / kSlowLiteThreads), kSlowLiteThreads, 0, s>>>(B, C); launches++; mark("pack_slow"); }
     } else if (c->use_tma_pack) {
         // the verify pass decides which CRC-carrying echoes k_pack_tma may move; k_pack_slow answers the ones that fail
         if (mask & 4) {
@@ -575,7 +623,7 @@ static int launch_pipeline(b2_ctx* c) {
         launches++; mark("emit_iov");
     }
     if (c->stream_armed) { int rc = launch_stream_pass(c, B, s, launches); if (rc != B2_OK) return rc; }
-    if (!prof) { c->stage_names[0] = "pipeline"; cudaEventRecord(c->ev[1], s); st = 1; }
+    if (!prof && timed) { c->stage_names[0] = "pipeline"; cudaEventRecord(c->ev[1], s); st = 1; }
     c->n_stages = st; c->last_launches = launches;
     CU(cudaGetLastError());
     return B2_OK;
@@ -632,7 +680,7 @@ extern "C" int b2_batch_launch(b2_ctx* c) {
     if (replay_refused(c)) return B2_E_INVAL;
     CU(cudaSetDevice(c->opt.device));
     if (c->first_pending) { CU(cudaEventRecord(c->ev_first, c->stream)); c->first_pending = false; }
-    int rc = launch_pipeline(c);
+    int rc = launch_pipeline(c, false);
     if (rc != B2_OK) return rc;
     CU(cudaEventRecord(c->ev_last, c->stream));
     c->executed = true;
@@ -1327,6 +1375,41 @@ extern "C" int b2_batch_info(b2_ctx* c, uint32_t out[4]) {
     if (!c || !out) return B2_E_INVAL;
     out[0] = c->cfg.tile_bytes; out[1] = c->n_tiles; out[2] = c->cfg.spec_k; out[3] = c->fused_last ? 1u : 0u;
     return B2_OK;
+}
+
+// Registers are allocated per warp in units of 256 (8 per thread); shared memory per block adds the SM's per-block reserve.  An SM's
+// shared memory is configured in steps (sm_90: 0, 8, 16, 32, 64, 100, 132, 164, 196 or 228 KB): one that a k_fused CTA holds is set to
+// the smallest step that holds the CTA, and the blocks beside it share what that step leaves (a k_resolve block with its tile records in
+// shared memory was seen to wait for the k_fused CTA to end).
+static uint32_t block_regs(const b2_resident_kernel& k) { return (k.threads + 31) / 32 * ((k.regs * 32 + 255) / 256 * 256); }
+static uint32_t smem_step(uint32_t bytes, uint32_t most) {
+    static const uint32_t kKB[] = { 0, 8, 16, 32, 64, 100, 132, 164, 196, 228 };
+    for (uint32_t kb : kKB) if (kb * 1024 >= bytes) return std::min(kb * 1024, most);
+    return most;
+}
+extern "C" int b2_resident_plan(b2_ctx* c, b2_resident_kernel* out, int cap) {
+    if (!c || (!out && cap > 0)) { set_err("null argument"); return B2_E_INVAL; }
+    if (!c->plan[kPlanFused].name) { set_err("this build has no function attributes to plan with"); return B2_E_INVAL; }
+    b2_resident_kernel k[kPlanKernels];
+    memcpy(k, c->plan, sizeof k);
+    const uint32_t fw = fused_warps(c);
+    k[kPlanFused].threads = fw * 32; k[kPlanFused].smem_bytes += (uint32_t)(sizeof(FusedWarpSmem) * fw);
+    k[kPlanResolve].smem_bytes += (uint32_t)resolve_smem(c, true);
+    // the room one k_fused CTA leaves on its SM
+    const b2_resident_kernel& f = k[kPlanFused];
+    const uint32_t f_regs = block_regs(f), f_smem = f.smem_bytes + c->block_smem_reserve;
+    const uint32_t room_regs = c->sm_regs > f_regs ? c->sm_regs - f_regs : 0, f_step = smem_step(f_smem, c->sm_smem);
+    const uint32_t room_smem = f_step > f_smem ? f_step - f_smem : 0;
+    const uint32_t room_warps = c->sm_warps > fw ? c->sm_warps - fw : 0, room_blocks = c->sm_blocks > 1 ? c->sm_blocks - 1 : 0;
+    for (int i = 0; i < kPlanKernels; i++) {
+        uint32_t n = room_blocks;
+        n = std::min(n, room_regs / std::max(1u, block_regs(k[i])));
+        n = std::min(n, room_smem / (k[i].smem_bytes + c->block_smem_reserve));
+        n = std::min(n, room_warps / ((k[i].threads + 31) / 32));
+        k[i].fits = n;
+    }
+    for (int i = 0; i < kPlanKernels && i < cap; i++) out[i] = k[i];
+    return kPlanKernels;
 }
 
 extern "C" int b2_device_pci_bus_id(int device, char* out, int cap) {

@@ -170,9 +170,13 @@ __device__ __forceinline__ bool is_magic(uint32_t w) { return w == kMagicPRPC ||
 // Finds the first position p in the tile where a frame of either protocol parses
 // completely (header sane, whole body inside the run) and is followed by another
 // magic or the run tail.  Pure speculation: k_resolve accepts it only if the true
-// chain arrives exactly there.
+// chain arrives exactly there.  Any block size (a warp's tile is its global warp index).  Ahead of k_fused it runs in 128-thread
+// blocks: 40 registers x 128 threads = 5,120 per block, so three blocks (12 warps) start on an SM that one 12-warp k_fused CTA of
+// the other batch holds, where a 256-thread block fits once (8 warps).
+constexpr uint32_t kSearchThreadsFused = 128;
 __global__ void __launch_bounds__(256, 6) k_tile_search(BatchPtrs B, DevConfig C) {
     const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (blockIdx.x == 0 && threadIdx.x < 12) B.totals[threadIdx.x] = 0;     // the pass's totals (the first kernel of a pass with tiles)
     if (warp >= B.n_tiles) return;
     const uint4 ti = __ldg(B.tile_info + warp);
     const uint32_t k = ti.z;
@@ -2059,9 +2063,10 @@ __global__ void __launch_bounds__(kPackWarps * 32, 1) k_pack_tma(BatchPtrs B, De
 #define B2_FUSED_BUF 10240
 #endif
 // Warps per CTA, chosen per batch at launch.  Measured on an H100 80GB HBM3 (700 W limit, 1980 MHz SM clock), bench.py with two batches
-// in flight: 12 warps x 128 registers leave 16K registers and ~100 KB of shared memory per SM, room for a k_resolve or k_tile_search
-// block (256 threads x 40 registers) of the other batch beside this kernel: 1 KB requests 1086 M msgs/s (16 warps: ~1045 M), 4 KB
-// 274 M (264 M), 1024 connections x 256 KiB 1065 M (1005 M).  Dense tiles (small requests, several rounds per tile, or tiles whose
+// in flight: 12 warps x 114 registers (allocated as 120 per thread, 46,080 per CTA) leave 19,456 of the SM's 65,536 registers, and the
+// SM's shared memory is configured at 132 KB for the CTA's 129 KB: the room the other batch's front stages and k_pack_slow<true> run in
+// beside this kernel (b2_resident_plan reports what fits there; the dense shape leaves 4,096 registers, where none of them fit): 1 KB
+// requests 1086 M msgs/s (16 warps: ~1045 M), 4 KB 274 M (264 M), 1024 connections x 256 KiB 1065 M (1005 M).  Dense tiles (small requests, several rounds per tile, or tiles whose
 // frames are walked again by lane 0 because the context did not know yet that they are small) want the whole register file instead:
 // 64 B requests 2980 M msgs/s with 16 warps, 2680 M with 12; 256 B 2248 M against 1995 M.
 #ifndef B2_FUSED_WARPS
@@ -2537,7 +2542,11 @@ __global__ void __launch_bounds__(256) k_pack_responses(const uint8_t* bytes, co
 #define B2_SLOW_MIN_BLOCKS 3
 #endif
 // kLite: no shared memory at all (CRC tables read through L1, no snappy ring) — the variant launched behind k_fused, where slow messages
-// are rare by construction and the kernel must be able to start on SMs whose shared memory the next batch's k_fused already holds
+// are rare by construction and the kernel must be able to start on SMs the other batch's k_fused already holds.  It is launched with
+// kSlowLiteThreads: at 80 registers a 256-thread block needs 20,480 registers, more than the 19,456 a 12-warp k_fused CTA leaves, so it
+// would wait for that k_fused to end and hold the next pass of its own stream behind it; a 128-thread block (10,240) starts beside it.
+// (The register count is left uncapped: at 80 the kernel already spills.)
+constexpr uint32_t kSlowLiteThreads = 128;
 template <bool kLite>
 __global__ void __launch_bounds__(256, B2_SLOW_MIN_BLOCKS) k_pack_slow(BatchPtrs B, DevConfig C) {
     const uint32_t lane = threadIdx.x & 31;

@@ -367,7 +367,8 @@ int  b2_batch_execute_many(b2_ctx* ctx, uint32_t steps, float* total_ms, uint32_
 /* Asynchronous form for pipelining several resident batches (one ctx each) on one GPU:
  * b2_batch_launch enqueues one pass on the ctx's stream and returns; b2_batch_wait blocks
  * until it is done.  b2_elapsed_ms(a, b) = device time from a's FIRST launch since its last
- * wait to b's LAST launch end (CUDA events; a and b may be the same ctx). */
+ * wait to b's LAST launch end (CUDA events; a and b may be the same ctx).  A launched pass records no stage events: b2_stage_times reports
+ * none after it, and kernel_ms keeps the value of the last executed or collected batch. */
 int  b2_batch_launch(b2_ctx* ctx);
 int  b2_batch_wait(b2_ctx* ctx);
 int  b2_elapsed_ms(b2_ctx* a, b2_ctx* b, float* ms);
@@ -375,6 +376,19 @@ int  b2_elapsed_ms(b2_ctx* a, b2_ctx* b, float* ms);
 /* What the last upload / launch decided: out[0] tile bytes, [1] tiles, [2] frame offsets kept per tile, [3] 1 = the fused
  * decode+pack kernel served the batch (0 = the slot-scan pipeline). */
 int  b2_batch_info(b2_ctx* ctx, uint32_t out[4]);
+
+/* Residency of a fused pass.  Two contexts on two streams overlap their passes: one batch's front stages (k_tile_search, k_tile_walk,
+ * k_resolve) and slow-reply kernel (k_pack_slow<true>) run on the SMs the other batch's k_fused holds, which they can only do where one
+ * of their blocks fits in what a k_fused CTA leaves of the SM.  Entry 0 is k_fused in the shape the uploaded batch uses, then those four
+ * kernels as launched: registers per thread and static shared memory from the compiled kernels, threads per block, shared memory per
+ * block including the dynamic part for the uploaded batch, and `fits`, the number of blocks an SM holding one k_fused CTA can start
+ * beside it (registers allocated 256 per warp; the shared memory the SM is configured with for the k_fused CTA, in the device's steps,
+ * less the CTA's own and each block's reserve; warp and block slots).  Writes up to `cap` entries and returns the number of kernels (5). */
+typedef struct b2_resident_kernel {
+    const char* name;
+    uint32_t regs, threads, smem_bytes, fits;
+} b2_resident_kernel;   /* 24 bytes */
+int  b2_resident_plan(b2_ctx* ctx, b2_resident_kernel* out, int cap);
 
 /* PCI bus id ("0000:1b:00.0") of a device, for a host side that wants to run its polling threads and first-touch its pinned blocks on
  * the CPUs next to the GPU (/sys/bus/pci/devices/<id>/local_cpulist): zero-copy reads that cross the socket interconnect lose most of
