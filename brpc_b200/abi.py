@@ -147,6 +147,8 @@ def _load():
     l.b2_set_server_identity.argtypes = [C.c_void_p, C.c_char_p]
     l.b2_set_stream_handler.argtypes = [C.c_void_p, C.c_int]
     l.b2_set_protocols.argtypes = [C.c_void_p, C.c_uint32]
+    l.b2_set_walk_group.argtypes = [C.c_void_p, C.c_uint32]
+    l.b2_walk_group.argtypes = [C.c_void_p]
     l.b2_block_alloc.restype = C.c_void_p; l.b2_block_alloc.argtypes = [C.c_size_t]
     l.b2_block_free.argtypes = [C.c_void_p]
     l.b2_block_pool_host_allocs.restype = C.c_uint64
@@ -229,7 +231,7 @@ lib = _load()
 ABI_SYMBOLS = ["b2_ctx_create", "b2_ctx_destroy", "b2_last_error", "b2_version", "b2_register_method",
                "b2_set_server_identity", "b2_set_stream_handler", "b2_set_protocols", "b2_block_alloc", "b2_block_free", "b2_block_pool_host_allocs", "b2_set_modes", "b2_ring_start", "b2_ring_stop", "b2_ring_submit", "b2_ring_wait", "b2_ring_launches", "b2_ring_phase_ns", "b2_latency_probe", "b2_process_batch", "b2_batch_submit", "b2_batch_collect", "b2_batch_upload",
                "b2_batch_execute", "b2_batch_execute_many", "b2_batch_download", "b2_batch_launch", "b2_batch_wait",
-               "b2_elapsed_ms", "b2_batch_info", "b2_resident_plan", "b2_device_pci_bus_id", "b2_stage_times", "b2_crc32c_batch", "b2_crc32c_extend", "b2_snappy_max_compressed_length", "b2_snappy_raw_compress", "b2_snappy_get_uncompressed_length", "b2_snappy_raw_uncompress", "b2_snappy_uncompress_batch", "b2_snappy_compress_batch", "b2_hpack_reset", "b2_hpack_decode_batch", "b2_pack_requests", "b2_pack_responses", "b2_h2_scan_batch", "b2_h2_conn_reset", "b2_h2_configure", "b2_h2_process_batch", "b2_h2_pack_responses", "b2_counters_read",
+               "b2_elapsed_ms", "b2_batch_info", "b2_set_walk_group", "b2_walk_group", "b2_resident_plan", "b2_device_pci_bus_id", "b2_stage_times", "b2_crc32c_batch", "b2_crc32c_extend", "b2_snappy_max_compressed_length", "b2_snappy_raw_compress", "b2_snappy_get_uncompressed_length", "b2_snappy_raw_uncompress", "b2_snappy_uncompress_batch", "b2_snappy_compress_batch", "b2_hpack_reset", "b2_hpack_decode_batch", "b2_pack_requests", "b2_pack_responses", "b2_h2_scan_batch", "b2_h2_conn_reset", "b2_h2_configure", "b2_h2_process_batch", "b2_h2_pack_responses", "b2_counters_read",
                "b2_counters_device_ptr", "b2_counters_allreduce", "b2_h2_pack_requests", "b2_h2_conn_set_next_stream_id", "b2_h2_conn_peer_update",
                "b2_h2_client_conn_reset", "b2_h2_client_process_batch", "b2_h2_client_abandon_streams", "b2_h2_conn_set_gunzip",
                "b2_h2_serve_batch", "b2_stream_configure", "b2_stream_open", "b2_stream_set_connected", "b2_stream_close", "b2_stream_query",
@@ -400,6 +402,14 @@ class Context:
 
     def set_protocols(self, mask):
         _check(lib.b2_set_protocols(self._h, mask))
+
+    def set_walk_group(self, mode):
+        """Tiles per walk group of the front stages: 0 auto, 1 one tile per group, 2..8 forced (b2_set_walk_group); upload again after."""
+        _check(lib.b2_set_walk_group(self._h, mode))
+
+    def walk_group(self):
+        """The walk group size the last launch used."""
+        return _check(lib.b2_walk_group(self._h))
 
     def set_modes(self, input_mode=INPUT_COPY, resp_mode=RESP_COPY):
         _check(lib.b2_set_modes(self._h, input_mode, resp_mode))

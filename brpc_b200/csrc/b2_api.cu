@@ -63,7 +63,7 @@ struct b2_ctx {
     std::vector<DevMethod> methods;
     // device
     uint8_t* d_bytes = nullptr; b2_run* d_runs = nullptr; uint32_t* d_run_tile_base = nullptr;
-    TileRec* d_tiles = nullptr; uint32_t* d_tile_base = nullptr; uint32_t* d_tile_scratch = nullptr; uint32_t* d_tile_spec = nullptr; b2_run_status* d_run_status = nullptr;
+    TileRec* d_tiles = nullptr; uint32_t* d_tile_base = nullptr; uint32_t* d_tile_scratch = nullptr; TileRec* d_head_recs = nullptr; uint32_t* d_tile_spec = nullptr; b2_run_status* d_run_status = nullptr;
     uint32_t* d_frame_off = nullptr; uint32_t* d_frame_run = nullptr; b2_msg_desc* d_msgs = nullptr; MsgAux* d_aux = nullptr; PackJob* d_jobs = nullptr; uint32_t* d_slow_idx = nullptr; uint8_t* d_heads = nullptr;
     uint32_t* d_slot = nullptr; uint32_t* d_scan_tmp = nullptr; uint8_t* d_resp = nullptr; uint8_t* d_unz = nullptr; uint16_t* d_snappy_tab = nullptr; HpackState* d_hpack = nullptr; H2Conn* d_h2 = nullptr; H2Stream* d_h2_streams = nullptr; uint8_t* d_h2_slots = nullptr; uint32_t h2_max_conns = B2_H2_MAX_CONNS, h2_pending = B2_H2_MAX_PENDING, h2_stream_bytes = B2_H2_STREAM_BYTES; uint64_t h2_last_in = 0, h2_last_out = 0;   // sizes of the last h2 batch still on the device
     uint32_t* d_frame_row = nullptr; uint4* d_rows = nullptr;
@@ -110,6 +110,9 @@ struct b2_ctx {
     cudaEvent_t ev_first = nullptr, ev_last = nullptr; bool first_pending = true;
     bool profile_stages = false; bool allow_small = true; bool use_fused = true; bool fused_last = false; bool slow_heavy = false;   // slow_heavy: the previous batch sent > 1/8 of its messages to k_pack_slow (CRC'd / compressed traffic): the classic pipeline serves that better
     bool adaptive_tile = false; bool dense = false; uint32_t avg_frame = 0;   // tile size follows the message size of the previous batch      // per-stage events only when a harness asks for stage times
+    // walk groups (k_tile_search / k_tile_walk, DESIGN §3): b2_set_walk_group's mode (0 auto, 1 off, 2..8 forced), the uploaded batch's
+    // group size and group count (the heads follow tile_info in the meta block), and the group size the last launch used
+    uint32_t walk_group_mode = 0, walk_group = 1, n_groups = 0, walk_group_last = 1; size_t meta_group_off = 0;
     // small-batch (latency) mode: one compact H2D block, one compact output block, one D2H, one sync
     uint8_t* d_meta = nullptr; uint8_t* h_meta = nullptr;       // [runs | run_tile_base]
     uint8_t* d_small = nullptr; uint8_t* h_small = nullptr;     // [totals | run_status | msgs | resp]
@@ -211,7 +214,7 @@ extern "C" void b2_ctx_destroy(b2_ctx* c) {
     if (c->ring_slots) cudaFreeHost(c->ring_slots);
     if (c->ring_ctl) cudaFreeHost((void*)c->ring_ctl);
     cudaFree(c->d_ring_ticket);
-    cudaFree(c->d_bytes); cudaFree(c->d_runs); cudaFree(c->d_run_tile_base); cudaFree(c->d_tiles); cudaFree(c->d_tile_base); cudaFree(c->d_tile_scratch); cudaFree(c->d_tile_spec);
+    cudaFree(c->d_bytes); cudaFree(c->d_runs); cudaFree(c->d_run_tile_base); cudaFree(c->d_tiles); cudaFree(c->d_tile_base); cudaFree(c->d_tile_scratch); cudaFree(c->d_head_recs); cudaFree(c->d_tile_spec);
     cudaFree(c->d_run_status); cudaFree(c->d_frame_off); cudaFree(c->d_frame_run); cudaFree(c->d_msgs); cudaFree(c->d_aux); cudaFree(c->d_jobs); cudaFree(c->d_slow_idx); cudaFree(c->d_heads); cudaFree(c->d_slot);
     cudaFree(c->d_scan_tmp); cudaFree(c->d_resp); cudaFree(c->d_unz); cudaFree(c->d_snappy_tab); cudaFree(c->d_refs); cudaFree(c->d_iov); cudaFreeHost(c->h_iov); cudaFree(c->d_frame_row); cudaFree(c->d_rows); cudaFreeHost(c->h_refs); cudaFree(c->d_hpack); cudaFree(c->d_h2); cudaFree(c->d_h2_streams); cudaFree(c->d_h2_slots); cudaFree(c->d_h2_gz_merge); cudaFree(c->d_counters); cudaFree(c->d_totals); cudaFree(c->d_methods); cudaFree(c->d_crc_adv); cudaFree(c->d_meta); cudaFree(c->d_small); cudaFreeHost(c->h_meta); cudaFreeHost(c->h_small);
     cudaFreeHost(c->h_run_status); cudaFreeHost(c->h_msgs); cudaFreeHost(c->h_resp); cudaFreeHost(c->h_totals);
@@ -260,6 +263,7 @@ extern "C" int b2_ctx_create(const b2_options* o, b2_ctx** out) {
     ALLOC(c->d_tiles, sizeof(TileRec) * (size_t)c->max_tiles);
     ALLOC(c->d_tile_base, 4 * (size_t)c->max_tiles);
     ALLOC(c->d_tile_scratch, 12 * (size_t)c->max_tiles);
+    ALLOC(c->d_head_recs, sizeof(TileRec) * (size_t)c->max_tiles);
     {   // kSpecK offsets per tile; dense mode (tiles >= 2 KiB holding many small frames) keeps kSpecKDense
         size_t dense_tiles = (size_t)o->max_batch_bytes / 2048 + o->max_runs + 1; if (dense_tiles > c->max_tiles) dense_tiles = c->max_tiles;
         size_t words = (size_t)kSpecK * c->max_tiles; if ((size_t)kSpecKDense * dense_tiles > words) words = (size_t)kSpecKDense * dense_tiles;
@@ -285,9 +289,9 @@ extern "C" int b2_ctx_create(const b2_options* o, b2_ctx** out) {
     ALLOC(c->d_totals, 64);
     ALLOC(c->d_methods, sizeof(DevMethod) * 64);
     ALLOC(c->d_crc_adv, (kCrcHotWords + kCrcTreeWords) * 4);
-    ALLOC(c->d_meta, (size_t)o->max_runs * 28 + 16 * (size_t)c->max_tiles + 64);
+    ALLOC(c->d_meta, (size_t)o->max_runs * 28 + 36 * (size_t)c->max_tiles + 64);
     ALLOC(c->d_small, kSmallBlock);
-    HALLOC(c->h_meta, (size_t)o->max_runs * 28 + 16 * (size_t)c->max_tiles + 64);
+    HALLOC(c->h_meta, (size_t)o->max_runs * 28 + 36 * (size_t)c->max_tiles + 64);
     HALLOC(c->h_small, kSmallBlock);
     HALLOC(c->h_run_status, sizeof(b2_run_status) * (size_t)o->max_runs);
     HALLOC(c->h_msgs, sizeof(b2_msg_desc) * (size_t)o->max_msgs);
@@ -428,6 +432,8 @@ static BatchPtrs make_ptrs(b2_ctx* c) {
     B.runs = reinterpret_cast<const b2_run*>(c->d_meta);
     B.run_tile_base = reinterpret_cast<const uint32_t*>(c->d_meta + (size_t)c->n_runs * sizeof(b2_run));
     B.tile_info = reinterpret_cast<const uint4*>(c->d_meta + c->meta_tile_off);
+    B.group_heads = reinterpret_cast<const uint32_t*>(c->d_meta + c->meta_group_off + 16 * (size_t)c->n_groups); B.head_recs = c->d_head_recs;
+    B.n_groups = c->n_groups; B.walk_group = 1;     // (launch_pipeline groups)
     if (c->input_mode == B2_INPUT_PULL) B.bytes = c->pull_bytes;          // the caller's pinned + mapped batch buffer, read in place
     if (c->small) {
         B.refs = reinterpret_cast<uint4*>(c->d_small + c->sm.off_refs);
@@ -438,6 +444,20 @@ static BatchPtrs make_ptrs(b2_ctx* c) {
         B.max_msgs = c->sm.msgs; B.max_resp = c->sm.resp;
     }
     return B;
+}
+
+// The fused decode+pack kernel serves batches whose bytes and replies both live in HBM
+static bool takes_fused(const b2_ctx* c) {
+    return c->use_fused && !c->slow_heavy && !c->small && c->input_mode == B2_INPUT_COPY && c->resp_mode == B2_RESP_COPY && c->use_tma_pack &&
+           (((uint64_t)c->nbytes + 255) & ~255ull) + 4096 <= c->opt.max_resp_bytes;
+}
+// Walk group of an uploaded batch.  Auto: 2 tiles on the fused path once the frame size is known and frames are not dense — the search
+// then reads half the windows, and the walk's longer chain still ends under the other batch's k_fused (4 and 8 tiles were slower on the
+// bench batch, DESIGN §9.1) — else 1 (pull mode keeps its own walk).
+static uint32_t pick_walk_group(const b2_ctx* c) {
+    if (c->input_mode == B2_INPUT_PULL || c->walk_group_mode == 1) return 1;
+    if (c->walk_group_mode >= 2) return c->walk_group_mode;
+    return takes_fused(c) && c->avg_frame && !c->dense ? 2u : 1u;
 }
 
 extern "C" int b2_batch_upload(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs) {
@@ -484,10 +504,18 @@ extern "C" int b2_batch_upload(b2_ctx* c, const void* bytes, uint32_t nbytes, co
     c->h_run_tile_base[n_runs] = (uint32_t)nt;
     if (nt > c->max_tiles) { set_err("too many tiles"); return B2_E_CAPACITY; }
     c->n_runs = n_runs; c->n_tiles = (uint32_t)nt; c->nbytes = nbytes; c->max_run_tiles = max_rt; c->host_bytes = bytes;
-    // runs + tile bases travel as one compact block (24 B * n is 4-byte aligned)
+    // latency path: outputs of a small batch live in one compact block -> one D2H copy, one sync
+    c->small = c->allow_small && nbytes <= kSmallBytes && n_runs <= kSmallRuns && n_runs > 0;
+    c->walk_group = pick_walk_group(c);
+    // runs + tile bases travel as one compact block (24 B * n is 4-byte aligned), then the tile records, and with walk groups the
+    // heads' tile records (k_tile_search's tiles) and tile indices
     const size_t tile_off = ((size_t)n_runs * sizeof(b2_run) + 4 * ((size_t)n_runs + 1) + 15) & ~(size_t)15;
-    const size_t meta_bytes = tile_off + 16 * (size_t)nt;
-    c->meta_tile_off = tile_off;
+    c->meta_tile_off = tile_off; c->meta_group_off = tile_off + 16 * (size_t)nt;
+    uint32_t ng = 0;
+    if (c->walk_group > 1)
+        for (uint32_t r = 0; r < n_runs; r++) ng += (c->h_run_tile_base[r + 1] - c->h_run_tile_base[r] + c->walk_group - 1) / c->walk_group;
+    c->n_groups = ng;
+    const size_t meta_bytes = c->meta_group_off + 20 * (size_t)ng;
     if (n_runs) memcpy(c->h_meta, runs, (size_t)n_runs * sizeof(b2_run));
     memcpy(c->h_meta + (size_t)n_runs * sizeof(b2_run), c->h_run_tile_base, 4 * ((size_t)n_runs + 1));
     {   // per-tile record {run offset, run length, tile index in the run, run | flags << 24}: one load per tile thread
@@ -496,6 +524,12 @@ extern "C" int b2_batch_upload(b2_ctx* c, const void* bytes, uint32_t nbytes, co
             const uint32_t t0 = c->h_run_tile_base[r], t1 = c->h_run_tile_base[r + 1];
             for (uint32_t t = t0; t < t1; t++) { uint32_t* q = ti + 4 * (size_t)t; q[0] = runs[r].offset; q[1] = runs[r].length; q[2] = t - t0; q[3] = r | (runs[r].flags << 24); }
         }
+        uint32_t* hi = reinterpret_cast<uint32_t*>(c->h_meta + c->meta_group_off);
+        uint32_t* heads = hi + 4 * (size_t)ng;
+        uint32_t g = 0;
+        if (c->walk_group > 1)
+            for (uint32_t r = 0; r < n_runs; r++)
+                for (uint32_t t = c->h_run_tile_base[r]; t < c->h_run_tile_base[r + 1]; t += c->walk_group, g++) { memcpy(hi + 4 * (size_t)g, ti + 4 * (size_t)t, 16); heads[g] = t; }
     }
     overwrites(c, kDevInput | kDevBatch);
     if (c->input_mode == B2_INPUT_PULL) {
@@ -507,8 +541,6 @@ extern "C" int b2_batch_upload(b2_ctx* c, const void* bytes, uint32_t nbytes, co
         c->pull_bytes = static_cast<const uint8_t*>(dp);
     } else if (nbytes) CU(cudaMemcpyAsync(c->d_bytes, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(c->d_meta, c->h_meta, meta_bytes, cudaMemcpyHostToDevice, c->stream));
-    // latency path: outputs of a small batch live in one compact block -> one D2H copy, one sync
-    c->small = c->allow_small && nbytes <= kSmallBytes && n_runs <= kSmallRuns && n_runs > 0;
     if (c->small) c->sm = small_layout(nbytes, n_runs, c->opt.max_msgs);
     if (const char* e = getenv("B2_STAGE_MASK")) c->stage_mask = (uint32_t)atoi(e);   // timing experiments only (tools/overlap_probe.py)
     c->uploaded = true;
@@ -545,11 +577,12 @@ static size_t resolve_smem(const b2_ctx* c, bool fused) { const size_t b = (size
 // timed: events around the pass (kernel_ms, b2_stage_times).  b2_batch_launch passes false: a record between two passes of a stream
 // sits on the path from one pass's last kernel to the next pass's first, which runs beside the other stream's k_fused.
 static int launch_pipeline(b2_ctx* c, bool timed = true) {
-    const BatchPtrs B = make_ptrs(c);
+    BatchPtrs B = make_ptrs(c);
     DevConfig C = c->cfg;
-    // the fused decode+pack kernel serves batches whose bytes and replies both live in HBM
-    const bool fused = c->use_fused && !c->slow_heavy && !c->small && c->input_mode == B2_INPUT_COPY && c->resp_mode == B2_RESP_COPY && c->use_tma_pack &&
-                       (((uint64_t)c->nbytes + 255) & ~255ull) + 4096 <= c->opt.max_resp_bytes;
+    const bool fused = takes_fused(c);
+    // the upload's walk groups, unless auto mode picked them for the fused path and this launch takes the slot-scan pipeline
+    B.walk_group = fused || c->walk_group_mode >= 2 ? c->walk_group : 1u;
+    c->walk_group_last = B.walk_group;
     C.fused = fused ? 1u : 0u; C.ovf_base = (c->nbytes + 255u) & ~255u; c->fused_last = fused;
     cudaStream_t s = c->stream;
     int st = 0; uint32_t launches = 0;
@@ -580,8 +613,11 @@ static int launch_pipeline(b2_ctx* c, bool timed = true) {
     if (c->n_tiles) {
         // (ahead of k_fused, in blocks that start beside the other batch's k_fused: b2_resident_plan)
         const uint32_t search_threads = fused ? kSearchThreadsFused : 256u;
-        k_tile_search<<<(c->n_tiles * 32 + search_threads - 1) / search_threads, search_threads, 0, s>>>(B, C); launches++; mark("tile_search");
+        BatchPtrs S = B;                            // (walk groups: only the heads are searched, their entries go to head_recs)
+        if (B.walk_group > 1) { S.tile_info = reinterpret_cast<const uint4*>(c->d_meta + c->meta_group_off); S.tiles = B.head_recs; S.n_tiles = c->n_groups; }
+        k_tile_search<<<(S.n_tiles * 32 + search_threads - 1) / search_threads, search_threads, 0, s>>>(S, C); launches++; mark("tile_search");
         if (C.pull) k_tile_walk_pull<<<(uint32_t)(((uint64_t)c->n_tiles * 8 + 127) / 128), 128, 0, s>>>(B, C);
+        else if (B.walk_group > 1) k_tile_walk<<<(c->n_groups + kWalkGroupThreads - 1) / kWalkGroupThreads, kWalkGroupThreads, 0, s>>>(B, C);
         else k_tile_walk<<<(c->n_tiles + 127) / 128, 128, 0, s>>>(B, C);
         launches++; mark("tile_walk");
     }
@@ -1371,6 +1407,15 @@ extern "C" int b2_stage_times(b2_ctx* c, const char** names, float* ms, int cap)
 }
 
 // what the last upload / launch decided: [0] tile bytes [1] tiles [2] frame offsets kept per tile [3] 1 = the fused kernel served it
+extern "C" int b2_set_walk_group(b2_ctx* c, uint32_t mode) {
+    if (!c || mode > 8) { set_err("walk group mode: 0 auto, 1 off, 2..8 tiles per group"); return B2_E_INVAL; }
+    c->walk_group_mode = mode;
+    overwrites(c, kDevBatch);                       // (the uploaded batch's groups were laid out for the old mode)
+    return B2_OK;
+}
+
+extern "C" int b2_walk_group(b2_ctx* c) { return c ? (int)c->walk_group_last : B2_E_INVAL; }
+
 extern "C" int b2_batch_info(b2_ctx* c, uint32_t out[4]) {
     if (!c || !out) return B2_E_INVAL;
     out[0] = c->cfg.tile_bytes; out[1] = c->n_tiles; out[2] = c->cfg.spec_k; out[3] = c->fused_last ? 1u : 0u;
@@ -1395,6 +1440,7 @@ extern "C" int b2_resident_plan(b2_ctx* c, b2_resident_kernel* out, int cap) {
     const uint32_t fw = fused_warps(c);
     k[kPlanFused].threads = fw * 32; k[kPlanFused].smem_bytes += (uint32_t)(sizeof(FusedWarpSmem) * fw);
     k[kPlanResolve].smem_bytes += (uint32_t)resolve_smem(c, true);
+    if (c->walk_group > 1) k[kPlanWalk].threads = kWalkGroupThreads;
     // the room one k_fused CTA leaves on its SM
     const b2_resident_kernel& f = k[kPlanFused];
     const uint32_t f_regs = block_regs(f), f_smem = f.smem_bytes + c->block_smem_reserve;

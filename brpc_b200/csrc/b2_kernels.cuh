@@ -94,6 +94,8 @@ struct BatchPtrs {
     const uint32_t* run_tile_base;   // [n_runs+1] first tile of each run
     const uint4* tile_info;          // [n_tiles] {run offset, run length, tile index inside the run, run index | run flags << 24}: host-built with
                                      // the batch so that a tile thread needs ONE load, not a tile->run->runs[] chain, before it can touch the bytes
+    const uint32_t* group_heads;     // [n_groups] first tile of every walk group (walk_group > 1); k_tile_walk walks each group
+    TileRec* head_recs;              // [n_groups] the groups' speculative entries: k_tile_search searches only the heads and writes here
     TileRec* tiles;
     uint32_t* tile_base;             // [n_tiles] run-relative index of the tile's first message
     uint32_t* tile_scratch;          // [3 * n_tiles] k_resolve spill when a run's tiles exceed shared memory
@@ -121,6 +123,7 @@ struct BatchPtrs {
     const DevMethod* methods;
     const uint32_t* crc_adv;         // warp CRC tables: hot [20][256] then tree [5][4][256]
     uint32_t n_runs, n_tiles, max_msgs, max_resp;
+    uint32_t n_groups, walk_group;   // walk groups of this launch (walk_group tiles each, fewer at a run's end); walk_group 1 = per tile
 };
 
 // ---------------------------------------------------------------------------
@@ -167,6 +170,7 @@ __device__ __forceinline__ bool is_magic(uint32_t w) { return w == kMagicPRPC ||
 #endif
 
 // --- k_tile_search: one warp per tile ---------------------------------------
+// (walk groups: the launch's BatchPtrs name the group heads as its tiles — tile_info = head_info, tiles = head_recs, n_tiles = n_groups)
 // Finds the first position p in the tile where a frame of either protocol parses
 // completely (header sane, whole body inside the run) and is followed by another
 // magic or the run tail.  Pure speculation: k_resolve accepts it only if the true
@@ -272,45 +276,101 @@ __device__ __forceinline__ HdrWords load_hdr_words(const uint8_t* p) {          
     HdrWords h; h.w0 = __ldg(q); h.w1 = __ldg(q + 1); h.w2 = __ldg(q + 2); h.w3 = __ldg(q + 3);
     return h;
 }
+// One step of the speculative walk at `pos` (the header chain of one connection; `a` carries the guessed next header).  The guess is only
+// loaded while it lies before `ahead_end`, where the walker stops.
+struct SpecAhead { HdrWords pre; uint32_t pre_pos, prev_len; };
+__device__ __forceinline__ Step spec_step(const uint8_t* run, uint32_t len, uint32_t pos, int pf, uint32_t ahead_end,
+                                          uint64_t max_body, bool client, uint32_t mask, SpecAhead& a) {
+    Step s;
+    bool fast = false;
+    if (len - pos >= 12) {
+        const HdrWords h = a.pre_pos == pos ? a.pre : load_hdr_words(run + pos);
+        const uint32_t guess = pos + a.prev_len;
+        // (guess <= len - 12, written so that a guess past the run's end — the last tile's end lies beyond it — cannot wrap around)
+        if (a.prev_len && guess < ahead_end && (uint64_t)guess + 12 <= len) { a.pre = load_hdr_words(run + guess); a.pre_pos = guess; }   // in flight while h is used
+        else a.pre_pos = kNone;
+        const uint32_t sh = 8u * (pos & 3u);                      // run offsets are 16-byte aligned: alignment of run + pos is pos & 3
+        const uint32_t h0 = sh ? __funnelshift_r(h.w0, h.w1, sh) : h.w0, h1 = sh ? __funnelshift_r(h.w1, h.w2, sh) : h.w1,
+                       h2 = sh ? __funnelshift_r(h.w2, h.w3, sh) : h.w2;
+        const int idx = h0 == kMagicPRPC ? 1 : h0 == kMagicSTRM ? 2 : 0;
+        const uint32_t body = __byte_perm(h1, 0, 0x0123), meta = __byte_perm(h2, 0, 0x0123);
+        // (a preferred nshead handler is asked first and may claim these bytes: pf == 12 goes the generic way)
+        if (idx && ((mask >> idx) & 1u) && pf != 12 && (uint64_t)body <= max_body && (uint64_t)(len - pos) >= 12ull + body && meta <= body) {
+            s.err = B2_PARSE_OK; s.index = idx; s.pf = idx; s.frame_pos = pos; s.new_pos = pos + 12 + body; s.body = body; s.meta = meta; s.popped = false;
+            fast = true;
+        }
+    }
+    if (!fast) s = cut_input_message(run, len, pos, pf, max_body, client, mask);
+    return s;
+}
 template <typename Emit>
 __device__ __forceinline__ void walk_tile_spec(const uint8_t* run, uint32_t len, uint32_t entry, uint32_t tile_end,
                                                uint64_t max_body, bool client, TileRec& t, Emit emit, uint32_t mask) {
-    uint32_t pos = entry, count = 0, prev_len = 0, pre_pos = kNone;
+    uint32_t pos = entry, count = 0;
     int pf = -1, last = 0;
     uint8_t kind = kRanOff;
-    HdrWords pre; pre.w0 = pre.w1 = pre.w2 = pre.w3 = 0;
+    SpecAhead a; a.pre.w0 = a.pre.w1 = a.pre.w2 = a.pre.w3 = 0; a.pre_pos = kNone; a.prev_len = 0;
     while (pos < tile_end) {
-        Step s;
-        bool fast = false;
-        if (len - pos >= 12) {
-            const HdrWords h = pre_pos == pos ? pre : load_hdr_words(run + pos);
-            const uint32_t guess = pos + prev_len;
-            // (guess <= len - 12, written so that a guess past the run's end — the last tile's end lies beyond it — cannot wrap around)
-            if (prev_len && guess < tile_end && (uint64_t)guess + 12 <= len) { pre = load_hdr_words(run + guess); pre_pos = guess; }   // in flight while h is used
-            else pre_pos = kNone;
-            const uint32_t sh = 8u * (pos & 3u);                      // run offsets are 16-byte aligned: alignment of run + pos is pos & 3
-            const uint32_t h0 = sh ? __funnelshift_r(h.w0, h.w1, sh) : h.w0, h1 = sh ? __funnelshift_r(h.w1, h.w2, sh) : h.w1,
-                           h2 = sh ? __funnelshift_r(h.w2, h.w3, sh) : h.w2;
-            const int idx = h0 == kMagicPRPC ? 1 : h0 == kMagicSTRM ? 2 : 0;
-            const uint32_t body = __byte_perm(h1, 0, 0x0123), meta = __byte_perm(h2, 0, 0x0123);
-            // (a preferred nshead handler is asked first and may claim these bytes: pf == 12 goes the generic way)
-            if (idx && ((mask >> idx) & 1u) && pf != 12 && (uint64_t)body <= max_body && (uint64_t)(len - pos) >= 12ull + body && meta <= body) {
-                s.err = B2_PARSE_OK; s.index = idx; s.pf = idx; s.frame_pos = pos; s.new_pos = pos + 12 + body; s.body = body; s.meta = meta; s.popped = false;
-                fast = true;
-            }
-        }
-        if (!fast) s = cut_input_message(run, len, pos, pf, max_body, client, mask);
+        const Step s = spec_step(run, len, pos, pf, tile_end, max_body, client, mask, a);
         if (count == 0 && (s.popped || (s.index != 12 && nshead_claims(run, len, pos, max_body, mask)))) { kind = kAmbig; break; }
         if (s.err != B2_PARSE_OK) { kind = kStop; break; }
         emit(count, s);
-        count++; last = s.index; pf = s.index; prev_len = s.new_pos - pos; pos = s.new_pos;
+        count++; last = s.index; pf = s.index; a.prev_len = s.new_pos - pos; pos = s.new_pos;
     }
     t.entry = entry; t.exit = pos; t.count = count; t.kind = kind; t.last_proto = (int8_t)last;
 }
 
-// --- k_tile_walk: one thread per tile ---------------------------------------
-__global__ void __launch_bounds__(128) k_tile_walk(BatchPtrs B, DevConfig C) {
+// The group walk of k_tile_walk (B.walk_group > 1): one thread walks the chain from the group head's speculative entry to the end of
+// the group's last tile (a group never crosses a run; a run's last group may be short).  Each member's record and offsets are what
+// walk_tile_spec writes for the member when entered where the chain crosses into it: the member's first step is taken with an unknown
+// preferred index, and a handler that popped bytes there, or an nshead handler that would claim them, makes the member kAmbig and ends
+// the walk — so k_resolve's exactness argument holds for every member, whichever route the true chain takes into it.  Members the
+// chain steps over, and members after the walk ended, get no entry (k_resolve re-walks them if the true chain arrives there).
+__device__ __forceinline__ void walk_group_spec(const BatchPtrs& B, const DevConfig& C, uint32_t g) {
+    const uint32_t t0 = __ldg(B.group_heads + g);
+    const uint4 ti = __ldg(B.tile_info + t0);
+    const uint32_t k0 = ti.z, len = ti.y, flags = ti.w >> 24;
+    const uint8_t* run = B.bytes + ti.x;
+    const bool client = (flags & B2_RUN_CLIENT) != 0;
+    const uint32_t mask = run_mask(C.proto_mask, flags);
+    const uint32_t run_tiles = (uint32_t)(((uint64_t)len + C.tile_bytes - 1) >> C.tile_shift);
+    const uint32_t gn = min(B.walk_group, run_tiles - k0), group_end = (k0 + gn) << C.tile_shift;
+    uint32_t pos = B.head_recs[g].entry;          // kNone once the walk has ended
+    SpecAhead a; a.pre.w0 = a.pre.w1 = a.pre.w2 = a.pre.w3 = 0; a.pre_pos = kNone; a.prev_len = 0;
+    for (uint32_t m = 0; m < gn; m++) {
+        TileRec rec;
+        rec.entry = kNone; rec.exit = 0; rec.count = 0; rec.kind = kStop; rec.last_proto = 0; rec.live = 0; rec.pf_in = -1;
+        const uint32_t tile_end = (k0 + m + 1) << C.tile_shift;
+        if (pos < tile_end) {
+            uint32_t* spec = B.tile_spec + (size_t)(t0 + m) * C.spec_k;
+            uint32_t count = 0;
+            int pf = -1, last = 0;
+            uint8_t kind = kRanOff;
+            rec.entry = pos;
+            while (pos < tile_end) {
+                const Step s = spec_step(run, len, pos, pf, group_end, C.max_body_size, client, mask, a);
+                if (count == 0 && (s.popped || (s.index != 12 && nshead_claims(run, len, pos, C.max_body_size, mask)))) { kind = kAmbig; break; }
+                if (s.err != B2_PARSE_OK) { kind = kStop; break; }
+                if (count < C.spec_k) spec[count] = (ti.x + s.frame_pos) | ((uint32_t)(s.index != 1) << 31);
+                count++; last = s.index; pf = s.index; a.prev_len = s.new_pos - pos; pos = s.new_pos;
+            }
+            rec.exit = pos; rec.count = count; rec.kind = kind; rec.last_proto = (int8_t)last;
+            if (kind != kRanOff) pos = kNone;
+        }
+        B.tiles[t0 + m] = rec;
+    }
+}
+
+// --- k_tile_walk: one thread per tile, or per group of B.walk_group tiles -----------------------------
+// (a grouped launch runs in kWalkGroupThreads-thread blocks: a bench batch's ~8k walkers then spread over every SM beside k_fused)
+// (12 blocks per SM: 40 registers, so that a block starts beside the other batch's k_fused, b2_resident_plan)
+constexpr uint32_t kWalkGroupThreads = 64;
+__global__ void __launch_bounds__(128, 12) k_tile_walk(BatchPtrs B, DevConfig C) {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (B.walk_group > 1) {
+        if (t < B.n_groups) walk_group_spec(B, C, t);
+        return;
+    }
     if (t >= B.n_tiles) return;
     const uint4 ti = __ldg(B.tile_info + t);
     const uint32_t k = ti.z;

@@ -377,6 +377,15 @@ int  b2_elapsed_ms(b2_ctx* a, b2_ctx* b, float* ms);
  * decode+pack kernel served the batch (0 = the slot-scan pipeline). */
 int  b2_batch_info(b2_ctx* ctx, uint32_t out[4]);
 
+/* Walk groups of the front stages (DESIGN §3): k_tile_search finds a speculative entry only in the first tile of each group of
+ * consecutive tiles of a connection, and one thread of k_tile_walk walks the frame chain across the whole group.  mode 0 (default) =
+ * auto: 2 tiles per group on the fused path once the frame size is known and frames are not small enough to take the dense shape, 1
+ * elsewhere; 1 = one tile per group (every tile searched); 2..8 = that many tiles per group on every path but B2_INPUT_PULL.  Results
+ * do not depend on it.  Takes effect at the next upload (an uploaded batch has to be uploaded again).  b2_walk_group returns the
+ * group size the last launch used. */
+int  b2_set_walk_group(b2_ctx* ctx, uint32_t mode);
+int  b2_walk_group(b2_ctx* ctx);
+
 /* Residency of a fused pass.  Two contexts on two streams overlap their passes: one batch's front stages (k_tile_search, k_tile_walk,
  * k_resolve) and slow-reply kernel (k_pack_slow<true>) run on the SMs the other batch's k_fused holds, which they can only do where one
  * of their blocks fits in what a k_fused CTA leaves of the SM.  Entry 0 is k_fused in the shape the uploaded batch uses, then those four

@@ -4,7 +4,9 @@ Writes every kernel's start, end, stream, grid and block as JSON under --out, an
   - the step time: from the end of one k_fused to the end of the next (a step is one pass; the two streams take turns),
   - the exposed time: the part of the step in which no k_fused runs on the device,
   - the kernels that run in those gaps,
-and the card's name, power limit and SM clock, read in the same run.  A run of its own: tracing slows the host, so its step times are
+then per k_fused its duration and how much of it each kind of kernel of the other stream overlapped (the search, the walk,
+k_resolve / k_pack_slow, anything else, the other k_fused, nothing), and every other kernel's mean duration beside another stream's
+k_fused and away from it, and the card's name, power limit and SM clock, read in the same run.  A run of its own: tracing slows the host, so its step times are
 not bench.py's.
 python tools/pass_timeline.py [--steps 30] [--warmup 5] [--payload 1024] [--out DIR (default: a new temporary directory)]"""
 import argparse
@@ -115,7 +117,7 @@ def main():
         inside = sorted({k["name"] + "@s%s" % k["stream"] for k in ks if k["name"] != "k_fused" and any(k["start_us"] < g1 and k["end_us"] > g0 for g0, g1 in gaps)})
         steps.append({"step": i, "step_us": b - a, "exposed_us": sum(g1 - g0 for g0, g1 in gaps), "gap_kernels": inside})
     info = {"card": card(), "payload": args.payload, "n_msgs": int(n_full), "kernels": ks, "steps": steps, "plan": plans,
-            "fused_shapes": sorted({(str(k["stream"]), str(k["block"])) for k in fused})}
+            "fused_shapes": sorted({(str(k["stream"]), str(k["block"])) for k in fused}), "fused_beside": fused_beside(ks, fused)}
     json.dump(info, open(os.path.join(args.out, "timeline.json"), "w"), indent=1)
     print("trace and timeline in", args.out)
     print("card (name, power limit, SM clock, max SM clock):", info["card"])
@@ -129,6 +131,50 @@ def main():
         st = statistics.mean(s["step_us"] for s in body); ex = statistics.mean(s["exposed_us"] for s in body)
         fz = statistics.mean(k["end_us"] - k["start_us"] for k in fused)
         print("mean step %.1f us, mean exposed %.1f us (%.0f %%), mean k_fused %.1f us" % (st, ex, 100.0 * ex / st, fz))
+    beside = info["fused_beside"]
+    print("k_fused and what the other stream runs beside it (us; a stretch where two of them run counts for the first named):")
+    for b in beside:
+        print("  k_fused %6.1f us @s%s  " % (b["dur_us"], b["stream"]) + "  ".join("%s %5.1f" % (c, b[c]) for c in CATS + ("nothing",)))
+    body = beside[2:-2] if len(beside) > 8 else beside         # (the first and last passes have no other stream beside them)
+    if body:
+        print("mean over %d k_fused: %.1f us; " % (len(body), statistics.mean(b["dur_us"] for b in body))
+              + ", ".join("%s %.1f" % (c, statistics.mean(b[c] for b in body)) for c in CATS + ("nothing",)))
+    for name in sorted({k["name"] for k in ks if k["name"] != "k_fused"}):
+        with_f, alone = [], []
+        for k in ks:
+            if k["name"] != name:
+                continue
+            d = k["end_us"] - k["start_us"]
+            ov = sum(max(0.0, min(k["end_us"], f["end_us"]) - max(k["start_us"], f["start_us"])) for f in fused if f["stream"] != k["stream"])
+            (with_f if d > 0 and ov >= 0.5 * d else alone).append(d)
+        print("  %-22s mean %6.1f us beside another stream's k_fused (%d), %6.1f us otherwise (%d)"
+              % (name, statistics.mean(with_f) if with_f else float("nan"), len(with_f), statistics.mean(alone) if alone else float("nan"), len(alone)))
+
+
+CATS = ("k_tile_search", "k_tile_walk", "k_resolve/k_pack_slow", "other", "k_fused")
+
+
+def category(name):
+    if name in ("k_tile_search", "k_tile_walk", "k_fused"):
+        return name
+    return CATS[2] if name == "k_resolve" or name.startswith("k_pack_slow") else CATS[3]
+
+
+def fused_beside(ks, fused):
+    """For every k_fused: its duration and how much of it each kind of kernel of the other stream(s) overlapped."""
+    out = []
+    for f in fused:
+        a, b = f["start_us"], f["end_us"]
+        others = [(max(a, k["start_us"]), min(b, k["end_us"]), category(k["name"])) for k in ks
+                  if k["stream"] != f["stream"] and k["start_us"] < b and k["end_us"] > a]
+        cuts = sorted({a, b} | {x for o in others for x in o[:2]})
+        row = {"stream": f["stream"], "start_us": a, "dur_us": b - a, "nothing": 0.0}
+        row.update({c: 0.0 for c in CATS})
+        for x, y in zip(cuts, cuts[1:]):
+            on = {o[2] for o in others if o[0] < y and o[1] > x}
+            row[next((c for c in CATS if c in on), "nothing")] += y - x
+        out.append(row)
+    return out
 
 
 if __name__ == "__main__":
