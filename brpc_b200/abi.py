@@ -108,6 +108,14 @@ class H2ClientRingResult(C.Structure):
 assert C.sizeof(H2ClientRingResult) == 64
 
 
+class ClientRingResult(C.Structure):
+    _fields_ = [("batch", BatchResult), ("n_reqs", C.c_uint32), ("reserved", C.c_uint32), ("req_offs", C.c_void_p), ("req_lens", C.c_void_p),
+                ("req_out", C.c_void_p)]
+
+
+assert C.sizeof(ClientRingResult) == 104
+
+
 class StreamState(C.Structure):
     _fields_ = [("local_consumed", C.c_uint64), ("remote_consumed", C.c_uint64), ("pending_bytes", C.c_uint32), ("flags", C.c_uint32),
                 ("error_code", C.c_int32), ("reserved", C.c_uint32)]
@@ -208,6 +216,9 @@ def _load():
     l.b2_h2_client_ring_enable.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]
     l.b2_h2_client_ring_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
     l.b2_h2_client_ring_wait.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(H2ClientRingResult)]
+    l.b2_client_ring_enable.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]
+    l.b2_client_ring_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
+    l.b2_client_ring_wait.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(ClientRingResult)]
     l.b2_h2_pack_responses.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     l.b2_pack_requests.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     l.b2_pack_responses.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
@@ -236,7 +247,8 @@ ABI_SYMBOLS = ["b2_ctx_create", "b2_ctx_destroy", "b2_last_error", "b2_version",
                "b2_h2_client_conn_reset", "b2_h2_client_process_batch", "b2_h2_client_abandon_streams", "b2_h2_conn_set_gunzip",
                "b2_h2_serve_batch", "b2_stream_configure", "b2_stream_open", "b2_stream_set_connected", "b2_stream_close", "b2_stream_query",
                "b2_stream_take_pending", "b2_stream_results", "b2_stream_write", "b2_stream_ring_enable", "b2_h2_ring_enable", "b2_h2_ring_submit",
-               "b2_h2_ring_wait", "b2_h2_client_ring_enable", "b2_h2_client_ring_submit", "b2_h2_client_ring_wait"]
+               "b2_h2_ring_wait", "b2_h2_client_ring_enable", "b2_h2_client_ring_submit", "b2_h2_client_ring_wait", "b2_client_ring_enable",
+               "b2_client_ring_submit", "b2_client_ring_wait"]
 
 ECHO_METHOD = dict(service_full_name=b"example.EchoService", service_name=b"EchoService", method_name=b"Echo",
                    request_type_name=b"example.EchoRequest", handler=1, echo_attachment=1,
@@ -796,6 +808,32 @@ class Context:
         frames = _view(res.req_out, end)
         return (_view(res.runs, 32 * res.n_runs, H2_RUN_STATUS_DT), _view(res.calls, 64 * res.n_calls, H2_CALL_DT), _view(res.out, res.region * res.n_runs),
                 reqs, [frames[int(r["out_off"]):int(r["out_off"]) + int(r["out_len"])].tobytes() for r in reqs])
+
+    # ---- baidu_std client connections on the latency path (b2_client_ring_*) ----
+    def client_ring_enable(self, max_bytes, max_reqs, req_out_cap):
+        """Serve client turns on the resident k_ring<true> with these per-ticket caps (b2_client_ring_enable): before the first ring call."""
+        _check(lib.b2_client_ring_enable(self._h, max_bytes, max_reqs, req_out_cap))
+
+    def client_ring_submit(self, data, runs, reqs, ptr=None, nbytes=None):
+        """One turn of a client's event loop: runs (RUN_DT, the bytes read from client sockets) are served as by ring_submit, then reqs
+        (REQUEST_DT, offsets into the same data) are packed as by pack_requests.  Either list may be empty, not both.  Returns the ticket."""
+        runs = np.ascontiguousarray(runs, dtype=RUN_DT); reqs = np.ascontiguousarray(reqs, dtype=REQUEST_DT)
+        ptr, nbytes = self._ring_bytes(data, ptr, nbytes)
+        t = C.c_uint32(0)
+        _check(lib.b2_client_ring_submit(self._h, ptr, nbytes, runs.ctypes.data if len(runs) else None, len(runs),
+                                         reqs.ctypes.data if len(reqs) else None, len(reqs), C.byref(t)))
+        return t.value
+
+    def client_ring_wait(self, ticket):
+        """ring_wait's (run_status, msgs, resp, info) of the ticket's runs, then the frame of every request (b"" where it could not be
+        packed, as pack_requests returns them).  The first three are views of the ticket's pinned slot, valid until the 8th later
+        submission; the frames are copies."""
+        res = ClientRingResult()
+        _check(lib.b2_client_ring_wait(self._h, ticket, C.byref(res)))
+        rs, msgs, resp = self._views(res.batch)
+        offs, lens = _view(res.req_offs, 4 * res.n_reqs, np.uint32), _view(res.req_lens, 4 * res.n_reqs, np.uint32)
+        frames = [C.string_at(res.req_out + int(o), int(n)) if n else b"" for o, n in zip(offs, lens)]
+        return rs, msgs, resp, self._info(res.batch), frames
 
     def pack_requests(self, data, reqs, out_cap=None):
         """reqs: REQUEST_DT array (offsets into data).  Returns the packed frame of every request (b"" = rejected)."""

@@ -46,8 +46,9 @@ constexpr uint32_t kSecEvents = 64, kSecMsgs = kSecEvents + kSmallMsgs * 80, kSe
                    kSecRunCtrl = kSecCtrl + 3 * kStreamCtrlMax * kSmallMsgs, kSecOut = kSecRunCtrl + kSmallRuns * 8;
 struct Stage { const char* name; cudaEvent_t ev; };
 // Which resident kernel a context's ring runs, fixed by its first ring call: k_ring (b2_ring_start / b2_ring_submit), k_ring with the
-// stream pass (b2_stream_ring_enable), k_h2_ring (b2_h2_ring_enable) or k_h2_client_ring (b2_h2_client_ring_enable)
-enum class RingKind { none, batch, batch_streams, h2_server, h2_client };
+// stream pass (b2_stream_ring_enable), k_ring<true> with the request phase (b2_client_ring_enable), k_h2_ring (b2_h2_ring_enable) or
+// k_h2_client_ring (b2_h2_client_ring_enable)
+enum class RingKind { none, batch, batch_streams, batch_client, h2_server, h2_client };
 // A slot's layout: the header (RingSlotHdr, then the kind's per-ticket args) in the first 256 bytes, then each part 256-byte aligned
 struct SlotLayout {
     uint64_t end = 256;
@@ -70,7 +71,7 @@ struct b2_ctx {
     std::vector<uint8_t> h2_gunzip; uint8_t* d_h2_gz_merge = nullptr;     // host mirror of the kH2Gunzip bits; merge scratch, B2_H2_HEADER_BYTES per run
     // persistent latency kernel (b2_ring_*): pinned + mapped submit ring, its own stream.  ring_slots: allocated (by the first ring call
     // that needs them); the slot parts of each kind live in that kind's kernel arguments (ring_dev: runs, staged input, output, stream section)
-    RingKind ring_kind = RingKind::none; RingDev ring_dev = {}; H2RingDev h2r_dev = {}; H2ClientRingDev h2c_dev = {};
+    RingKind ring_kind = RingKind::none; RingDev ring_dev = {}; ClientRingDev cr_dev = {}; H2RingDev h2r_dev = {}; H2ClientRingDev h2c_dev = {};
     uint8_t* ring_slots = nullptr; volatile uint32_t* ring_ctl = nullptr; uint32_t* d_ring_ticket = nullptr; cudaStream_t ring_stream = nullptr;
     uint32_t ring_next = 1, ring_stride = 0; bool ring_collected[8] = { true, true, true, true, true, true, true, true };
     const void* ring_bytes[8] = {}; const void* ring_pin_base = nullptr; unsigned long long ring_pin_dev = 0; uint64_t ring_launches = 0;
@@ -81,6 +82,7 @@ struct b2_ctx {
     // the caps every ticket of an h2 ring (k_h2_ring, k_h2_client_ring) is served with
     uint32_t h2r_max_bytes = 0, h2r_msg_cap = 0, h2r_out_cap = 0, h2r_replies_cap = 0;
     uint32_t h2c_max_bytes = 0, h2c_call_cap = 0, h2c_out_cap = 0, h2c_max_reqs = 0, h2c_req_out_cap = 0;
+    uint32_t cr_max_bytes = 0, cr_max_reqs = 0, cr_req_out_cap = 0;        // ... and of the client ring (k_ring<true>)
     ulonglong2* d_iov = nullptr; b2_iovec* h_iov = nullptr; const void* host_bytes = nullptr;      // B2_RESP_IOVEC
     uint4* d_refs = nullptr; b2_resp_ref* h_refs = nullptr; int input_mode = B2_INPUT_COPY, resp_mode = B2_RESP_COPY; const uint8_t* pull_bytes = nullptr;
     uint32_t* d_crc_adv = nullptr; unsigned long long* d_counters = nullptr; uint32_t* d_totals = nullptr; DevMethod* d_methods = nullptr;
@@ -196,14 +198,20 @@ static void ring_halt(b2_ctx* c);
 static void stream_free(b2_ctx* c);
 static bool ring_busy(const b2_ctx* c) { for (uint32_t k = 0; k < kRingSlots; k++) if (!c->ring_collected[k]) return true; return false; }
 static uint8_t* ring_slot(const b2_ctx* c, uint32_t ticket) { return c->ring_slots + (size_t)(ticket % kRingSlots) * c->ring_stride; }
-// Every call that uploads to the context or touches h2 state is refused while a ticket of an h2 ring (k_h2_ring or k_h2_client_ring) is
-// outstanding: the ticket uses the same device scratch and connection state.  A call that writes h2 connection state also retires the
-// resident kernel first: the resident CTA reads that state through L1, and a launch boundary is where L1 is known not to hold lines
-// another kernel wrote since.
-static bool h2_ring_refuses(b2_ctx* c, bool writes_h2_state) {
-    if (c->ring_kind != RingKind::h2_server && c->ring_kind != RingKind::h2_client) return false;
-    if (ring_busy(c)) { set_err(c->ring_kind == RingKind::h2_server ? "an h2 ring ticket is outstanding: b2_h2_ring_wait it first" : "an h2 client ring ticket is outstanding: b2_h2_client_ring_wait it first"); return true; }
-    if (writes_h2_state) ring_halt(c);
+// Every call that uploads to the context or touches h2 state is refused while a ticket of an h2 ring (k_h2_ring or k_h2_client_ring) or
+// of the client ring (k_ring<true>) is outstanding: the ticket uses the same device scratch and connection state.  A call that writes h2
+// connection state also retires an h2 ring's resident kernel first: that CTA reads the state through L1, and a launch boundary is where
+// L1 is known not to hold lines another kernel wrote since.
+static bool ring_refuses(b2_ctx* c, bool writes_h2_state) {
+    const RingKind k = c->ring_kind;
+    if (k != RingKind::h2_server && k != RingKind::h2_client && k != RingKind::batch_client) return false;
+    if (ring_busy(c)) {
+        set_err(k == RingKind::h2_server ? "an h2 ring ticket is outstanding: b2_h2_ring_wait it first" :
+                k == RingKind::h2_client ? "an h2 client ring ticket is outstanding: b2_h2_client_ring_wait it first" :
+                                           "a client ring ticket is outstanding: b2_client_ring_wait it first");
+        return true;
+    }
+    if (writes_h2_state && k != RingKind::batch_client) ring_halt(c);
     return false;
 }
 extern "C" void b2_ctx_destroy(b2_ctx* c) {
@@ -350,7 +358,7 @@ extern "C" int b2_ctx_create(const b2_options* o, b2_ctx** out) {
 
 extern "C" int b2_set_server_identity(b2_ctx* c, const char* ip_port) {
     if (!c) return B2_E_INVAL;
-    if (h2_ring_refuses(c, true)) return B2_E_INVAL;              // (the identity is a launch argument of k_h2_ring)
+    if (ring_refuses(c, true)) return B2_E_INVAL;              // (the identity is a launch argument of k_h2_ring)
     const size_t n = ip_port ? strlen(ip_port) : 0;
     if (n >= sizeof c->cfg.identity) { set_err("identity too long"); return B2_E_INVAL; }
     memset(c->cfg.identity, 0, sizeof c->cfg.identity);
@@ -462,7 +470,7 @@ static uint32_t pick_walk_group(const b2_ctx* c) {
 
 extern "C" int b2_batch_upload(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs) {
     if (!c || (!bytes && nbytes) || (!runs && n_runs)) { set_err("null argument"); return B2_E_INVAL; }
-    if (h2_ring_refuses(c, false)) return B2_E_INVAL;
+    if (ring_refuses(c, false)) return B2_E_INVAL;
     // (B2_INPUT_PULL: `bytes` is the caller's whole pinned arena and nothing is copied — what is bounded is the bytes the runs cover)
     if ((c->input_mode != B2_INPUT_PULL && nbytes > c->opt.max_batch_bytes) || nbytes >= (1u << 31) || n_runs > c->opt.max_runs) { set_err("batch exceeds ctx capacity"); return B2_E_CAPACITY; }
     uint64_t covered = 0; for (uint32_t r = 0; r < n_runs; r++) covered += runs[r].length;
@@ -1069,7 +1077,7 @@ extern "C" int b2_stream_write(b2_ctx* c, const void* bytes, uint32_t nbytes, co
     static_assert(sizeof(b2_stream_write_desc) == 24 && sizeof(b2_stream_write_result) == 32 && sizeof(SwRec) == 24, "stream write ABI layout");
     if (!c || !c->has_streams || (!bytes && nbytes) || (!writes && n) || (!results && n) || (!out && out_cap)) { set_err("no stream table (b2_stream_configure) or null argument"); return B2_E_INVAL; }
     if (c->stream_armed) { set_err("a submitted batch must be collected first: the stream table belongs to it"); return B2_E_INVAL; }
-    if (ring_owns_table(c) || h2_ring_refuses(c, false)) return B2_E_INVAL;
+    if (ring_owns_table(c) || ring_refuses(c, false)) return B2_E_INVAL;
     if (n > c->opt.max_msgs || nbytes > c->opt.max_batch_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     CU(cudaSetDevice(c->opt.device));
     const uint64_t seg = max_segment_size ? max_segment_size : 512ull << 20;       // -stream_write_max_segment_size (stream.cpp:39)
@@ -1189,13 +1197,19 @@ static int ring_launch(b2_ctx* c) {
     switch (c->ring_kind) {
     case RingKind::h2_server: { const H2RingDev H = h2_ring_dev(c); k_h2_ring<<<1, kSmallThreads, kH2RingSmem, c->ring_stream>>>(R, H); break; }
     case RingKind::h2_client: { const H2ClientRingDev H = h2_client_ring_dev(c); k_h2_client_ring<<<1, kSmallThreads, kH2ClientRingSmem, c->ring_stream>>>(R, H); break; }
-    default: {                              // batch, batch_streams
+    default: {                              // batch, batch_streams, batch_client
         const bool was_small = c->small; c->small = false;
         BatchPtrs B = make_ptrs(c);
         c->small = was_small;
         B.bytes = c->d_bytes;
         const StreamPass SP = c->ring_kind == RingKind::batch_streams ? c->sp_ring : StreamPass{};   // (tab null: the ring runs no stream pass)
-        k_ring<<<1, kSmallThreads, sizeof(SmallSmem), c->ring_stream>>>(R, B, c->cfg, SP);
+        if (c->ring_kind == RingKind::batch_client) {
+            // the scratch of b2_pack_requests, except that the requests and their offsets go to d_msgs / d_refs, which k_ring leaves alone
+            ClientRingDev Q = c->cr_dev;
+            Q.reqs = reinterpret_cast<ReqDesc*>(c->d_msgs); Q.offs = reinterpret_cast<uint32_t*>(c->d_refs); Q.lens = Q.offs + c->opt.max_msgs;
+            Q.scratch = c->d_unz; Q.out = c->d_resp;
+            k_ring<true><<<1, kSmallThreads, sizeof(SmallSmem), c->ring_stream>>>(R, B, c->cfg, SP, Q);
+        } else k_ring<false><<<1, kSmallThreads, sizeof(SmallSmem), c->ring_stream>>>(R, B, c->cfg, SP, ClientRingDev{});
     }
     }
     c->ring_launches++;
@@ -1228,7 +1242,7 @@ extern "C" int b2_ring_start(b2_ctx* c) {
         R.off_out = L.add(kSmallBlock);
         if (c->ring_kind == RingKind::batch_streams) R.off_st = L.add(kSecOut + ((c->sp_ring.out_cap + 15u) & ~15u));
         int rc = ring_alloc(c, L.end); if (rc != B2_OK) return rc;
-        CU(cudaFuncSetAttribute(k_ring, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmallSmem)));
+        CU(cudaFuncSetAttribute(k_ring<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmallSmem)));
     }
     if (!c->ring_ctl[1]) return ring_launch(c);
     return B2_OK;
@@ -1261,6 +1275,11 @@ static RingSlotHdr* ring_fill(b2_ctx* c, uint8_t* slot, const void* bytes, uint3
     if (n_runs) memcpy(slot + c->ring_dev.off_runs, runs, sizeof(b2_run) * (size_t)n_runs);
     h->n_runs = n_runs; h->nbytes = nbytes;
     return h;
+}
+// k_ring's compact output block of the ticket (small_layout), in its header
+static void ring_compact(const b2_ctx* c, RingSlotHdr* h, const SmallLayout& L) {
+    h->small_msgs = L.msgs; h->small_resp = L.resp; h->off_rs = L.off_rs; h->off_msgs = L.off_msgs;
+    h->off_refs = L.off_refs; h->off_resp = L.off_resp; h->total = L.total; h->by_ref = c->cfg.by_ref;
 }
 // marks the next ticket outstanding, rings its doorbell (everything else the host stores in the slot first) and relaunches the kernel if it
 // idled out
@@ -1306,6 +1325,7 @@ static uint8_t* ring_collect(b2_ctx* c, bool args_ok, uint32_t ticket, const cha
     if (in_order) c->ring_next_wait = ticket + 1;
     return slot;
 }
+static int ring_batch_result(b2_ctx* c, uint32_t ticket, uint8_t* slot, b2_batch_result* out);
 extern "C" int b2_ring_stop(b2_ctx* c) { if (!c) return B2_E_INVAL; cudaSetDevice(c->opt.device); ring_halt(c); return B2_OK; }
 
 extern "C" int b2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs, uint32_t* ticket) {
@@ -1313,6 +1333,7 @@ extern "C" int b2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, con
     if (c->has_streams && c->ring_kind != RingKind::batch_streams) { set_err("the ring path runs the stream pass only after b2_stream_ring_enable: use b2_batch_submit on a context with a stream table"); return B2_E_INVAL; }
     if (c->ring_kind == RingKind::h2_server) { set_err("this context's ring serves h2 (b2_h2_ring_enable): use b2_h2_ring_submit"); return B2_E_INVAL; }
     if (c->ring_kind == RingKind::h2_client) { set_err("this context's ring serves h2 client connections (b2_h2_client_ring_enable): use b2_h2_client_ring_submit"); return B2_E_INVAL; }
+    if (c->ring_kind == RingKind::batch_client) { set_err("this context's ring serves client turns (b2_client_ring_enable): use b2_client_ring_submit"); return B2_E_INVAL; }
     if (nbytes > kSmallBytes || n_runs > kSmallRuns) { set_err("b2_ring_submit serves batches up to 128 KiB / 512 runs: use b2_batch_submit"); return B2_E_CAPACITY; }
     if (!c->ring_slots) { int rc = b2_ring_start(c); if (rc != B2_OK) return rc; }
     uint8_t* slot = ring_claim(c, "b2_ring_wait");
@@ -1320,18 +1341,22 @@ extern "C" int b2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, con
     for (uint32_t r = 0; r < n_runs; r++)
         if ((runs[r].offset & 15u) || (uint64_t)runs[r].offset + runs[r].length > nbytes) { set_err("run offset must be 16-aligned and inside the batch"); return B2_E_INVAL; }
     RingSlotHdr* h = ring_fill(c, slot, bytes, nbytes, runs, n_runs);
-    const SmallLayout L = small_layout(nbytes, n_runs, c->opt.max_msgs);
-    h->small_msgs = L.msgs; h->small_resp = L.resp; h->off_rs = L.off_rs; h->off_msgs = L.off_msgs;
-    h->off_refs = L.off_refs; h->off_resp = L.off_resp; h->total = L.total; h->by_ref = c->cfg.by_ref;
+    ring_compact(c, h, small_layout(nbytes, n_runs, c->opt.max_msgs));
     return ring_ring(c, h, bytes, ticket);
 }
 
 extern "C" int b2_ring_wait(b2_ctx* c, uint32_t ticket, b2_batch_result* out) {
     if (c && c->ring_kind == RingKind::h2_server) { set_err("this context's ring serves h2: use b2_h2_ring_wait"); return B2_E_INVAL; }
     if (c && c->ring_kind == RingKind::h2_client) { set_err("this context's ring serves h2 client connections: use b2_h2_client_ring_wait"); return B2_E_INVAL; }
+    if (c && c->ring_kind == RingKind::batch_client) { set_err("this context's ring serves client turns: use b2_client_ring_wait"); return B2_E_INVAL; }
     int rc;
     uint8_t* slot = ring_collect(c, c && out, ticket, "bad ring ticket", rc);
     if (!slot) return rc;
+    return ring_batch_result(c, ticket, slot, out);
+}
+// The runs' result of a collected k_ring ticket, from its compact block, or from the big pipeline when the runs overflowed it
+static int ring_batch_result(b2_ctx* c, uint32_t ticket, uint8_t* slot, b2_batch_result* out) {
+    int rc;
     const uint32_t si = ticket % kRingSlots;
     const bool streams = c->ring_kind == RingKind::batch_streams;
     RingSlotHdr* h = reinterpret_cast<RingSlotHdr*>(slot);
@@ -1504,7 +1529,7 @@ static bool out_place(uint64_t& total, uint64_t need, uint32_t out_cap, uint32_t
 extern "C" int b2_crc32c_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const uint32_t* offs, const uint32_t* lens,
                                uint32_t n, uint32_t* out) {
     if (!c || !bytes || !offs || !lens || !out) { set_err("null argument"); return B2_E_INVAL; }
-    if (h2_ring_refuses(c, false)) return B2_E_INVAL;
+    if (ring_refuses(c, false)) return B2_E_INVAL;
     if (nbytes > c->opt.max_batch_bytes || n > c->opt.max_msgs) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     for (uint32_t i = 0; i < n; i++) if ((uint64_t)offs[i] + lens[i] > nbytes) { set_err("slice outside buffer"); return B2_E_INVAL; }
     CU(cudaSetDevice(c->opt.device));
@@ -1533,7 +1558,7 @@ __global__ void k_snappy_batch(const uint8_t* bytes, const uint32_t* offs, const
 extern "C" int b2_snappy_uncompress_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const uint32_t* offs, const uint32_t* lens,
                                           uint32_t n, void* out, uint32_t out_cap, uint32_t* out_offs, int32_t* out_lens) {
     if (!c || !bytes || !offs || !lens || !out || !out_offs || !out_lens) { set_err("null argument"); return B2_E_INVAL; }
-    if (h2_ring_refuses(c, false)) return B2_E_INVAL;
+    if (ring_refuses(c, false)) return B2_E_INVAL;
     if (nbytes > c->opt.max_batch_bytes || n > c->opt.max_msgs || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     // output layout from the announced lengths (the preamble varint), nothing else is read on the host
     std::vector<uint32_t> caps(n);
@@ -1576,7 +1601,7 @@ __global__ void __launch_bounds__(256) k_snappy_compress_batch(const uint8_t* by
 extern "C" int b2_snappy_compress_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const uint32_t* offs, const uint32_t* lens,
                                         uint32_t n, void* out, uint32_t out_cap, uint32_t* out_offs, uint32_t* out_lens) {
     if (!c || !bytes || !offs || !lens || !out || !out_offs || !out_lens) { set_err("null argument"); return B2_E_INVAL; }
-    if (h2_ring_refuses(c, false)) return B2_E_INVAL;
+    if (ring_refuses(c, false)) return B2_E_INVAL;
     if (nbytes > c->opt.max_batch_bytes || n > c->opt.max_msgs || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     uint64_t total = 0;
     for (uint32_t i = 0; i < n; i++) {
@@ -1667,7 +1692,7 @@ extern "C" int b2_snappy_raw_uncompress(const char* compressed, size_t compresse
 
 extern "C" int b2_hpack_reset(b2_ctx* c, uint32_t conn, uint32_t max_table_size) {
     if (!c || conn >= B2_HPACK_MAX_CONNS || max_table_size > 4096) { set_err("bad connection / table size"); return B2_E_INVAL; }
-    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
+    if (ring_refuses(c, true)) return B2_E_INVAL;
     CU(cudaSetDevice(c->opt.device));
     k_hpack_reset<<<1, 1, 0, c->stream>>>(c->d_hpack, conn, max_table_size);
     CU(cudaStreamSynchronize(c->stream));
@@ -1684,7 +1709,7 @@ template <class Conn> static bool conn_groups(uint32_t n, Conn conn, std::vector
 extern "C" int b2_hpack_decode_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_hpack_block* blocks, uint32_t n,
                                      void* out, uint32_t per_block_cap, uint32_t* out_lens, int32_t* status, uint32_t* n_headers) {
     if (!c || !bytes || !blocks || !out || !out_lens || !status || !n_headers) { set_err("null argument"); return B2_E_INVAL; }
-    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
+    if (ring_refuses(c, true)) return B2_E_INVAL;
     if (nbytes > c->opt.max_batch_bytes || n > c->opt.max_msgs / 4 || (uint64_t)n * per_block_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     std::vector<uint32_t> conn(n), off(n), len(n), first;
     for (uint32_t i = 0; i < n; i++) {
@@ -1714,7 +1739,7 @@ extern "C" int b2_hpack_decode_batch(b2_ctx* c, const void* bytes, uint32_t nbyt
 extern "C" int b2_h2_scan_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs, uint32_t max_frame_size,
                                 b2_h2_frame* frames, uint32_t cap_per_run, uint32_t* n_frames, uint32_t* consumed, uint32_t* err) {
     if (!c || !bytes || !runs || !frames || !n_frames || !consumed || !err) { set_err("null argument"); return B2_E_INVAL; }
-    if (h2_ring_refuses(c, false)) return B2_E_INVAL;
+    if (ring_refuses(c, false)) return B2_E_INVAL;
     if (nbytes > c->opt.max_batch_bytes || n_runs > c->opt.max_runs || (uint64_t)n_runs * cap_per_run * sizeof(b2_h2_frame) > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     for (uint32_t r = 0; r < n_runs; r++) if ((uint64_t)runs[r].offset + runs[r].length > nbytes) { set_err("run outside buffer"); return B2_E_INVAL; }
     CU(cudaSetDevice(c->opt.device));
@@ -1760,7 +1785,7 @@ extern "C" int b2_h2_configure(b2_ctx* c, uint32_t max_conns, uint32_t max_pendi
 }
 extern "C" int b2_h2_conn_reset(b2_ctx* c, uint32_t conn) {
     if (!c || conn >= c->h2_max_conns) { set_err("bad connection index"); return B2_E_INVAL; }
-    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
+    if (ring_refuses(c, true)) return B2_E_INVAL;
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     k_h2_conn_reset<<<1, 1, 0, c->stream>>>(c->d_h2, c->d_hpack, conn, h2_pool(c));
     CU(cudaStreamSynchronize(c->stream));
@@ -1769,7 +1794,7 @@ extern "C" int b2_h2_conn_reset(b2_ctx* c, uint32_t conn) {
 }
 extern "C" int b2_h2_conn_set_gunzip(b2_ctx* c, uint32_t conn, int enable) {
     if (!c || conn >= c->h2_max_conns) { set_err("bad connection index"); return B2_E_INVAL; }
-    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
+    if (ring_refuses(c, true)) return B2_E_INVAL;
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     CU(cudaSetDevice(c->opt.device));
     if (enable && !c->d_h2_gz_merge) {                            // once per context: the merge scratch of the select pass
@@ -1848,7 +1873,7 @@ static int h2_parse_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, const b
     static_assert(sizeof(M) == 64 && sizeof(b2_h2_run_status) == 32, "h2 ABI layout");
     if (nbytes > c->opt.max_batch_bytes || n_runs > c->opt.max_runs || out_cap > 2ull * c->opt.max_resp_bytes || cap > c->opt.max_msgs ||
         (serve && serve->replies_cap > c->opt.max_resp_bytes)) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
-    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
+    if (ring_refuses(c, true)) return B2_E_INVAL;
     *n_descs = 0;
     if (n_runs == 0) return B2_OK;
     if (!h2_runs_ok(c, runs, n_runs, nbytes)) return B2_E_INVAL;
@@ -1915,7 +1940,7 @@ extern "C" int b2_h2_serve_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, 
 extern "C" int b2_h2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_h2_response* resps, uint32_t n,
                                     void* out, uint32_t out_cap, uint32_t* out_offs, uint32_t* out_lens) {
     if (!c || (!bytes && nbytes) || !resps || !out || !out_offs || !out_lens) { set_err("null argument"); return B2_E_INVAL; }
-    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
+    if (ring_refuses(c, true)) return B2_E_INVAL;
     static_assert(sizeof(b2_h2_response) == 48, "h2 response ABI layout");
     if (nbytes > c->opt.max_resp_bytes || n > c->opt.max_msgs || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     if (n == 0) return B2_OK;
@@ -1982,7 +2007,7 @@ static int h2_place_requests(const b2_ctx* c, const void* bytes, uint32_t nbytes
 extern "C" int b2_h2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_h2_request* reqs, uint32_t n,
                                    void* out, uint32_t out_cap, b2_h2_request_result* results) {
     if (!c || !bytes || !reqs || !out || !results) { set_err("null argument"); return B2_E_INVAL; }
-    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
+    if (ring_refuses(c, true)) return B2_E_INVAL;
     static_assert(sizeof(b2_h2_request) == 48 && sizeof(b2_h2_request_result) == 16, "h2 request ABI layout");
     if (nbytes > c->opt.max_resp_bytes || n > c->opt.max_msgs || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     if (n == 0) return B2_OK;
@@ -2013,7 +2038,7 @@ extern "C" int b2_h2_conn_peer_update(b2_ctx* c, uint32_t conn, const b2_h2_peer
     static_assert(sizeof(b2_h2_peer_update) == 24, "peer update ABI layout");
     if ((u->set & B2_H2_PEER_MAX_FRAME_SIZE) && (u->max_frame_size < 16384u || u->max_frame_size > 16777215u)) { set_err("max_frame_size out of range"); return B2_E_INVAL; }   // ParseH2Settings :166-211
     if ((u->set & B2_H2_PEER_STREAM_WINDOW) && u->stream_window_size > 0x7fffffffu) { set_err("stream_window_size out of range"); return B2_E_INVAL; }
-    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
+    if (ring_refuses(c, true)) return B2_E_INVAL;
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     if (conn >= c->h2_max_conns) { set_err("conn out of range"); return B2_E_INVAL; }
     CU(cudaSetDevice(c->opt.device));
@@ -2026,7 +2051,7 @@ extern "C" int b2_h2_conn_peer_update(b2_ctx* c, uint32_t conn, const b2_h2_peer
 }
 extern "C" int b2_h2_conn_set_next_stream_id(b2_ctx* c, uint32_t conn, uint32_t next_id) {
     if (!c) { set_err("null argument"); return B2_E_INVAL; }
-    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
+    if (ring_refuses(c, true)) return B2_E_INVAL;
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     if (conn >= c->h2_max_conns) { set_err("conn out of range"); return B2_E_INVAL; }
     CU(cudaSetDevice(c->opt.device));
@@ -2038,7 +2063,7 @@ extern "C" int b2_h2_conn_set_next_stream_id(b2_ctx* c, uint32_t conn, uint32_t 
 // the receiving half of a client connection: see include/b2rpc.h
 extern "C" int b2_h2_client_conn_reset(b2_ctx* c, uint32_t conn) {
     if (!c || conn >= c->h2_max_conns) { set_err("bad connection index"); return B2_E_INVAL; }
-    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
+    if (ring_refuses(c, true)) return B2_E_INVAL;
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     CU(cudaSetDevice(c->opt.device));
     k_h2_client_conn_reset<<<1, 1, 0, c->stream>>>(c->d_h2, c->d_hpack, conn, h2_pool(c));
@@ -2048,7 +2073,7 @@ extern "C" int b2_h2_client_conn_reset(b2_ctx* c, uint32_t conn) {
 }
 extern "C" int b2_h2_client_abandon_streams(b2_ctx* c, uint32_t conn, const uint32_t* stream_ids, uint32_t n) {
     if (!c || (!stream_ids && n)) { set_err("null argument"); return B2_E_INVAL; }
-    if (h2_ring_refuses(c, true)) return B2_E_INVAL;
+    if (ring_refuses(c, true)) return B2_E_INVAL;
     if (conn >= c->h2_max_conns) { set_err("bad connection index"); return B2_E_INVAL; }
     if ((uint64_t)n * 4 > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }   // (the ids go to unz_upper)
     if (n == 0) return B2_OK;
@@ -2066,14 +2091,8 @@ extern "C" int b2_h2_client_process_batch(b2_ctx* c, const void* bytes, uint32_t
     return h2_parse_batch(c, bytes, nbytes, runs, n_runs, rs, calls, call_cap, n_calls, out, out_cap);
 }
 
-extern "C" int b2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_request* reqs, uint32_t n,
-                                void* out, uint32_t out_cap, uint32_t* out_offs, uint32_t* out_lens) {
-    if (!c || (!bytes && nbytes) || !reqs || !out || !out_offs || !out_lens) { set_err("null argument"); return B2_E_INVAL; }
-    if (h2_ring_refuses(c, false)) return B2_E_INVAL;
-    static_assert(sizeof(b2_request) == 64 && sizeof(ReqDesc) == 64, "request ABI layout");
-    if (nbytes > c->opt.max_batch_bytes || n > c->opt.max_msgs || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
-    if (n == 0) return B2_OK;
-    uint64_t total = 0;
+// the frame of every request, placed with out_place at its worst-case size (b2_pack_requests, b2_client_ring_submit); total: the bytes placed
+static int place_requests(uint32_t nbytes, const b2_request* reqs, uint32_t n, uint32_t out_cap, uint32_t* out_offs, uint64_t& total) {
     for (uint32_t i = 0; i < n; i++) {
         const b2_request& r = reqs[i];
         if ((uint64_t)r.payload_off + r.payload_len > nbytes || (uint64_t)r.attachment_off + r.attachment_len > nbytes) { set_err("payload outside buffer"); return B2_E_INVAL; }
@@ -2081,6 +2100,18 @@ extern "C" int b2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes, c
         const uint64_t need = 12 + 512 + (r.compress_type == B2_COMPRESS_TYPE_SNAPPY ? snappy_max_compressed_length((uint32_t)pb) : pb) + r.attachment_len;
         if (!out_place(total, need, out_cap, &out_offs[i])) { set_err("out_cap too small"); return B2_E_CAPACITY; }
     }
+    return B2_OK;
+}
+extern "C" int b2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_request* reqs, uint32_t n,
+                                void* out, uint32_t out_cap, uint32_t* out_offs, uint32_t* out_lens) {
+    if (!c || (!bytes && nbytes) || !reqs || !out || !out_offs || !out_lens) { set_err("null argument"); return B2_E_INVAL; }
+    if (ring_refuses(c, false)) return B2_E_INVAL;
+    static_assert(sizeof(b2_request) == 64 && sizeof(ReqDesc) == 64, "request ABI layout");
+    if (nbytes > c->opt.max_batch_bytes || n > c->opt.max_msgs || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    if (n == 0) return B2_OK;
+    uint64_t total = 0;
+    const int rc = place_requests(nbytes, reqs, n, out_cap, out_offs, total);
+    if (rc != B2_OK) return rc;
     CU(cudaSetDevice(c->opt.device));
     ReqDesc* d_reqs = reinterpret_cast<ReqDesc*>(c->d_msgs);
     uint32_t* d_offs = c->d_frame_off; uint32_t* d_lens = c->d_slot;
@@ -2099,7 +2130,7 @@ extern "C" int b2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes, c
 extern "C" int b2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_reply* reps, uint32_t n,
                                  void* out, uint32_t out_cap, uint32_t* out_offs, uint32_t* out_lens) {
     if (!c || (!bytes && nbytes) || !reps || !out || !out_offs || !out_lens) { set_err("null argument"); return B2_E_INVAL; }
-    if (h2_ring_refuses(c, false)) return B2_E_INVAL;
+    if (ring_refuses(c, false)) return B2_E_INVAL;
     static_assert(sizeof(b2_reply) == 88 && sizeof(ReplyDesc) == 88, "reply ABI layout");
     if (nbytes > c->opt.max_batch_bytes || (uint64_t)n * sizeof(b2_reply) > (uint64_t)c->opt.max_msgs * 64 || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     if (n == 0) return B2_OK;
@@ -2304,4 +2335,72 @@ extern "C" int b2_h2_client_ring_wait(b2_ctx* c, uint32_t ticket, b2_h2_client_r
     out->reqs = reinterpret_cast<const b2_h2_request_result*>(slot + L.off_req_res);
     out->req_out = slot + L.off_req_out;
     return B2_OK;
+}
+
+// ---- a baidu_std client's turn on the latency path: k_ring<true> on the same submit ring (include/b2rpc.h, b2_client_ring_enable) ----
+extern "C" int b2_client_ring_enable(b2_ctx* c, uint32_t max_bytes, uint32_t max_reqs, uint32_t req_out_cap) {
+    if (!c) { set_err("null argument"); return B2_E_INVAL; }
+    if (c->ring_kind != RingKind::none) { set_err("b2_client_ring_enable: once, before the context's first ring call, and not with another ring kind"); return B2_E_INVAL; }
+    if (c->has_streams) { set_err("b2_client_ring_enable: the client ring runs no stream pass, so not on a context with a stream table"); return B2_E_INVAL; }
+    if (max_bytes == 0 || max_reqs == 0 || req_out_cap == 0) { set_err("capacities must be non-zero"); return B2_E_INVAL; }
+    // the limits of b2_process_batch and b2_pack_requests, both of which read the ticket's bytes
+    if (max_bytes > c->opt.max_batch_bytes || max_reqs > c->opt.max_msgs || req_out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    CU(cudaSetDevice(c->opt.device));
+    static_assert(sizeof(RingSlotHdr) + sizeof(ClientRingArgs) <= 256, "client ring slot header");
+    // [RingSlotHdr | args | runs | staged input | requests + placed offsets | compact block | frame lengths | frames]
+    SlotLayout L;
+    ClientRingDev& Q = c->cr_dev;
+    Q.off_args = sizeof(RingSlotHdr);
+    c->ring_dev.off_runs = L.add(kSmallRuns * sizeof(b2_run));
+    c->ring_dev.off_in = L.add((uint64_t)max_bytes + 16);
+    Q.off_reqs = L.add((uint64_t)max_reqs * (sizeof(b2_request) + 4));
+    c->ring_dev.off_out = L.add(kSmallBlock);
+    Q.off_req_lens = L.add((uint64_t)max_reqs * 4);
+    Q.off_req_out = L.add((uint64_t)req_out_cap + 16);
+    int rc = ring_alloc(c, L.end); if (rc != B2_OK) return rc;
+    CU(cudaFuncSetAttribute(k_ring<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmallSmem)));
+    c->cr_max_bytes = max_bytes; c->cr_max_reqs = max_reqs; c->cr_req_out_cap = req_out_cap;
+    c->ring_kind = RingKind::batch_client;
+    return B2_OK;
+}
+extern "C" int b2_client_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
+                                     const b2_request* reqs, uint32_t n_reqs, uint32_t* ticket) {
+    if (!c || !bytes || !ticket || (!runs && n_runs) || (!reqs && n_reqs)) { set_err("null argument"); return B2_E_INVAL; }
+    if (n_runs == 0 && n_reqs == 0) { set_err("a ticket carries runs, requests or both"); return B2_E_INVAL; }
+    if (c->ring_kind != RingKind::batch_client) { set_err("b2_client_ring_enable first"); return B2_E_INVAL; }
+    // the argument checks of b2_ring_submit and b2_pack_requests with the caps of b2_client_ring_enable
+    if (nbytes > c->cr_max_bytes) { set_err("ticket larger than b2_client_ring_enable's max_bytes: use the batch calls"); return B2_E_CAPACITY; }
+    if (n_runs > kSmallRuns || n_runs > c->opt.max_runs) { set_err("b2_client_ring_submit serves up to 512 runs: use the batch calls"); return B2_E_CAPACITY; }
+    if (n_reqs > c->cr_max_reqs) { set_err("more requests than b2_client_ring_enable's max_reqs"); return B2_E_CAPACITY; }
+    uint8_t* slot = ring_claim(c, "b2_client_ring_wait");
+    if (!slot) return B2_E_CAPACITY;
+    uint32_t extent = 0;                                         // (the compact block is sized for the bytes the runs cover)
+    for (uint32_t r = 0; r < n_runs; r++) {
+        if ((runs[r].offset & 15u) || (uint64_t)runs[r].offset + runs[r].length > nbytes) { set_err("run offset must be 16-aligned and inside the batch"); return B2_E_INVAL; }
+        extent = std::max(extent, runs[r].offset + runs[r].length);
+    }
+    uint8_t* block = slot + c->cr_dev.off_reqs;                  // the request block the kernel pulls: requests, then their placed offsets
+    uint64_t total = 0;
+    int rc = place_requests(nbytes, reqs, n_reqs, c->cr_req_out_cap, reinterpret_cast<uint32_t*>(block + sizeof(b2_request) * (size_t)n_reqs), total);
+    if (rc != B2_OK) return rc;
+    if (n_reqs) memcpy(block, reqs, sizeof(b2_request) * (size_t)n_reqs);
+    const ClientRingArgs a = { n_reqs, { 0, 0, 0 } };
+    RingSlotHdr* h = ring_fill(c, slot, bytes, nbytes, runs, n_runs);
+    ring_compact(c, h, small_layout(std::min(extent, kSmallBytes), n_runs, c->opt.max_msgs));
+    memcpy(slot + c->cr_dev.off_args, &a, sizeof a);
+    return ring_ring(c, h, bytes, ticket);
+}
+extern "C" int b2_client_ring_wait(b2_ctx* c, uint32_t ticket, b2_client_ring_result* out) {
+    static_assert(sizeof(b2_client_ring_result) == 104, "client ring result ABI layout");
+    int rc;
+    uint8_t* slot = ring_collect(c, c && out && c->ring_kind == RingKind::batch_client, ticket, "bad client ring ticket", rc);
+    if (!slot) return rc;
+    memset(out, 0, sizeof *out);
+    const ClientRingDev& L = c->cr_dev;
+    const uint32_t n = reinterpret_cast<const ClientRingArgs*>(slot + L.off_args)->n_reqs;
+    out->n_reqs = n;
+    out->req_offs = reinterpret_cast<const uint32_t*>(slot + L.off_reqs + sizeof(b2_request) * (size_t)n);
+    out->req_lens = reinterpret_cast<const uint32_t*>(slot + L.off_req_lens);
+    out->req_out = slot + L.off_req_out;
+    return ring_batch_result(c, ticket, slot, &out->batch);      // (an overflowing ticket's runs go through the big pipeline here)
 }

@@ -473,6 +473,42 @@ typedef struct b2_request {
 } b2_request;                        /* 64 bytes */
 int  b2_pack_requests(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2_request* reqs, uint32_t n,
                       void* out, uint32_t out_cap, uint32_t* out_offs, uint32_t* out_lens);
+/* baidu_std CLIENT connections on the latency path: b2_process_batch followed by b2_pack_requests inside the resident k_ring
+ * (k_ring<true>) fed through the same submit ring.  A ticket is one turn of a client's event loop: read what arrived, then send what is
+ * queued.  The runs (the bytes read from client sockets, B2_RUN_CLIENT) are served as by b2_ring_submit, then the requests are packed as
+ * by b2_pack_requests; their fields index the same `bytes` as the runs.  A baidu_std client keeps no connection state on the device
+ * (correlation ids live on the host), so a ticket's requests do not depend on its runs: they are packed even when the runs overflow the
+ * compact block.  Runs are served whatever their flags: server runs in a client ticket are answered as b2_ring_submit answers them.
+ * For each socket hand its reads over first, then write its request frames in request order.
+ * A context runs one ring kind: b2_ring_submit / _wait, b2_stream_ring_enable and the b2_h2_*ring* calls refuse a context that runs this
+ * one, and b2_client_ring_* refuse a context of another kind.
+ * b2_client_ring_enable: once, before the context's first ring call, and not on a context with a stream table (else B2_E_INVAL; the
+ * ticket runs no stream pass).  max_bytes bounds a ticket's whole `bytes` (the runs' bytes plus the request payloads, <= max_batch_bytes,
+ * so a turn may exceed b2_ring_submit's 128 KiB); max_reqs (<= max_msgs) and req_out_cap (<= max_resp_bytes) play the roles of
+ * b2_pack_requests' n and out_cap.  Caps above those limits fail with B2_E_CAPACITY; they fix the slot layout.
+ * b2_ring_stop, b2_ring_launches, b2_ring_phase_ns ([2]: runs served and requests packed) and B2_RING_IDLE_MS apply as to k_ring.
+ * b2_client_ring_submit: n_runs or n_reqs may be 0, not both.  Every check of b2_ring_submit (<= 512 runs, 16-aligned runs inside
+ * `bytes`) and of b2_pack_requests (payloads inside `bytes`, every frame placed at its worst-case size within req_out_cap) applies with
+ * the enable-time caps; a failed check claims no slot and leaves the next ticket number unchanged.  The runs keep the compact block's
+ * limits (1024 messages, its reply bytes), sized from the extent the runs cover.  Bytes in b2_block_alloc memory are pulled in place,
+ * others staged into the slot.
+ * b2_client_ring_wait: tickets may be waited in any order.  For every ticket `batch` equals b2_process_batch(bytes, runs) on a context
+ * with the same settings, and the request offsets, lengths and frame bytes equal b2_pack_requests(bytes, reqs, req_out_cap) — for any
+ * sequence of tickets, byte for byte.  A ticket whose runs overflow the compact block has them served through the big pipeline inside the
+ * wait, as b2_ring_wait does (every other ticket collected first); its frames still come from the kernel.  B2_RESP_BY_REF / B2_RESP_IOVEC
+ * behave as in b2_ring_wait.  While a ticket is outstanding every call that uploads to the context (b2_process_batch, b2_batch_*,
+ * b2_pack_requests, b2_pack_responses, the crc32c / snappy / hpack / h2 calls, b2_stream_write) fails with B2_E_INVAL. */
+typedef struct b2_client_ring_result {   /* views into the ticket's pinned slot, valid until the 8th later submission */
+    b2_batch_result batch;               /* the runs, exactly as b2_ring_wait returns them */
+    uint32_t n_reqs, reserved;
+    const uint32_t* req_offs;            /* as b2_pack_requests' out_offs */
+    const uint32_t* req_lens;            /* as its out_lens: 0 = could not be packed */
+    const uint8_t*  req_out;             /* request i's frame at req_out + req_offs[i] */
+} b2_client_ring_result;                 /* 104 bytes */
+int  b2_client_ring_enable(b2_ctx* ctx, uint32_t max_bytes, uint32_t max_reqs, uint32_t req_out_cap);
+int  b2_client_ring_submit(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
+                           const b2_request* reqs, uint32_t n_reqs, uint32_t* ticket);
+int  b2_client_ring_wait(b2_ctx* ctx, uint32_t ticket, b2_client_ring_result* out);
 
 /* ---- replies the HOST produced (B2_HANDLER_HOST methods, any service above the transport): SendRpcResponse
  * (src/brpc/policy/baidu_rpc_protocol.cpp:273-460) as a batch, one warp per reply.  `bytes` holds what the host has: the response
