@@ -116,6 +116,13 @@ class ClientRingResult(C.Structure):
 assert C.sizeof(ClientRingResult) == 104
 
 
+class StreamRingResult(C.Structure):
+    _fields_ = [("batch", BatchResult), ("n_writes", C.c_uint32), ("out_bytes", C.c_uint32), ("results", C.c_void_p), ("out", C.c_void_p)]
+
+
+assert C.sizeof(StreamRingResult) == 96
+
+
 class StreamState(C.Structure):
     _fields_ = [("local_consumed", C.c_uint64), ("remote_consumed", C.c_uint64), ("pending_bytes", C.c_uint32), ("flags", C.c_uint32),
                 ("error_code", C.c_int32), ("reserved", C.c_uint32)]
@@ -231,6 +238,9 @@ def _load():
     l.b2_stream_results.argtypes = [C.c_void_p, C.POINTER(StreamBatchResult)]
     l.b2_stream_ring_enable.argtypes = [C.c_void_p, C.c_uint32]
     l.b2_stream_write.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p]
+    l.b2_stream_ring_write_enable.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]
+    l.b2_stream_ring_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
+    l.b2_stream_ring_wait.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(StreamRingResult)]
     l.b2_counters_read.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
     l.b2_counters_device_ptr.restype = C.c_void_p; l.b2_counters_device_ptr.argtypes = [C.c_void_p]
     return l
@@ -248,7 +258,7 @@ ABI_SYMBOLS = ["b2_ctx_create", "b2_ctx_destroy", "b2_last_error", "b2_version",
                "b2_h2_serve_batch", "b2_stream_configure", "b2_stream_open", "b2_stream_set_connected", "b2_stream_close", "b2_stream_query",
                "b2_stream_take_pending", "b2_stream_results", "b2_stream_write", "b2_stream_ring_enable", "b2_h2_ring_enable", "b2_h2_ring_submit",
                "b2_h2_ring_wait", "b2_h2_client_ring_enable", "b2_h2_client_ring_submit", "b2_h2_client_ring_wait", "b2_client_ring_enable",
-               "b2_client_ring_submit", "b2_client_ring_wait"]
+               "b2_client_ring_submit", "b2_client_ring_wait", "b2_stream_ring_write_enable", "b2_stream_ring_submit", "b2_stream_ring_wait"]
 
 ECHO_METHOD = dict(service_full_name=b"example.EchoService", service_name=b"EchoService", method_name=b"Echo",
                    request_type_name=b"example.EchoRequest", handler=1, echo_attachment=1,
@@ -538,16 +548,21 @@ class Context:
         return (_view(r.msgs, 32 * r.n_msgs, STREAM_MSG_DT), _view(r.events, 80 * r.n_events, STREAM_EVENT_DT), _view(r.out, r.out_bytes, np.uint8),
                 _view(r.ctrl, r.ctrl_bytes, np.uint8), _view(r.run_ctrl, 8 * r.n_runs, np.uint32).reshape(-1, 2))
 
-    def stream_write(self, writes, data=None, max_segment_size=0, out_cap=None, out=None):
-        """StreamWrite for a batch of writes (b2_stream_write).  writes: STREAM_WRITE_DT array or a list of (stream_id, flags, src_off,
-        src_len); data: the bytes host-sourced writes index.  Returns (results, out): write i's frames are
-        out[results[i]["out_off"]:results[i]["out_off"] + results[i]["out_len"]]."""
+    @staticmethod
+    def _write_list(writes):
+        """STREAM_WRITE_DT array of writes given as such an array or as a list of (stream_id, flags, src_off, src_len)"""
         if not isinstance(writes, np.ndarray):
             a = np.zeros(len(writes), STREAM_WRITE_DT)
             for i, t in enumerate(writes):
                 a[i] = tuple(t) + (0,) * (5 - len(t))
             writes = a
-        writes = np.ascontiguousarray(writes, dtype=STREAM_WRITE_DT)
+        return np.ascontiguousarray(writes, dtype=STREAM_WRITE_DT)
+
+    def stream_write(self, writes, data=None, max_segment_size=0, out_cap=None, out=None):
+        """StreamWrite for a batch of writes (b2_stream_write).  writes: STREAM_WRITE_DT array or a list of (stream_id, flags, src_off,
+        src_len); data: the bytes host-sourced writes index.  Returns (results, out): write i's frames are
+        out[results[i]["out_off"]:results[i]["out_off"] + results[i]["out_len"]]."""
+        writes = self._write_list(writes)
         n = len(writes)
         if data is None:
             ptr, nb = None, 0
@@ -811,7 +826,7 @@ class Context:
 
     # ---- baidu_std client connections on the latency path (b2_client_ring_*) ----
     def client_ring_enable(self, max_bytes, max_reqs, req_out_cap):
-        """Serve client turns on the resident k_ring<true> with these per-ticket caps (b2_client_ring_enable): before the first ring call."""
+        """Serve client turns on the resident k_ring<RingBody::requests> with these per-ticket caps (b2_client_ring_enable): before the first ring call."""
         _check(lib.b2_client_ring_enable(self._h, max_bytes, max_reqs, req_out_cap))
 
     def client_ring_submit(self, data, runs, reqs, ptr=None, nbytes=None):
@@ -834,6 +849,36 @@ class Context:
         offs, lens = _view(res.req_offs, 4 * res.n_reqs, np.uint32), _view(res.req_lens, 4 * res.n_reqs, np.uint32)
         frames = [C.string_at(res.req_out + int(o), int(n)) if n else b"" for o, n in zip(offs, lens)]
         return rs, msgs, resp, self._info(res.batch), frames
+
+    # ---- a Stream producer's turn on the latency path (b2_stream_ring_*) ----
+    def stream_ring_write_enable(self, max_bytes, max_writes, write_out_cap, max_segment_size=0):
+        """Serve producer turns on the resident k_ring with these per-ticket caps (b2_stream_ring_write_enable): after stream_ring_enable,
+        before the first ring call."""
+        _check(lib.b2_stream_ring_write_enable(self._h, max_bytes, max_writes, write_out_cap, max_segment_size))
+
+    def stream_ring_submit(self, data, runs, writes, ptr=None, nbytes=None):
+        """One producer turn: runs (RUN_DT) are served as by ring_submit on a stream ring, then writes (as for stream_write, offsets into
+        the same data) are applied as by stream_write.  Either list may be empty, not both.  Returns the ticket; the context keeps data
+        referenced until the ticket's slot is reused."""
+        runs = np.ascontiguousarray(runs, dtype=RUN_DT); writes = self._write_list(writes)
+        own = ptr is None
+        ptr, nbytes = self._ring_bytes(data, ptr, nbytes)
+        t = C.c_uint32(0)
+        _check(lib.b2_stream_ring_submit(self._h, ptr, nbytes, runs.ctypes.data if len(runs) else None, len(runs),
+                                         writes.ctypes.data if len(writes) else None, len(writes), C.byref(t)))
+        keep = self.__dict__.setdefault("_stream_ring_keep", [None] * 8)
+        keep[t.value % 8] = self._ring_keep if own else None      # (an overflowing ticket's wait reads its bytes again)
+        return t.value
+
+    def stream_ring_wait(self, ticket):
+        """ring_wait's (run_status, msgs, resp, info) of the ticket's runs, then the write results (STREAM_WRITE_RESULT_DT) and the frames
+        (write i's at out[out_off:out_off + out_len], the zero gaps included): views of the ticket's pinned slot, valid until the 8th later
+        submission."""
+        res = StreamRingResult()
+        _check(lib.b2_stream_ring_wait(self._h, ticket, C.byref(res)))
+        rs, msgs, resp = self._views(res.batch)
+        return (rs, msgs, resp, self._info(res.batch), _view(res.results, 32 * res.n_writes, STREAM_WRITE_RESULT_DT),
+                _view(res.out, res.out_bytes))
 
     def pack_requests(self, data, reqs, out_cap=None):
         """reqs: REQUEST_DT array (offsets into data).  Returns the packed frame of every request (b"" = rejected)."""

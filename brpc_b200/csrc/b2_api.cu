@@ -46,9 +46,13 @@ constexpr uint32_t kSecEvents = 64, kSecMsgs = kSecEvents + kSmallMsgs * 80, kSe
                    kSecRunCtrl = kSecCtrl + 3 * kStreamCtrlMax * kSmallMsgs, kSecOut = kSecRunCtrl + kSmallRuns * 8;
 struct Stage { const char* name; cudaEvent_t ev; };
 // Which resident kernel a context's ring runs, fixed by its first ring call: k_ring (b2_ring_start / b2_ring_submit), k_ring with the
-// stream pass (b2_stream_ring_enable), k_ring<true> with the request phase (b2_client_ring_enable), k_h2_ring (b2_h2_ring_enable) or
-// k_h2_client_ring (b2_h2_client_ring_enable)
-enum class RingKind { none, batch, batch_streams, batch_client, h2_server, h2_client };
+// stream pass (b2_stream_ring_enable), k_ring<RingBody::stream_writes> with the stream pass and the write pass (b2_stream_ring_write_enable),
+// k_ring<RingBody::requests> with the request phase (b2_client_ring_enable), k_h2_ring (b2_h2_ring_enable) or k_h2_client_ring
+// (b2_h2_client_ring_enable)
+enum class RingKind { none, batch, batch_streams, batch_stream_writes, batch_client, h2_server, h2_client };
+// The kinds whose tickets run the stream pass: the table belongs to an outstanding ticket, tickets are collected in ticket order, the
+// kernel parks behind a ticket that overflows the compact block, and the slot carries a stream section
+bool ring_runs_streams(RingKind k) { return k == RingKind::batch_streams || k == RingKind::batch_stream_writes; }
 // A slot's layout: the header (RingSlotHdr, then the kind's per-ticket args) in the first 256 bytes, then each part 256-byte aligned
 struct SlotLayout {
     uint64_t end = 256;
@@ -82,7 +86,9 @@ struct b2_ctx {
     // the caps every ticket of an h2 ring (k_h2_ring, k_h2_client_ring) is served with
     uint32_t h2r_max_bytes = 0, h2r_msg_cap = 0, h2r_out_cap = 0, h2r_replies_cap = 0;
     uint32_t h2c_max_bytes = 0, h2c_call_cap = 0, h2c_out_cap = 0, h2c_max_reqs = 0, h2c_req_out_cap = 0;
-    uint32_t cr_max_bytes = 0, cr_max_reqs = 0, cr_req_out_cap = 0;        // ... and of the client ring (k_ring<true>)
+    uint32_t cr_max_bytes = 0, cr_max_reqs = 0, cr_req_out_cap = 0;        // ... and of the client ring (k_ring<RingBody::requests>)
+    // the stream write ring (k_ring<RingBody::stream_writes>): its caps, its slot parts and the write pass's device scratch (d_swr)
+    uint32_t swr_max_bytes = 0, swr_max_writes = 0, swr_out_cap = 0; SwRingDev swr_dev = {}; uint8_t* d_swr = nullptr;
     ulonglong2* d_iov = nullptr; b2_iovec* h_iov = nullptr; const void* host_bytes = nullptr;      // B2_RESP_IOVEC
     uint4* d_refs = nullptr; b2_resp_ref* h_refs = nullptr; int input_mode = B2_INPUT_COPY, resp_mode = B2_RESP_COPY; const uint8_t* pull_bytes = nullptr;
     uint32_t* d_crc_adv = nullptr; unsigned long long* d_counters = nullptr; uint32_t* d_totals = nullptr; DevMethod* d_methods = nullptr;
@@ -199,7 +205,7 @@ static void stream_free(b2_ctx* c);
 static bool ring_busy(const b2_ctx* c) { for (uint32_t k = 0; k < kRingSlots; k++) if (!c->ring_collected[k]) return true; return false; }
 static uint8_t* ring_slot(const b2_ctx* c, uint32_t ticket) { return c->ring_slots + (size_t)(ticket % kRingSlots) * c->ring_stride; }
 // Every call that uploads to the context or touches h2 state is refused while a ticket of an h2 ring (k_h2_ring or k_h2_client_ring) or
-// of the client ring (k_ring<true>) is outstanding: the ticket uses the same device scratch and connection state.  A call that writes h2
+// of the client ring (k_ring<RingBody::requests>) is outstanding: the ticket uses the same device scratch and connection state.  A call that writes h2
 // connection state also retires an h2 ring's resident kernel first: that CTA reads the state through L1, and a launch boundary is where
 // L1 is known not to hold lines another kernel wrote since.
 static bool ring_refuses(b2_ctx* c, bool writes_h2_state) {
@@ -569,7 +575,7 @@ static int launch_stream_pass(b2_ctx* c, const BatchPtrs& B, cudaStream_t s, uin
     k_stream_run<<<grid(c->st_max, 4, sms * 8), 128, 0, s>>>(B, S); CU(cudaEventRecord(c->st_ev[4], s));
     k_stream_rst<<<grid(c->n_runs, 4, sms * 4), 128, 0, s>>>(B, S); CU(cudaEventRecord(c->st_ev[5], s));
     CU(cudaMemcpyAsync(c->h_st_cnts, S.cnts, 64, cudaMemcpyDeviceToHost, s));
-    if (c->ring_kind == RingKind::batch_streams) CU(cudaMemsetAsync(S.cnt, 0, 8 * (size_t)S.cap, s));     // cnt | fill: zero when the ring's next ticket starts
+    if (ring_runs_streams(c->ring_kind)) CU(cudaMemsetAsync(S.cnt, 0, 8 * (size_t)S.cap, s));     // cnt | fill: zero when the ring's next ticket starts
     launches += 5; c->stream_ran = true; c->st_input = B.bytes;
     return B2_OK;
 }
@@ -877,7 +883,7 @@ static void stream_free(b2_ctx* c) {
     for (cudaEvent_t& e : c->st_ev) if (e) { cudaEventDestroy(e); e = nullptr; }
     for (int i = 0; i < 4; i++) { cudaFree(c->d_sw[i]); c->d_sw[i] = nullptr; c->sw_have[i] = 0; }
     cudaFreeHost(c->h_sw_recs); c->h_sw_recs = nullptr; c->h_sw_have = 0; cudaFreeHost(c->h_sw_cnts); c->h_sw_cnts = nullptr;
-    cudaFree(c->d_st_ring); c->d_st_ring = nullptr;
+    cudaFree(c->d_st_ring); c->d_st_ring = nullptr; cudaFree(c->d_swr); c->d_swr = nullptr;
     for (cudaEvent_t& e : c->sw_ev) if (e) { cudaEventDestroy(e); e = nullptr; }
     cudaGetLastError();
 }
@@ -931,7 +937,7 @@ static int stream_configure(b2_ctx* c, uint32_t max_streams, uint32_t pending_by
 
 // a ring ticket of a context whose ring runs the stream pass is submitted and not collected: the table belongs to k_ring
 static bool ring_owns_table(const b2_ctx* c) {
-    if (c->ring_kind != RingKind::batch_streams || !ring_busy(c)) return false;
+    if (!ring_runs_streams(c->ring_kind) || !ring_busy(c)) return false;
     set_err("a ring ticket is outstanding: b2_ring_wait it first, the stream table belongs to it");
     return true;
 }
@@ -1072,53 +1078,55 @@ static int sw_reserve(b2_ctx* c, int i, size_t need) {          // device stagin
     c->sw_have[i] = n;
     return B2_OK;
 }
-extern "C" int b2_stream_write(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_stream_write_desc* writes, uint32_t n,
-                               uint32_t max_segment_size, void* out, uint32_t out_cap, b2_stream_write_result* results) {
-    static_assert(sizeof(b2_stream_write_desc) == 24 && sizeof(b2_stream_write_result) == 32 && sizeof(SwRec) == 24, "stream write ABI layout");
-    if (!c || !c->has_streams || (!bytes && nbytes) || (!writes && n) || (!results && n) || (!out && out_cap)) { set_err("no stream table (b2_stream_configure) or null argument"); return B2_E_INVAL; }
-    if (c->stream_armed) { set_err("a submitted batch must be collected first: the stream table belongs to it"); return B2_E_INVAL; }
-    if (ring_owns_table(c) || ring_refuses(c, false)) return B2_E_INVAL;
-    if (n > c->opt.max_msgs || nbytes > c->opt.max_batch_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
-    CU(cudaSetDevice(c->opt.device));
-    const uint64_t seg = max_segment_size ? max_segment_size : 512ull << 20;       // -stream_write_max_segment_size (stream.cpp:39)
+// the pinned host records hold at least n writes
+static int sw_host_recs(b2_ctx* c, uint32_t n) {
+    if ((size_t)n * sizeof(SwRec) <= c->h_sw_have) return B2_OK;
+    cudaFreeHost(c->h_sw_recs); c->h_sw_recs = nullptr; c->h_sw_have = 0;
+    size_t m = 4096; while (m < (size_t)n * sizeof(SwRec)) m <<= 1;
+    if (cudaHostAlloc((void**)&c->h_sw_recs, m, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); set_err("cudaHostAlloc of the stream write records failed"); return B2_E_NOMEM; }
+    c->h_sw_have = m;
+    return B2_OK;
+}
+// Checks a write list and resolves it into recs[0, n) (b2_stream_write, b2_stream_ring_submit): a host-sourced payload at base + src_off
+// of the nbytes the call carries; with from_msg a FROM_MSG write at the message of the last collected batch or ring ticket, else the flag
+// is refused.  bound: the sum over writes of align16(len + ceil(len / seg) * 38), what the frames may take.  Nothing changes on failure.
+static int sw_resolve(b2_ctx* c, const b2_stream_write_desc* writes, uint32_t n, uint32_t nbytes, uint64_t seg, const uint8_t* base,
+                      bool from_msg, SwRec* recs, uint64_t& bound) {
     // FROM_MSG: the messages b2_stream_results describes — a ring ticket's only while it is the most recent one (the next ticket
     // overwrites the device input and the ring's out staging)
     const b2_stream_msg* from_msgs = c->h_st_msgs; const uint8_t* from_out = c->sp.out;
     uint32_t n_msgs = c->stream_valid && c->stream_ran ? c->h_st_cnts[0] : 0;
-    if (c->stream_valid && c->st_view_ticket) {
+    if (from_msg && c->stream_valid && c->st_view_ticket) {
         b2_stream_batch_result v; b2_stream_results(c, &v);
         from_msgs = v.msgs; from_out = c->sp_ring.out; n_msgs = c->st_view_ticket + 1 == c->ring_next ? v.n_msgs : 0;
     }
-    if ((size_t)n * sizeof(SwRec) > c->h_sw_have) {
-        cudaFreeHost(c->h_sw_recs); c->h_sw_recs = nullptr; c->h_sw_have = 0;
-        size_t m = 4096; while (m < (size_t)n * sizeof(SwRec)) m <<= 1;
-        if (cudaHostAlloc((void**)&c->h_sw_recs, m, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); set_err("cudaHostAlloc of the stream write records failed"); return B2_E_NOMEM; }
-        c->h_sw_have = m;
-    }
-    int rc = sw_reserve(c, 0, nbytes);
-    if (rc != B2_OK) return rc;
-    // every argument is checked before anything changes; each record carries its payload's device address
-    const uint8_t* d_in = static_cast<const uint8_t*>(c->d_sw[0]);
-    uint64_t bound = 0;
+    bound = 0;
     for (uint32_t i = 0; i < n; i++) {
         const b2_stream_write_desc& w = writes[i];
-        SwRec& r = c->h_sw_recs[i];
+        SwRec& r = recs[i];
         r.id = w.stream_id; r.pad = 0;
         if (w.flags & ~B2_STREAM_W_FROM_MSG) { set_err("unknown b2_stream_write flag"); return B2_E_INVAL; }
         if (w.flags & B2_STREAM_W_FROM_MSG) {
+            if (!from_msg) { set_err("B2_STREAM_W_FROM_MSG is refused in a ring ticket: the messages a ticket completes are not known when it is submitted (b2_stream_write between tickets)"); return B2_E_INVAL; }
             if (w.src_off >= n_msgs) { set_err("B2_STREAM_W_FROM_MSG: no such message in the last collected batch (or ring ticket, when it is the most recent)"); return B2_E_INVAL; }
             const b2_stream_msg& m = from_msgs[w.src_off];
             if ((m.flags & B2_STREAM_MSG_IN_INPUT) && !c->st_input) { set_err("B2_STREAM_W_FROM_MSG: a later call overwrote the last batch's input bytes on the device"); return B2_E_INVAL; }
             r.src = ((m.flags & B2_STREAM_MSG_IN_INPUT) ? c->st_input : from_out) + m.off; r.len = m.len;
         } else {
             if ((uint64_t)w.src_off + w.src_len > nbytes) { set_err("write outside bytes"); return B2_E_INVAL; }
-            r.src = d_in + w.src_off; r.len = w.src_len;
+            r.src = base + w.src_off; r.len = w.src_len;
         }
         const uint64_t nfr = r.len <= seg ? 1 : (r.len + seg - 1) / seg;
         bound += (r.len + nfr * kSwHeadMax + 15) & ~15ull;
     }
-    if (bound > out_cap || bound > c->opt.max_resp_bytes) { set_err("out_cap (or max_resp_bytes) below the sum of align16(len + ceil(len / seg) * 38)"); return B2_E_CAPACITY; }
-    if (n == 0) return B2_OK;
+    return B2_OK;
+}
+// The grid path over the n records in h_sw_recs, whose host-sourced payloads point into d_sw[0]: bytes staged there, the seven k_sw_*
+// kernels on the context's stream, the results and the used frame bytes copied to `results` / `out` (b2_stream_write, and the writes of
+// a stream ring ticket whose runs overflowed).  bound: what sw_resolve computed.  *out_bytes: the frame bytes copied.
+static int sw_launch(b2_ctx* c, const void* bytes, uint32_t nbytes, uint32_t n, uint64_t seg, uint64_t bound, b2_stream_write_result* results,
+                     void* out, uint32_t* out_bytes) {
+    int rc;
     const size_t cap = c->sp.cap;
     const size_t o_res = ((size_t)n * 24 + 15) & ~(size_t)15, o_slot = o_res + 32 * (size_t)n, o_group = o_slot + ((4 * (size_t)n + 15) & ~(size_t)15),
                  o_fb = o_group + 8 * (size_t)n, o_cb = o_fb + ((4 * (size_t)n + 15) & ~(size_t)15);
@@ -1153,11 +1161,32 @@ extern "C" int b2_stream_write(b2_ctx* c, const void* bytes, uint32_t nbytes, co
     CU(cudaMemcpyAsync(c->h_sw_cnts, P.cnts, 64, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     c->sw_ran = true;
+    *out_bytes = c->h_sw_cnts[2];
     if (c->h_sw_cnts[2]) {
         CU(cudaMemcpyAsync(out, P.out, c->h_sw_cnts[2], cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
     }
     return B2_OK;
+}
+extern "C" int b2_stream_write(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_stream_write_desc* writes, uint32_t n,
+                               uint32_t max_segment_size, void* out, uint32_t out_cap, b2_stream_write_result* results) {
+    static_assert(sizeof(b2_stream_write_desc) == 24 && sizeof(b2_stream_write_result) == 32 && sizeof(SwRec) == 24, "stream write ABI layout");
+    if (!c || !c->has_streams || (!bytes && nbytes) || (!writes && n) || (!results && n) || (!out && out_cap)) { set_err("no stream table (b2_stream_configure) or null argument"); return B2_E_INVAL; }
+    if (c->stream_armed) { set_err("a submitted batch must be collected first: the stream table belongs to it"); return B2_E_INVAL; }
+    if (ring_owns_table(c) || ring_refuses(c, false)) return B2_E_INVAL;
+    if (n > c->opt.max_msgs || nbytes > c->opt.max_batch_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    CU(cudaSetDevice(c->opt.device));
+    const uint64_t seg = max_segment_size ? max_segment_size : 512ull << 20;       // -stream_write_max_segment_size (stream.cpp:39)
+    int rc = sw_host_recs(c, n);
+    if (rc == B2_OK) rc = sw_reserve(c, 0, nbytes);
+    if (rc != B2_OK) return rc;
+    // every argument is checked before anything changes; each record carries its payload's device address
+    uint64_t bound = 0;
+    if ((rc = sw_resolve(c, writes, n, nbytes, seg, static_cast<const uint8_t*>(c->d_sw[0]), true, c->h_sw_recs, bound)) != B2_OK) return rc;
+    if (bound > out_cap || bound > c->opt.max_resp_bytes) { set_err("out_cap (or max_resp_bytes) below the sum of align16(len + ceil(len / seg) * 38)"); return B2_E_CAPACITY; }
+    if (n == 0) return B2_OK;
+    uint32_t used = 0;
+    return sw_launch(c, bytes, nbytes, n, seg, bound, results, out, &used);
 }
 
 extern "C" int b2_stream_ring_enable(b2_ctx* c, uint32_t out_bytes) {
@@ -1197,19 +1226,21 @@ static int ring_launch(b2_ctx* c) {
     switch (c->ring_kind) {
     case RingKind::h2_server: { const H2RingDev H = h2_ring_dev(c); k_h2_ring<<<1, kSmallThreads, kH2RingSmem, c->ring_stream>>>(R, H); break; }
     case RingKind::h2_client: { const H2ClientRingDev H = h2_client_ring_dev(c); k_h2_client_ring<<<1, kSmallThreads, kH2ClientRingSmem, c->ring_stream>>>(R, H); break; }
-    default: {                              // batch, batch_streams, batch_client
+    default: {                              // batch, batch_streams, batch_stream_writes, batch_client
         const bool was_small = c->small; c->small = false;
         BatchPtrs B = make_ptrs(c);
         c->small = was_small;
         B.bytes = c->d_bytes;
-        const StreamPass SP = c->ring_kind == RingKind::batch_streams ? c->sp_ring : StreamPass{};   // (tab null: the ring runs no stream pass)
+        const StreamPass SP = ring_runs_streams(c->ring_kind) ? c->sp_ring : StreamPass{};   // (tab null: the ring runs no stream pass)
         if (c->ring_kind == RingKind::batch_client) {
             // the scratch of b2_pack_requests, except that the requests and their offsets go to d_msgs / d_refs, which k_ring leaves alone
             ClientRingDev Q = c->cr_dev;
             Q.reqs = reinterpret_cast<ReqDesc*>(c->d_msgs); Q.offs = reinterpret_cast<uint32_t*>(c->d_refs); Q.lens = Q.offs + c->opt.max_msgs;
             Q.scratch = c->d_unz; Q.out = c->d_resp;
-            k_ring<true><<<1, kSmallThreads, sizeof(SmallSmem), c->ring_stream>>>(R, B, c->cfg, SP, Q);
-        } else k_ring<false><<<1, kSmallThreads, sizeof(SmallSmem), c->ring_stream>>>(R, B, c->cfg, SP, ClientRingDev{});
+            k_ring<RingBody::requests><<<1, kSmallThreads, sizeof(SmallSmem), c->ring_stream>>>(R, B, c->cfg, SP, Q);
+        } else if (c->ring_kind == RingKind::batch_stream_writes) {
+            k_ring<RingBody::stream_writes><<<1, kSmallThreads, sizeof(SmallSmem), c->ring_stream>>>(R, B, c->cfg, SP, c->swr_dev);
+        } else k_ring<RingBody::batch><<<1, kSmallThreads, sizeof(SmallSmem), c->ring_stream>>>(R, B, c->cfg, SP, ClientRingDev{});
     }
     }
     c->ring_launches++;
@@ -1242,7 +1273,7 @@ extern "C" int b2_ring_start(b2_ctx* c) {
         R.off_out = L.add(kSmallBlock);
         if (c->ring_kind == RingKind::batch_streams) R.off_st = L.add(kSecOut + ((c->sp_ring.out_cap + 15u) & ~15u));
         int rc = ring_alloc(c, L.end); if (rc != B2_OK) return rc;
-        CU(cudaFuncSetAttribute(k_ring<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmallSmem)));
+        CU(cudaFuncSetAttribute(k_ring<RingBody::batch>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmallSmem)));
     }
     if (!c->ring_ctl[1]) return ring_launch(c);
     return B2_OK;
@@ -1317,7 +1348,7 @@ static uint8_t* ring_collect(b2_ctx* c, bool args_ok, uint32_t ticket, const cha
     rc = B2_E_INVAL;
     if (!args_ok || !c->ring_slots || ticket == 0 || ticket >= c->ring_next || ticket + kRingSlots < c->ring_next) { set_err(bad_ticket); return nullptr; }
     if (c->ring_collected[ticket % kRingSlots]) { set_err("ticket already collected"); return nullptr; }
-    const bool in_order = c->ring_kind == RingKind::batch_streams;
+    const bool in_order = ring_runs_streams(c->ring_kind);
     if (in_order && ticket != c->ring_next_wait) { set_err("a context whose ring runs the stream pass collects its tickets in ticket order"); return nullptr; }
     uint8_t* slot = ring_slot(c, ticket);
     if ((rc = ring_spin(c, reinterpret_cast<const RingSlotHdr*>(slot), ticket)) != B2_OK) return nullptr;
@@ -1325,15 +1356,16 @@ static uint8_t* ring_collect(b2_ctx* c, bool args_ok, uint32_t ticket, const cha
     if (in_order) c->ring_next_wait = ticket + 1;
     return slot;
 }
-static int ring_batch_result(b2_ctx* c, uint32_t ticket, uint8_t* slot, b2_batch_result* out);
+static int ring_batch_result(b2_ctx* c, uint32_t ticket, uint8_t* slot, b2_batch_result* out, bool unpark = true);
 extern "C" int b2_ring_stop(b2_ctx* c) { if (!c) return B2_E_INVAL; cudaSetDevice(c->opt.device); ring_halt(c); return B2_OK; }
 
 extern "C" int b2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs, uint32_t* ticket) {
     if (!c || !bytes || !runs || !ticket || n_runs == 0) { set_err("null argument"); return B2_E_INVAL; }
-    if (c->has_streams && c->ring_kind != RingKind::batch_streams) { set_err("the ring path runs the stream pass only after b2_stream_ring_enable: use b2_batch_submit on a context with a stream table"); return B2_E_INVAL; }
+    if (c->has_streams && !ring_runs_streams(c->ring_kind)) { set_err("the ring path runs the stream pass only after b2_stream_ring_enable: use b2_batch_submit on a context with a stream table"); return B2_E_INVAL; }
     if (c->ring_kind == RingKind::h2_server) { set_err("this context's ring serves h2 (b2_h2_ring_enable): use b2_h2_ring_submit"); return B2_E_INVAL; }
     if (c->ring_kind == RingKind::h2_client) { set_err("this context's ring serves h2 client connections (b2_h2_client_ring_enable): use b2_h2_client_ring_submit"); return B2_E_INVAL; }
     if (c->ring_kind == RingKind::batch_client) { set_err("this context's ring serves client turns (b2_client_ring_enable): use b2_client_ring_submit"); return B2_E_INVAL; }
+    if (c->ring_kind == RingKind::batch_stream_writes) { set_err("this context's ring serves Stream producer turns (b2_stream_ring_write_enable): use b2_stream_ring_submit"); return B2_E_INVAL; }
     if (nbytes > kSmallBytes || n_runs > kSmallRuns) { set_err("b2_ring_submit serves batches up to 128 KiB / 512 runs: use b2_batch_submit"); return B2_E_CAPACITY; }
     if (!c->ring_slots) { int rc = b2_ring_start(c); if (rc != B2_OK) return rc; }
     uint8_t* slot = ring_claim(c, "b2_ring_wait");
@@ -1349,16 +1381,20 @@ extern "C" int b2_ring_wait(b2_ctx* c, uint32_t ticket, b2_batch_result* out) {
     if (c && c->ring_kind == RingKind::h2_server) { set_err("this context's ring serves h2: use b2_h2_ring_wait"); return B2_E_INVAL; }
     if (c && c->ring_kind == RingKind::h2_client) { set_err("this context's ring serves h2 client connections: use b2_h2_client_ring_wait"); return B2_E_INVAL; }
     if (c && c->ring_kind == RingKind::batch_client) { set_err("this context's ring serves client turns: use b2_client_ring_wait"); return B2_E_INVAL; }
+    if (c && c->ring_kind == RingKind::batch_stream_writes) { set_err("this context's ring serves Stream producer turns: use b2_stream_ring_wait"); return B2_E_INVAL; }
     int rc;
     uint8_t* slot = ring_collect(c, c && out, ticket, "bad ring ticket", rc);
     if (!slot) return rc;
     return ring_batch_result(c, ticket, slot, out);
 }
-// The runs' result of a collected k_ring ticket, from its compact block, or from the big pipeline when the runs overflowed it
-static int ring_batch_result(b2_ctx* c, uint32_t ticket, uint8_t* slot, b2_batch_result* out) {
+// The runs' result of a collected k_ring ticket, from its compact block, or from the big pipeline when the runs overflowed it.  unpark:
+// release the kernel parked behind an overflowing ticket of a stream ring here (false: the caller has more of the ticket to serve first,
+// and releases it with ring_unpark)
+static void ring_unpark(b2_ctx* c, uint32_t ticket) { __sync_synchronize(); c->ring_ctl[3] = ticket; __sync_synchronize(); }
+static int ring_batch_result(b2_ctx* c, uint32_t ticket, uint8_t* slot, b2_batch_result* out, bool unpark) {
     int rc;
     const uint32_t si = ticket % kRingSlots;
-    const bool streams = c->ring_kind == RingKind::batch_streams;
+    const bool streams = ring_runs_streams(c->ring_kind);
     RingSlotHdr* h = reinterpret_cast<RingSlotHdr*>(slot);
     memset(out, 0, sizeof *out);
     const uint8_t* ob = slot + c->ring_dev.off_out;
@@ -1372,7 +1408,7 @@ static int ring_batch_result(b2_ctx* c, uint32_t ticket, uint8_t* slot, b2_batch
         const bool allow = c->allow_small; c->allow_small = false;
         rc = b2_process_batch(c, c->ring_bytes[si], h->nbytes, reinterpret_cast<const b2_run*>(slot + c->ring_dev.off_runs), h->n_runs, out);
         c->allow_small = allow;
-        if (streams) { __sync_synchronize(); c->ring_ctl[3] = ticket; __sync_synchronize(); }
+        if (streams && unpark) ring_unpark(c, ticket);
         return rc;
     }
     out->runs = reinterpret_cast<const b2_run_status*>(ob + h->off_rs); out->n_runs = h->n_runs;
@@ -2337,7 +2373,7 @@ extern "C" int b2_h2_client_ring_wait(b2_ctx* c, uint32_t ticket, b2_h2_client_r
     return B2_OK;
 }
 
-// ---- a baidu_std client's turn on the latency path: k_ring<true> on the same submit ring (include/b2rpc.h, b2_client_ring_enable) ----
+// ---- a baidu_std client's turn on the latency path: k_ring<RingBody::requests> on the same submit ring (include/b2rpc.h, b2_client_ring_enable) ----
 extern "C" int b2_client_ring_enable(b2_ctx* c, uint32_t max_bytes, uint32_t max_reqs, uint32_t req_out_cap) {
     if (!c) { set_err("null argument"); return B2_E_INVAL; }
     if (c->ring_kind != RingKind::none) { set_err("b2_client_ring_enable: once, before the context's first ring call, and not with another ring kind"); return B2_E_INVAL; }
@@ -2358,7 +2394,7 @@ extern "C" int b2_client_ring_enable(b2_ctx* c, uint32_t max_bytes, uint32_t max
     Q.off_req_lens = L.add((uint64_t)max_reqs * 4);
     Q.off_req_out = L.add((uint64_t)req_out_cap + 16);
     int rc = ring_alloc(c, L.end); if (rc != B2_OK) return rc;
-    CU(cudaFuncSetAttribute(k_ring<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmallSmem)));
+    CU(cudaFuncSetAttribute(k_ring<RingBody::requests>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmallSmem)));
     c->cr_max_bytes = max_bytes; c->cr_max_reqs = max_reqs; c->cr_req_out_cap = req_out_cap;
     c->ring_kind = RingKind::batch_client;
     return B2_OK;
@@ -2403,4 +2439,114 @@ extern "C" int b2_client_ring_wait(b2_ctx* c, uint32_t ticket, b2_client_ring_re
     out->req_lens = reinterpret_cast<const uint32_t*>(slot + L.off_req_lens);
     out->req_out = slot + L.off_req_out;
     return ring_batch_result(c, ticket, slot, &out->batch);      // (an overflowing ticket's runs go through the big pipeline here)
+}
+
+// ---- a Stream producer's turn on the latency path: k_ring<RingBody::stream_writes> (include/b2rpc.h, b2_stream_ring_write_enable) ----
+extern "C" int b2_stream_ring_write_enable(b2_ctx* c, uint32_t max_bytes, uint32_t max_writes, uint32_t write_out_cap, uint32_t max_segment_size) {
+    if (!c) { set_err("null argument"); return B2_E_INVAL; }
+    if (c->ring_kind != RingKind::batch_streams || c->ring_slots) { set_err("b2_stream_ring_write_enable: after b2_stream_ring_enable and before the context's first ring call"); return B2_E_INVAL; }
+    if (max_bytes == 0 || max_writes == 0 || write_out_cap == 0) { set_err("capacities must be non-zero"); return B2_E_INVAL; }
+    // the limits of b2_process_batch and b2_stream_write, both of which read the ticket's bytes
+    if (max_bytes > c->opt.max_batch_bytes || max_writes > c->opt.max_msgs || write_out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    CU(cudaSetDevice(c->opt.device));
+    static_assert(sizeof(RingSlotHdr) + sizeof(SwRingArgs) <= 256, "stream write ring slot header");
+    int rc = sw_host_recs(c, max_writes);               // (the records are resolved there before they go into the slot)
+    if (rc != B2_OK) return rc;
+    // the write pass's scratch, as sw_launch lays out d_sw[2] / d_sw[3] / d_sw[1] for a call of max_writes writes
+    const size_t mw = max_writes, cap = c->sp.cap;
+    const size_t o_res = (mw * 24 + 15) & ~(size_t)15, o_slot = o_res + 32 * mw, o_group = o_slot + ((4 * mw + 15) & ~(size_t)15),
+                 o_fb = o_group + 8 * mw, o_cb = o_fb + ((4 * mw + 15) & ~(size_t)15), o_ps = (o_cb + 4 * mw + 255) & ~(size_t)255,
+                 o_out = (o_ps + 64 + 16 * cap + 255) & ~(size_t)255;
+    cudaFree(c->d_swr); c->d_swr = nullptr;
+    if (cudaMalloc((void**)&c->d_swr, o_out + write_out_cap + 32) != cudaSuccess) { cudaGetLastError(); set_err("cudaMalloc of the stream write ring scratch failed"); return B2_E_NOMEM; }
+    CU(cudaMemset(c->d_swr + o_ps, 0, 64 + 16 * cap));  // counters | cnt | fill: the ring's tickets start from zeros
+    SwPass& P = c->swr_dev.pass;
+    P.tab = c->sp.tab; P.cap = c->sp.cap; P.recs = reinterpret_cast<const SwRec*>(c->d_swr); P.n = 0;
+    P.seg = max_segment_size ? max_segment_size : 512u << 20;                     // -stream_write_max_segment_size (stream.cpp:39)
+    uint32_t* per_slot = reinterpret_cast<uint32_t*>(c->d_swr + o_ps);
+    P.cnts = per_slot; P.cnt = per_slot + 16; P.fill = P.cnt + cap; P.base = P.fill + cap; P.touched = P.base + cap;
+    P.res = reinterpret_cast<b2_stream_write_result*>(c->d_swr + o_res); P.slot = reinterpret_cast<uint32_t*>(c->d_swr + o_slot);
+    P.group = reinterpret_cast<uint32_t*>(c->d_swr + o_group); P.frame_base = reinterpret_cast<uint32_t*>(c->d_swr + o_fb);
+    P.chunk_base = reinterpret_cast<uint32_t*>(c->d_swr + o_cb); P.out = c->d_swr + o_out;
+    // [RingSlotHdr | args | runs | staged input | write records | compact block | stream section | write results | frames]
+    SlotLayout L;
+    SwRingDev& Q = c->swr_dev;
+    RingDev& R = c->ring_dev;
+    Q.off_args = sizeof(RingSlotHdr);
+    R.off_runs = L.add(kSmallRuns * sizeof(b2_run));
+    R.off_in = L.add((uint64_t)max_bytes + 16);
+    Q.off_recs = L.add(mw * sizeof(SwRec) + 16);
+    R.off_out = L.add(kSmallBlock);
+    R.off_st = L.add(kSecOut + ((c->sp_ring.out_cap + 15u) & ~15u));
+    Q.off_res = L.add(mw * sizeof(b2_stream_write_result) + 16);
+    Q.off_wout = L.add((uint64_t)write_out_cap + 16);
+    if ((rc = ring_alloc(c, L.end)) != B2_OK) return rc;
+    CU(cudaFuncSetAttribute(k_ring<RingBody::stream_writes>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmallSmem)));
+    c->swr_max_bytes = max_bytes; c->swr_max_writes = max_writes; c->swr_out_cap = write_out_cap;
+    c->ring_kind = RingKind::batch_stream_writes;
+    return B2_OK;
+}
+extern "C" int b2_stream_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
+                                     const b2_stream_write_desc* writes, uint32_t n_writes, uint32_t* ticket) {
+    if (!c || !bytes || !ticket || (!runs && n_runs) || (!writes && n_writes)) { set_err("null argument"); return B2_E_INVAL; }
+    if (n_runs == 0 && n_writes == 0) { set_err("a ticket carries runs, writes or both"); return B2_E_INVAL; }
+    if (c->ring_kind != RingKind::batch_stream_writes) { set_err("b2_stream_ring_write_enable first"); return B2_E_INVAL; }
+    // the argument checks of b2_ring_submit and b2_stream_write with the caps of b2_stream_ring_write_enable
+    if (nbytes > c->swr_max_bytes) { set_err("ticket larger than b2_stream_ring_write_enable's max_bytes: use the batch calls"); return B2_E_CAPACITY; }
+    if (n_runs > kSmallRuns || n_runs > c->opt.max_runs) { set_err("b2_stream_ring_submit serves up to 512 runs: use the batch calls"); return B2_E_CAPACITY; }
+    if (n_writes > c->swr_max_writes) { set_err("more writes than b2_stream_ring_write_enable's max_writes"); return B2_E_CAPACITY; }
+    uint8_t* slot = ring_claim(c, "b2_stream_ring_wait");
+    if (!slot) return B2_E_CAPACITY;
+    uint32_t extent = 0;                                         // (the compact block is sized for the bytes the runs cover)
+    for (uint32_t r = 0; r < n_runs; r++) {
+        if ((runs[r].offset & 15u) || (uint64_t)runs[r].offset + runs[r].length > nbytes) { set_err("run offset must be 16-aligned and inside the batch"); return B2_E_INVAL; }
+        extent = std::max(extent, runs[r].offset + runs[r].length);
+    }
+    // the kernel pulls every ticket into d_bytes: that is where a host-sourced payload is
+    uint64_t bound = 0;
+    int rc = sw_resolve(c, writes, n_writes, nbytes, c->swr_dev.pass.seg, c->d_bytes, false, c->h_sw_recs, bound);
+    if (rc != B2_OK) return rc;
+    if (bound > c->swr_out_cap) { set_err("write_out_cap below the sum of align16(len + ceil(len / seg) * 38)"); return B2_E_CAPACITY; }
+    const SwRingArgs a = { n_writes, (uint32_t)bound, { 0, 0 } };
+    RingSlotHdr* h = ring_fill(c, slot, bytes, nbytes, runs, n_runs);
+    ring_compact(c, h, small_layout(std::min(extent, kSmallBytes), n_runs, c->opt.max_msgs));
+    if (n_writes) memcpy(slot + c->swr_dev.off_recs, c->h_sw_recs, sizeof(SwRec) * (size_t)n_writes);
+    memcpy(slot + c->swr_dev.off_args, &a, sizeof a);
+    return ring_ring(c, h, bytes, ticket);
+}
+extern "C" int b2_stream_ring_wait(b2_ctx* c, uint32_t ticket, b2_stream_ring_result* out) {
+    static_assert(sizeof(b2_stream_ring_result) == 96, "stream ring result ABI layout");
+    int rc;
+    uint8_t* slot = ring_collect(c, c && out && c->ring_kind == RingKind::batch_stream_writes, ticket, "bad stream ring ticket", rc);
+    if (!slot) return rc;
+    memset(out, 0, sizeof *out);
+    const SwRingDev& L = c->swr_dev;
+    const SwRingArgs args = *reinterpret_cast<const SwRingArgs*>(slot + L.off_args);
+    const uint32_t n = args.n_writes;
+    b2_stream_write_result* res = reinterpret_cast<b2_stream_write_result*>(slot + L.off_res);
+    const bool overflow = reinterpret_cast<const uint32_t*>(slot + c->ring_dev.off_out)[2] & 3u;
+    rc = ring_batch_result(c, ticket, slot, &out->batch, false);
+    if (overflow) {
+        // k_ring ran neither pass and parks behind the ticket: the big pipeline has served the runs (and their stream pass); the writes go
+        // through the grid path on the ticket's own bytes, and only then does the next ticket see the table
+        if (rc == B2_OK && n) {
+            const SwRec* recs = reinterpret_cast<const SwRec*>(slot + L.off_recs);
+            uint32_t used = 0;
+            rc = sw_reserve(c, 0, reinterpret_cast<const RingSlotHdr*>(slot)->nbytes);
+            if (rc == B2_OK) {
+                const uint8_t* d_in = static_cast<const uint8_t*>(c->d_sw[0]);      // (the staging the grid path copies the bytes into)
+                for (uint32_t i = 0; i < n; i++) { c->h_sw_recs[i] = recs[i]; c->h_sw_recs[i].src = d_in + (recs[i].src - c->d_bytes); }
+                rc = sw_launch(c, c->ring_bytes[ticket % kRingSlots], reinterpret_cast<const RingSlotHdr*>(slot)->nbytes, n, L.pass.seg, args.bound, res,
+                               slot + L.off_wout, &used);
+            }
+        }
+        ring_unpark(c, ticket);
+        if (rc != B2_OK) return rc;
+    }
+    if (rc != B2_OK) return rc;
+    uint32_t used = 0;                                           // (out_off grows in array order; the gaps are part of the frames)
+    for (uint32_t i = 0; i < n; i++) used = std::max(used, res[i].out_off + ((res[i].out_len + 15u) & ~15u));
+    out->n_writes = n; out->out_bytes = used;
+    out->results = res; out->out = slot + L.off_wout;
+    return B2_OK;
 }

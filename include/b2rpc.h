@@ -474,7 +474,7 @@ typedef struct b2_request {
 int  b2_pack_requests(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2_request* reqs, uint32_t n,
                       void* out, uint32_t out_cap, uint32_t* out_offs, uint32_t* out_lens);
 /* baidu_std CLIENT connections on the latency path: b2_process_batch followed by b2_pack_requests inside the resident k_ring
- * (k_ring<true>) fed through the same submit ring.  A ticket is one turn of a client's event loop: read what arrived, then send what is
+ * (k_ring<RingBody::requests>) fed through the same submit ring.  A ticket is one turn of a client's event loop: read what arrived, then send what is
  * queued.  The runs (the bytes read from client sockets, B2_RUN_CLIENT) are served as by b2_ring_submit, then the requests are packed as
  * by b2_pack_requests; their fields index the same `bytes` as the runs.  A baidu_std client keeps no connection state on the device
  * (correlation ids live on the host), so a ticket's requests do not depend on its runs: they are packed even when the runs overflow the
@@ -1060,6 +1060,45 @@ typedef struct b2_stream_write_result {
 /* max_segment_size: -stream_write_max_segment_size (stream.cpp:39); 0 = brpc's default, 512 MiB. */
 int  b2_stream_write(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2_stream_write_desc* writes, uint32_t n,
                      uint32_t max_segment_size, void* out, uint32_t out_cap, b2_stream_write_result* results);
+/* A Stream producer's turn on the latency path: b2_process_batch followed by b2_stream_write inside the resident k_ring
+ * (k_ring<RingBody::stream_writes>) fed through the same submit ring.  A ticket is one turn: read the FEEDBACK / RST / CLOSE (and DATA)
+ * frames the peers sent, then write what is queued.  Its runs are served as b2_ring_submit serves them on a context with
+ * b2_stream_ring_enable (the batch, then the stream pass); then its writes are applied as b2_stream_write applies them, in array order,
+ * against the table the stream pass just updated.  brpc leaves the race between a socket's read and StreamWrite callers to scheduling;
+ * here a ticket reads first: a FEEDBACK in its runs moves remote_consumed before its writes are admitted, and an RST / CLOSE in its runs
+ * closes the stream before its writes (EINVAL).  B2_STREAM_EV_WRITABLE keeps its meaning: produced does not move during the stream pass.
+ * A context runs one ring kind: b2_ring_submit / _wait and the other kinds' calls refuse a context that runs this one, and
+ * b2_stream_ring_* refuse a context of another kind.  Every rule of b2_stream_ring_enable holds: tickets are collected in ticket order,
+ * the table calls and b2_stream_write fail with B2_E_INVAL while a ticket is outstanding, and b2_stream_results describes the ticket
+ * after its wait (an empty pass for a ticket without runs).
+ * b2_stream_ring_write_enable: after b2_stream_ring_enable and before the context's first ring call (else B2_E_INVAL).  max_bytes bounds
+ * a ticket's whole `bytes` (the runs' bytes plus the write payloads, <= max_batch_bytes, so a turn may exceed b2_ring_submit's 128 KiB);
+ * max_writes (<= max_msgs) and write_out_cap (<= max_resp_bytes) play the roles of b2_stream_write's n and out_cap; max_segment_size has
+ * b2_stream_write's meaning (0 = 512 MiB) for every ticket.  Caps above those limits fail with B2_E_CAPACITY; they fix the slot layout.
+ * b2_ring_stop, b2_ring_launches, b2_ring_phase_ns ([2]: runs, stream pass and writes done) and B2_RING_IDLE_MS apply as to k_ring.
+ * b2_stream_ring_submit: n_runs or n_writes may be 0, not both.  Every check of b2_ring_submit (<= 512 runs, 16-aligned runs inside
+ * `bytes`) and of b2_stream_write (n_writes <= max_writes, known flags, payloads inside `bytes`, the sum over writes of
+ * align16(len + ceil(len / seg) * 38) <= write_out_cap: B2_E_CAPACITY) applies with the enable-time caps; a failed check claims no slot
+ * and leaves the next ticket number unchanged.  Write payloads index the same `bytes` as the runs.  B2_STREAM_W_FROM_MSG is refused
+ * (B2_E_INVAL): which messages a ticket completes is not known when it is submitted; echo a received message with b2_stream_write
+ * between tickets, which resolves FROM_MSG against the most recent ticket.  The runs keep the compact block's limits, sized from the extent
+ * the runs cover.  Bytes in b2_block_alloc memory are pulled in place, others staged into the slot.
+ * b2_stream_ring_wait: for any sequence of tickets, `batch`, b2_stream_results, every write result and the frames (the zero gaps between
+ * writes included, out_bytes of them) equal, byte for byte, what a context with the same table returns for b2_process_batch(bytes, runs)
+ * followed by b2_stream_write(bytes, writes, max_segment_size), each call skipped when its list is empty; so does b2_stream_query of every
+ * stream afterwards.  A ticket whose runs overflow the compact block has its runs served through the big pipeline inside the wait, then
+ * its writes through b2_stream_write's kernels, and only then does the kernel serve the next ticket.  `bytes` must stay unchanged until
+ * the ticket is collected. */
+typedef struct b2_stream_ring_result {      /* views into the ticket's pinned slot, valid until the 8th later submission */
+    b2_batch_result batch;                  /* the runs, exactly as b2_ring_wait returns them */
+    uint32_t n_writes, out_bytes;
+    const b2_stream_write_result* results;  /* as b2_stream_write's results */
+    const uint8_t* out;                     /* write i's frames at out + results[i].out_off */
+} b2_stream_ring_result;                    /* 96 bytes */
+int  b2_stream_ring_write_enable(b2_ctx* ctx, uint32_t max_bytes, uint32_t max_writes, uint32_t write_out_cap, uint32_t max_segment_size);
+int  b2_stream_ring_submit(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
+                           const b2_stream_write_desc* writes, uint32_t n_writes, uint32_t* ticket);
+int  b2_stream_ring_wait(b2_ctx* ctx, uint32_t ticket, b2_stream_ring_result* out);
 
 /* ---- counters (bvar::Adder-like, SURVEY §8e): per-GPU totals accumulated by
  * the kernels: [0] in_bytes [1] in_msgs [2] out_bytes [3] out_msgs [4] errors
