@@ -99,6 +99,14 @@ class H2RingResult(C.Structure):
 assert C.sizeof(H2RingResult) == 64
 
 
+class H2RingTurnResult(C.Structure):
+    _fields_ = [("ring", H2RingResult), ("n_resps", C.c_uint32), ("reserved", C.c_uint32), ("resp_offs", C.c_void_p), ("resp_lens", C.c_void_p),
+                ("resp_out", C.c_void_p)]
+
+
+assert C.sizeof(H2RingTurnResult) == 96
+
+
 class H2ClientRingResult(C.Structure):
     _fields_ = [("runs", C.c_void_p), ("n_runs", C.c_uint32), ("n_calls", C.c_uint32), ("calls", C.c_void_p), ("out", C.c_void_p),
                 ("region", C.c_uint32), ("n_reqs", C.c_uint32), ("reqs", C.c_void_p), ("req_out", C.c_void_p), ("status", C.c_int32),
@@ -220,6 +228,9 @@ def _load():
     l.b2_h2_ring_enable.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]
     l.b2_h2_ring_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
     l.b2_h2_ring_wait.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(H2RingResult)]
+    l.b2_h2_ring_turn_enable.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]
+    l.b2_h2_ring_turn_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
+    l.b2_h2_ring_turn_wait.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(H2RingTurnResult)]
     l.b2_h2_client_ring_enable.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]
     l.b2_h2_client_ring_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
     l.b2_h2_client_ring_wait.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(H2ClientRingResult)]
@@ -257,7 +268,7 @@ ABI_SYMBOLS = ["b2_ctx_create", "b2_ctx_destroy", "b2_last_error", "b2_version",
                "b2_h2_client_conn_reset", "b2_h2_client_process_batch", "b2_h2_client_abandon_streams", "b2_h2_conn_set_gunzip",
                "b2_h2_serve_batch", "b2_stream_configure", "b2_stream_open", "b2_stream_set_connected", "b2_stream_close", "b2_stream_query",
                "b2_stream_take_pending", "b2_stream_results", "b2_stream_write", "b2_stream_ring_enable", "b2_h2_ring_enable", "b2_h2_ring_submit",
-               "b2_h2_ring_wait", "b2_h2_client_ring_enable", "b2_h2_client_ring_submit", "b2_h2_client_ring_wait", "b2_client_ring_enable",
+               "b2_h2_ring_wait", "b2_h2_ring_turn_enable", "b2_h2_ring_turn_submit", "b2_h2_ring_turn_wait", "b2_h2_client_ring_enable", "b2_h2_client_ring_submit", "b2_h2_client_ring_wait", "b2_client_ring_enable",
                "b2_client_ring_submit", "b2_client_ring_wait", "b2_stream_ring_write_enable", "b2_stream_ring_submit", "b2_stream_ring_wait"]
 
 ECHO_METHOD = dict(service_full_name=b"example.EchoService", service_name=b"EchoService", method_name=b"Echo",
@@ -274,6 +285,15 @@ def _check(rc):
 def _view(ptr, nbytes, dtype=np.uint8):
     """nbytes of context-owned memory at ptr as a dtype array (no copy)"""
     return np.ctypeslib.as_array((C.c_uint8 * nbytes).from_address(ptr)).view(dtype) if nbytes else np.zeros(0, dtype)
+
+
+def _h2_ring_views(res):
+    """(run_status, msgs, out, replies, spans) of an H2RingResult: out covers n_runs * region bytes, replies every span"""
+    n = res.n_runs
+    spans = _view(res.spans, 16 * n, H2_REPLY_SPAN_DT)
+    rep_end = int((spans["off"].astype(np.int64) + spans["len"]).max()) if n else 0
+    return (_view(res.runs, 32 * n, H2_RUN_STATUS_DT), _view(res.msgs, 64 * res.n_msgs, H2_MSG_DT), _view(res.out, res.region * n),
+            _view(res.replies, rep_end), spans)
 
 
 # The cyclic garbage collector runs at whatever allocation crosses its threshold — inside a latency loop as well — and b2_ctx_destroy waits
@@ -788,11 +808,34 @@ class Context:
         _check(lib.b2_h2_ring_wait(self._h, ticket, C.byref(res)))
         if res.status < 0:
             raise B2Error(res.status, "h2 ring ticket %d" % ticket)
-        n = res.n_runs
-        spans = _view(res.spans, 16 * n, H2_REPLY_SPAN_DT)
-        rep_end = int((spans["off"].astype(np.int64) + spans["len"]).max()) if n else 0
-        return (_view(res.runs, 32 * n, H2_RUN_STATUS_DT), _view(res.msgs, 64 * res.n_msgs, H2_MSG_DT), _view(res.out, res.region * n),
-                _view(res.replies, rep_end), spans)
+        return _h2_ring_views(res)
+
+    def h2_ring_turn_enable(self, max_bytes, msg_cap, out_cap, replies_cap, max_resps, resp_out_cap):
+        """h2_ring_enable whose tickets may also carry the replies the host produced (b2_h2_ring_turn_enable): at most max_resps of them,
+        framed within resp_out_cap bytes, per turn."""
+        _check(lib.b2_h2_ring_turn_enable(self._h, max_bytes, msg_cap, out_cap, replies_cap, max_resps, resp_out_cap))
+
+    def h2_ring_turn_submit(self, data, runs, resps, ptr=None, nbytes=None):
+        """One turn of a gRPC server's event loop: the runs are served as by h2_serve_batch, then resps (H2_RESPONSE_DT, offsets into the
+        same data, no zero-copy flags) are packed as by h2_pack_responses.  Either list may be empty, not both.  Returns the ticket."""
+        runs = np.ascontiguousarray(runs, dtype=RUN_DT); resps = np.ascontiguousarray(resps, dtype=H2_RESPONSE_DT)
+        ptr, nbytes = self._ring_bytes(data, ptr, nbytes)
+        t = C.c_uint32(0)
+        _check(lib.b2_h2_ring_turn_submit(self._h, ptr, nbytes, runs.ctypes.data if len(runs) else None, len(runs),
+                                          resps.ctypes.data if len(resps) else None, len(resps), C.byref(t)))
+        return t.value
+
+    def h2_ring_turn_wait(self, ticket):
+        """(status, served, [frames per host reply]): status is what h2_serve_batch would have returned for the runs (0, or B2_E_CAPACITY,
+        when served lists no messages); served is (run_status, msgs, out, replies, spans) as h2_ring_wait returns them (views of the slot);
+        the frames are copies."""
+        res = H2RingTurnResult()
+        _check(lib.b2_h2_ring_turn_wait(self._h, ticket, C.byref(res)))
+        n = res.n_resps
+        offs, lens = _view(res.resp_offs, 4 * n, np.uint32), _view(res.resp_lens, 4 * n, np.uint32)
+        end = int((offs.astype(np.int64) + lens).max()) if n else 0
+        frames = _view(res.resp_out, end)
+        return res.ring.status, _h2_ring_views(res.ring), [frames[int(o):int(o) + int(ln)].tobytes() for o, ln in zip(offs, lens)]
 
     # ---- h2/gRPC client connections on the latency path (b2_h2_client_ring_*) ----
     def h2_client_ring_enable(self, max_bytes, call_cap, out_cap, max_reqs, req_out_cap):

@@ -85,6 +85,7 @@ struct b2_ctx {
     StreamPass sp_ring = {}; uint8_t* d_st_ring = nullptr; uint32_t ring_next_wait = 1, st_view_ticket = 0;
     // the caps every ticket of an h2 ring (k_h2_ring, k_h2_client_ring) is served with
     uint32_t h2r_max_bytes = 0, h2r_msg_cap = 0, h2r_out_cap = 0, h2r_replies_cap = 0;
+    uint32_t h2r_max_resps = 0, h2r_resp_out_cap = 0; H2TurnDev h2t_dev = {};   // ... and the host replies of a turn (b2_h2_ring_turn_enable)
     uint32_t h2c_max_bytes = 0, h2c_call_cap = 0, h2c_out_cap = 0, h2c_max_reqs = 0, h2c_req_out_cap = 0;
     uint32_t cr_max_bytes = 0, cr_max_reqs = 0, cr_req_out_cap = 0;        // ... and of the client ring (k_ring<RingBody::requests>)
     // the stream write ring (k_ring<RingBody::stream_writes>): its caps, its slot parts and the write pass's device scratch (d_swr)
@@ -227,7 +228,7 @@ extern "C" void b2_ctx_destroy(b2_ctx* c) {
     if (c->ring_stream) cudaStreamDestroy(c->ring_stream);
     if (c->ring_slots) cudaFreeHost(c->ring_slots);
     if (c->ring_ctl) cudaFreeHost((void*)c->ring_ctl);
-    cudaFree(c->d_ring_ticket);
+    cudaFree(c->d_ring_ticket); cudaFree(c->h2t_dev.turn);
     cudaFree(c->d_bytes); cudaFree(c->d_runs); cudaFree(c->d_run_tile_base); cudaFree(c->d_tiles); cudaFree(c->d_tile_base); cudaFree(c->d_tile_scratch); cudaFree(c->d_head_recs); cudaFree(c->d_tile_spec);
     cudaFree(c->d_run_status); cudaFree(c->d_frame_off); cudaFree(c->d_frame_run); cudaFree(c->d_msgs); cudaFree(c->d_aux); cudaFree(c->d_jobs); cudaFree(c->d_slow_idx); cudaFree(c->d_heads); cudaFree(c->d_slot);
     cudaFree(c->d_scan_tmp); cudaFree(c->d_resp); cudaFree(c->d_unz); cudaFree(c->d_snappy_tab); cudaFree(c->d_refs); cudaFree(c->d_iov); cudaFreeHost(c->h_iov); cudaFree(c->d_frame_row); cudaFree(c->d_rows); cudaFreeHost(c->h_refs); cudaFree(c->d_hpack); cudaFree(c->d_h2); cudaFree(c->d_h2_streams); cudaFree(c->d_h2_slots); cudaFree(c->d_h2_gz_merge); cudaFree(c->d_counters); cudaFree(c->d_totals); cudaFree(c->d_methods); cudaFree(c->d_crc_adv); cudaFree(c->d_meta); cudaFree(c->d_small); cudaFreeHost(c->h_meta); cudaFreeHost(c->h_small);
@@ -1224,7 +1225,12 @@ static int ring_launch(b2_ctx* c) {
     R.d_bytes = c->d_bytes; R.d_meta = c->d_meta; R.d_small = c->d_small;
     c->ring_ctl[1] = 1; __sync_synchronize();
     switch (c->ring_kind) {
-    case RingKind::h2_server: { const H2RingDev H = h2_ring_dev(c); k_h2_ring<<<1, kSmallThreads, kH2RingSmem, c->ring_stream>>>(R, H); break; }
+    case RingKind::h2_server: {             // k_h2_ring<true> on a turn-enabled context (b2_h2_ring_turn_enable)
+        const H2RingDev H = h2_ring_dev(c);
+        if (c->h2r_max_resps) k_h2_ring<true><<<1, kSmallThreads, kH2RingSmem, c->ring_stream>>>(R, H, c->h2t_dev);
+        else k_h2_ring<false><<<1, kSmallThreads, kH2RingSmem, c->ring_stream>>>(R, H, H2TurnDev{});
+        break;
+    }
     case RingKind::h2_client: { const H2ClientRingDev H = h2_client_ring_dev(c); k_h2_client_ring<<<1, kSmallThreads, kH2ClientRingSmem, c->ring_stream>>>(R, H); break; }
     default: {                              // batch, batch_streams, batch_stream_writes, batch_client
         const bool was_small = c->small; c->small = false;
@@ -1973,15 +1979,11 @@ extern "C" int b2_h2_serve_batch(b2_ctx* c, const void* bytes, uint32_t nbytes, 
     return h2_parse_batch(c, bytes, nbytes, runs, n_runs, rs, msgs, msg_cap, n_msgs, out, out_cap, &serve);
 }
 
-extern "C" int b2_h2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_h2_response* resps, uint32_t n,
-                                    void* out, uint32_t out_cap, uint32_t* out_offs, uint32_t* out_lens) {
-    if (!c || (!bytes && nbytes) || !resps || !out || !out_offs || !out_lens) { set_err("null argument"); return B2_E_INVAL; }
-    if (ring_refuses(c, true)) return B2_E_INVAL;
-    static_assert(sizeof(b2_h2_response) == 48, "h2 response ABI layout");
-    if (nbytes > c->opt.max_resp_bytes || n > c->opt.max_msgs || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
-    if (n == 0) return B2_OK;
-    std::vector<uint32_t> first;
-    uint64_t total = 0;
+// the replies of b2_h2_pack_responses or of a turn (b2_h2_ring_turn_submit): the connection in range, every field inside its source
+// (bytes, or the last batch's input / out for the zero-copy flags), content-type <= 256 and grpc-message <= 512 bytes, each reply's room
+// in out placed at its bound (h2_reply_bound; total: the bytes placed), and replies of one connection adjacent (first: the connection groups)
+static int h2_place_responses(const b2_ctx* c, uint32_t nbytes, const b2_h2_response* resps, uint32_t n, uint32_t out_cap,
+                              uint32_t* out_offs, std::vector<uint32_t>& first, uint64_t& total) {
     for (uint32_t i = 0; i < n; i++) {
         const b2_h2_response& r = resps[i];
         const uint64_t body_lim = (r.flags & B2_H2_RESP_BODY_IN_INPUT) ? c->h2_last_in : (r.flags & B2_H2_RESP_BODY_IN_OUT) ? c->h2_last_out : nbytes;
@@ -1993,6 +1995,18 @@ extern "C" int b2_h2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbyte
         if (!out_place(total, need, out_cap, &out_offs[i])) { set_err("out_cap too small"); return B2_E_CAPACITY; }
     }
     if (!conn_groups(n, [&](uint32_t i) { return resps[i].conn; }, first)) { set_err("responses of one connection must be adjacent"); return B2_E_INVAL; }
+    return B2_OK;
+}
+extern "C" int b2_h2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_h2_response* resps, uint32_t n,
+                                    void* out, uint32_t out_cap, uint32_t* out_offs, uint32_t* out_lens) {
+    if (!c || (!bytes && nbytes) || !resps || !out || !out_offs || !out_lens) { set_err("null argument"); return B2_E_INVAL; }
+    if (ring_refuses(c, true)) return B2_E_INVAL;
+    static_assert(sizeof(b2_h2_response) == 48, "h2 response ABI layout");
+    if (nbytes > c->opt.max_resp_bytes || n > c->opt.max_msgs || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    if (n == 0) return B2_OK;
+    std::vector<uint32_t> first;
+    uint64_t total = 0;
+    { int rc = h2_place_responses(c, nbytes, resps, n, out_cap, out_offs, first, total); if (rc != B2_OK) return rc; }
     const uint32_t n_groups = (uint32_t)first.size() - 1;
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     CU(cudaSetDevice(c->opt.device));
@@ -2215,31 +2229,48 @@ static H2RingDev h2_ring_dev(const b2_ctx* c) {
     H.spans = reinterpret_cast<b2_h2_reply_span*>(c->d_refs); H.replies = c->d_resp;
     return H;
 }
-extern "C" int b2_h2_ring_enable(b2_ctx* c, uint32_t max_bytes, uint32_t msg_cap, uint32_t out_cap, uint32_t replies_cap) {
-    if (!c) { set_err("null argument"); return B2_E_INVAL; }
-    if (c->ring_kind != RingKind::none) { set_err("b2_h2_ring_enable: once, before the context's first ring call, and not with another ring kind"); return B2_E_INVAL; }
+// b2_h2_ring_enable, and b2_h2_ring_turn_enable with max_resps > 0: the host-reply parts of the slot and their device scratch too
+static int h2_ring_setup(b2_ctx* c, const char* call, uint32_t max_bytes, uint32_t msg_cap, uint32_t out_cap, uint32_t replies_cap,
+                         uint32_t max_resps, uint32_t resp_out_cap) {
+    if (c->ring_kind != RingKind::none) { set_err("%s: once, before the context's first ring call, and not with another ring kind", call); return B2_E_INVAL; }
     if (max_bytes == 0 || msg_cap == 0 || out_cap == 0 || replies_cap == 0) { set_err("capacities must be non-zero"); return B2_E_INVAL; }
     if (max_bytes > c->opt.max_batch_bytes || out_cap > 2ull * c->opt.max_resp_bytes || msg_cap > c->opt.max_msgs || replies_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
     int rc = h2_ensure(c); if (rc != B2_OK) return rc;
     CU(cudaSetDevice(c->opt.device));
     static_assert(sizeof(RingSlotHdr) + sizeof(H2RingArgs) <= 256, "h2 ring slot header");
-    // [RingSlotHdr | args | runs | staged input | statuses | msgs | spans | out | replies]
+    // [RingSlotHdr | args | runs | staged input | (host-reply block) | statuses | msgs | spans | out | replies | (reply lengths | frames)]
     const uint64_t runs = (uint64_t)c->opt.max_runs;
     SlotLayout L;
     H2RingDev& H = c->h2r_dev;
     H.off_args = sizeof(RingSlotHdr);
     c->ring_dev.off_runs = L.add(runs * sizeof(b2_run));
     c->ring_dev.off_in = L.add((uint64_t)max_bytes + 16);
+    H2TurnDev& Q = c->h2t_dev;
+    if (max_resps) Q.off_resps = L.add(h2r_turn_block(max_resps, max_resps));
     H.off_rs = L.add(runs * sizeof(b2_h2_run_status));
     H.off_msgs = L.add((uint64_t)msg_cap * sizeof(b2_h2_msg));
     H.off_spans = L.add(runs * sizeof(b2_h2_reply_span));
     H.off_out = L.add((uint64_t)out_cap + 16);
     H.off_replies = L.add((uint64_t)replies_cap + 16);
+    if (max_resps) {
+        Q.off_resp_lens = L.add(max_resps * 4ull);
+        Q.off_resp_out = L.add((uint64_t)resp_out_cap + 16);
+        // the device scratch: [block | lengths | frames]
+        const uint64_t block = h2r_turn_block(max_resps, max_resps), lens = (max_resps * 4ull + 15u) & ~15ull;
+        if (cudaMalloc((void**)&Q.turn, block + lens + resp_out_cap + 16) != cudaSuccess) { cudaGetLastError(); set_err("cudaMalloc of the turn's reply scratch failed"); return B2_E_NOMEM; }
+        Q.turn_lens = reinterpret_cast<uint32_t*>(Q.turn + block); Q.turn_out = Q.turn + block + lens;
+    }
     rc = ring_alloc(c, L.end); if (rc != B2_OK) return rc;
-    CU(cudaFuncSetAttribute(k_h2_ring, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kH2RingSmem));
+    if (max_resps) CU(cudaFuncSetAttribute(k_h2_ring<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kH2RingSmem));
+    else CU(cudaFuncSetAttribute(k_h2_ring<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kH2RingSmem));
     c->h2r_max_bytes = max_bytes; c->h2r_msg_cap = msg_cap; c->h2r_out_cap = out_cap; c->h2r_replies_cap = replies_cap;
+    c->h2r_max_resps = max_resps; c->h2r_resp_out_cap = resp_out_cap;
     c->ring_kind = RingKind::h2_server;
     return B2_OK;
+}
+extern "C" int b2_h2_ring_enable(b2_ctx* c, uint32_t max_bytes, uint32_t msg_cap, uint32_t out_cap, uint32_t replies_cap) {
+    if (!c) { set_err("null argument"); return B2_E_INVAL; }
+    return h2_ring_setup(c, "b2_h2_ring_enable", max_bytes, msg_cap, out_cap, replies_cap, 0, 0);
 }
 extern "C" int b2_h2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs, uint32_t* ticket) {
     if (!c || !bytes || !runs || !ticket || n_runs == 0) { set_err("null argument"); return B2_E_INVAL; }
@@ -2250,20 +2281,18 @@ extern "C" int b2_h2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, 
     if (!h2_runs_ok(c, runs, n_runs, nbytes)) return B2_E_INVAL;
     const H2Split sp = h2_split(c->h2r_out_cap, c->h2r_msg_cap, c->h2r_replies_cap, n_runs);
     if (!sp.fits) { set_err("out_cap / msg_cap too small for the number of runs"); return B2_E_CAPACITY; }
-    const H2RingArgs a = { sp.per_run, sp.region, sp.reply_region, h2_gz_wanted(c, runs, n_runs) ? 1u : 0u };
+    const H2RingArgs a = { sp.per_run, sp.region, sp.reply_region, h2_gz_wanted(c, runs, n_runs) ? 1u : 0u, 0, 0, { 0, 0 } };
     uint8_t* slot = ring_claim(c, "b2_h2_ring_wait");
     if (!slot) return B2_E_CAPACITY;
     RingSlotHdr* h = ring_fill(c, slot, bytes, nbytes, runs, n_runs);
     memcpy(slot + c->h2r_dev.off_args, &a, sizeof a);
     return ring_ring(c, h, bytes, ticket);
 }
-extern "C" int b2_h2_ring_wait(b2_ctx* c, uint32_t ticket, b2_h2_ring_result* out) {
-    static_assert(sizeof(b2_h2_ring_result) == 64, "h2 ring result ABI layout");
-    int rc;
-    const uint8_t* slot = ring_collect(c, c && out && c->ring_kind == RingKind::h2_server, ticket, "bad h2 ring ticket", rc);
-    if (!slot) return rc;
+// the served half of a collected k_h2_ring ticket
+static void h2_ring_result(b2_ctx* c, uint32_t ticket, const uint8_t* slot, b2_h2_ring_result* out) {
     const RingSlotHdr* h = reinterpret_cast<const RingSlotHdr*>(slot);
     const H2RingDev& L = c->h2r_dev;
+    const H2RingArgs* a = reinterpret_cast<const H2RingArgs*>(slot + L.off_args);
     const uint32_t n_runs = h->n_runs;
     const b2_h2_run_status* rs = reinterpret_cast<const b2_h2_run_status*>(slot + L.off_rs);
     uint32_t n_msgs = 0;
@@ -2271,11 +2300,76 @@ extern "C" int b2_h2_ring_wait(b2_ctx* c, uint32_t ticket, b2_h2_ring_result* ou
     memset(out, 0, sizeof *out);
     out->runs = rs; out->n_runs = n_runs; out->n_msgs = n_msgs;
     out->msgs = reinterpret_cast<const b2_h2_msg*>(slot + L.off_msgs);
-    out->out = slot + L.off_out; out->region = h2_split(c->h2r_out_cap, c->h2r_msg_cap, c->h2r_replies_cap, n_runs).region;
+    out->out = slot + L.off_out; out->region = a->region;     // (h2_split's, as the submission placed it; 0 on a turn without runs)
     out->replies = slot + L.off_replies; out->spans = reinterpret_cast<const b2_h2_reply_span*>(slot + L.off_spans);
     if (n_msgs > c->h2r_msg_cap) { out->n_msgs = 0; out->status = B2_E_CAPACITY; }
     // the most recent ticket's input and out regions stay on the device: b2_h2_pack_responses may take bodies and content-types from them
     if (ticket + 1 == c->ring_next) { c->h2_last_in = h->nbytes; c->h2_last_out = (uint64_t)out->region * n_runs; }
+}
+extern "C" int b2_h2_ring_wait(b2_ctx* c, uint32_t ticket, b2_h2_ring_result* out) {
+    static_assert(sizeof(b2_h2_ring_result) == 64, "h2 ring result ABI layout");
+    int rc;
+    const uint8_t* slot = ring_collect(c, c && out && c->ring_kind == RingKind::h2_server, ticket, "bad h2 ring ticket", rc);
+    if (!slot) return rc;
+    h2_ring_result(c, ticket, slot, out);
+    return B2_OK;
+}
+
+// ---- a gRPC server's turn on the latency path: k_h2_ring with the host-reply phase (include/b2rpc.h, b2_h2_ring_turn_enable) ----------
+extern "C" int b2_h2_ring_turn_enable(b2_ctx* c, uint32_t max_bytes, uint32_t msg_cap, uint32_t out_cap, uint32_t replies_cap,
+                                      uint32_t max_resps, uint32_t resp_out_cap) {
+    if (!c) { set_err("null argument"); return B2_E_INVAL; }
+    if (max_resps == 0 || resp_out_cap == 0) { set_err("capacities must be non-zero"); return B2_E_INVAL; }
+    // the limits of b2_h2_pack_responses, which reads the ticket's bytes
+    if (max_bytes > c->opt.max_resp_bytes || max_resps > c->opt.max_msgs || resp_out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    return h2_ring_setup(c, "b2_h2_ring_turn_enable", max_bytes, msg_cap, out_cap, replies_cap, max_resps, resp_out_cap);
+}
+extern "C" int b2_h2_ring_turn_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
+                                      const b2_h2_response* resps, uint32_t n_resps, uint32_t* ticket) {
+    if (!c || !bytes || !ticket || (!runs && n_runs) || (!resps && n_resps)) { set_err("null argument"); return B2_E_INVAL; }
+    if (n_runs == 0 && n_resps == 0) { set_err("a turn carries runs, host replies or both"); return B2_E_INVAL; }
+    if (c->ring_kind != RingKind::h2_server || !c->h2r_max_resps) { set_err("b2_h2_ring_turn_enable first"); return B2_E_INVAL; }
+    // the checks of b2_h2_ring_submit for the runs, then those of b2_h2_pack_responses for the replies, with the enable-time caps
+    if (nbytes > c->h2r_max_bytes) { set_err("turn larger than b2_h2_ring_turn_enable's max_bytes: use the batch calls"); return B2_E_CAPACITY; }
+    if (n_runs > c->opt.max_runs || n_resps > c->h2r_max_resps) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    H2Split sp = { 0, 0, 0, true };
+    if (n_runs) {
+        if (!h2_runs_ok(c, runs, n_runs, nbytes)) return B2_E_INVAL;
+        sp = h2_split(c->h2r_out_cap, c->h2r_msg_cap, c->h2r_replies_cap, n_runs);
+        if (!sp.fits) { set_err("out_cap / msg_cap too small for the number of runs"); return B2_E_CAPACITY; }
+    }
+    // the zero-copy sources are the previous ticket's device buffers, which this ticket's pull overwrites
+    for (uint32_t i = 0; i < n_resps; i++)
+        if (resps[i].flags & (B2_H2_RESP_BODY_IN_INPUT | B2_H2_RESP_BODY_IN_OUT | B2_H2_RESP_CT_IN_OUT)) { set_err("a turn's replies index its own bytes: no zero-copy flags"); return B2_E_INVAL; }
+    std::vector<uint32_t> first, offs(n_resps);
+    uint64_t total = 0;
+    if (n_resps) { int rc = h2_place_responses(c, nbytes, resps, n_resps, c->h2r_resp_out_cap, offs.data(), first, total); if (rc != B2_OK) return rc; }
+    uint8_t* slot = ring_claim(c, "b2_h2_ring_turn_wait");
+    if (!slot) return B2_E_CAPACITY;
+    const uint32_t n_groups = n_resps ? (uint32_t)first.size() - 1 : 0u;
+    const H2RingArgs a = { sp.per_run, sp.region, sp.reply_region, n_runs && h2_gz_wanted(c, runs, n_runs) ? 1u : 0u, n_resps, n_groups, { 0, 0 } };
+    RingSlotHdr* h = ring_fill(c, slot, bytes, nbytes, runs, n_runs);
+    uint8_t* block = slot + c->h2t_dev.off_resps;                 // the host-reply block the kernel pulls: records, placed offsets, group_first
+    if (n_resps) {
+        memcpy(block, resps, sizeof(b2_h2_response) * (size_t)n_resps);
+        memcpy(block + h2r_turn_offs_off(n_resps), offs.data(), 4 * (size_t)n_resps);
+        memcpy(block + h2r_turn_first_off(n_resps), first.data(), 4 * first.size());
+    }
+    memcpy(slot + c->h2r_dev.off_args, &a, sizeof a);
+    return ring_ring(c, h, bytes, ticket);
+}
+extern "C" int b2_h2_ring_turn_wait(b2_ctx* c, uint32_t ticket, b2_h2_ring_turn_result* out) {
+    static_assert(sizeof(b2_h2_ring_turn_result) == 96, "h2 ring turn result ABI layout");
+    int rc;
+    const uint8_t* slot = ring_collect(c, c && out && c->ring_kind == RingKind::h2_server && c->h2r_max_resps, ticket, "bad h2 ring turn ticket", rc);
+    if (!slot) return rc;
+    memset(out, 0, sizeof *out);
+    h2_ring_result(c, ticket, slot, &out->ring);
+    const H2TurnDev& Q = c->h2t_dev;
+    out->n_resps = reinterpret_cast<const H2RingArgs*>(slot + c->h2r_dev.off_args)->n_resps;
+    out->resp_offs = reinterpret_cast<const uint32_t*>(slot + Q.off_resps + h2r_turn_offs_off(out->n_resps));
+    out->resp_lens = reinterpret_cast<const uint32_t*>(slot + Q.off_resp_lens);
+    out->resp_out = slot + Q.off_resp_out;
     return B2_OK;
 }
 

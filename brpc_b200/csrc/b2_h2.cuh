@@ -1749,7 +1749,16 @@ __device__ __forceinline__ void h2_ring_push_run(uint32_t r, uint32_t lane, uint
 // __syncthreads() where the batch call has kernel boundaries, on the same device scratch, then only the used parts are pushed into the
 // ticket's slot.  H2Conn, HpackState and the stream pool are read through L1: every call that writes them from another kernel retires
 // this one first (ring_halt), so a launch boundary lies between their writes and this CTA's loads.
-struct H2RingArgs { uint32_t per_run, region, reply_region, gunzip; };   // per ticket, from the host, at the slot's off_args
+// A turn (b2_h2_ring_turn_*) also carries the replies the host produced: after the served replies, b2_h2_pack_responses over them as
+// one more block phase, so that they take the encoder table and windows the served replies left.  Their block (records, the offsets the
+// host placed, group_first) is pulled into scratch of its own (turn), which also holds their lengths and frames; only out_len bytes of
+// each frame are pushed.  The phase is k_h2_ring<true>'s (b2_h2_ring_turn_enable): k_h2_ring<false> is the kernel without it, so that
+// contexts without turns keep its registers, stack and spills as they were.
+struct H2RingArgs { uint32_t per_run, region, reply_region, gunzip, n_resps, n_groups, pad[2]; };   // per ticket, from the host, at the slot's off_args
+// the host-reply block of a turn: n records, their placed offsets, then group_first (n_groups + 1 words); all parts 16-byte aligned
+B2_HD uint32_t h2r_turn_offs_off(uint32_t n) { return n * (uint32_t)sizeof(b2_h2_response); }
+B2_HD uint32_t h2r_turn_first_off(uint32_t n) { return h2r_turn_offs_off(n) + ((n * 4 + 15u) & ~15u); }
+B2_HD uint32_t h2r_turn_block(uint32_t n, uint32_t n_groups) { return h2r_turn_first_off(n) + (((n_groups + 1) * 4 + 15u) & ~15u); }
 struct H2RingDev {
     uint32_t off_args, off_rs, off_msgs, off_spans, off_out, off_replies;  // the slot's parts behind RingSlotHdr (runs, staged input: RingDev)
     H2Conn* conns; HpackState* hps; const DevMethod* methods; uint32_t n_methods; H2ServeCfg cfg; H2Pool pool;
@@ -1760,14 +1769,28 @@ struct H2RingDev {
     b2_h2_response* strided; uint32_t* strided_offs; b2_h2_response* list; uint32_t* list_offs; uint32_t* first;
     b2_h2_reply_span* spans; uint8_t* replies;
 };
+// k_h2_ring<true>'s own parts (a parameter of their own, so that k_h2_ring<false> keeps H2RingDev's size and stack): the slot's
+// host-reply block, lengths and frames, and the device scratch they are pulled into and packed in
+struct H2TurnDev {
+    uint32_t off_resps, off_resp_lens, off_resp_out;
+    uint8_t* turn; uint32_t* turn_lens; uint8_t* turn_out;
+};
 constexpr uint32_t kH2RingSmem = kSmallWarps * 3 * kH2FragCap;          // k_h2_pack's scratch for each warp
-__global__ void __launch_bounds__(kSmallThreads, 1) k_h2_ring(RingDev R, H2RingDev H) {
+template <bool kReplies>
+__global__ void __launch_bounds__(kSmallThreads, 1) k_h2_ring(RingDev R, H2RingDev H, H2TurnDev Q) {
     extern __shared__ __align__(16) uint8_t h2_ring_raw[];
     const uint32_t tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const uint8_t* bytes = R.d_bytes;
     const b2_run* runs = reinterpret_cast<const b2_run*>(R.d_meta);
     ring_serve<H2RingArgs>(R, H.off_args, [] {}, [&](uint8_t* slot, const RingSlotHdr& s_hdr, const H2RingArgs& s_args, unsigned long long (&t)[4]) __attribute__((always_inline)) {
         const uint32_t n_runs = s_hdr.n_runs, per_run = s_args.per_run, region = s_args.region, reply_region = s_args.reply_region, n_slots = n_runs * per_run;
+        if constexpr (kReplies) {
+            if (s_args.n_resps) {   // the host-reply block, while the serve passes below run (they never touch it)
+                const uint4* src = reinterpret_cast<const uint4*>(slot + Q.off_resps);
+                uint4* dst = reinterpret_cast<uint4*>(Q.turn);
+                for (uint32_t k = tid; k < h2r_turn_block(s_args.n_resps, s_args.n_groups) / 16u; k += kSmallThreads) dst[k] = src[k];
+            }
+        }
         for (uint32_t r = tid; r < n_runs; r += kSmallThreads)
             h2_consume_run<false>(r, bytes, runs, H.conns, H.hps, H.methods, H.n_methods, H.rs, H.msgs, per_run, H.out, region, H.pool);
         __syncthreads();
@@ -1784,6 +1807,16 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_h2_ring(RingDev R, H2RingD
         __syncthreads();
         for (uint32_t r = wid; r < n_runs; r += kSmallWarps) h2_gather_run(r, lane, H.first, H.list_offs, H.gz, H.replies, H.spans);
         __syncthreads();
+        if constexpr (kReplies) {
+            if (s_args.n_resps) {   // the host's replies, framed against the encoder tables and windows the served replies just moved
+                const uint32_t n_resps = s_args.n_resps;
+                for (uint32_t g = wid; g < s_args.n_groups; g += kSmallWarps)
+                    h2_pack_group(g, lane, h2_ring_raw + wid * 3 * kH2FragCap, bytes, nullptr, nullptr, reinterpret_cast<const b2_h2_response*>(Q.turn),
+                                  reinterpret_cast<const uint32_t*>(Q.turn + h2r_turn_first_off(n_resps)), H.conns, Q.turn_out,
+                                  reinterpret_cast<const uint32_t*>(Q.turn + h2r_turn_offs_off(n_resps)), Q.turn_lens);
+                __syncthreads();
+            }
+        }
         if (tid == 0) t[3] = globaltimer_ns();                          // replies packed
         // the descriptors become one list in run order (the batch call compacts them on the host): first[r] = run r's first list index
         if (wid == 0) h2_warp_scan_runs(n_runs, lane, [&](uint32_t r) { return H.rs[r].n_msgs; }, H.first);
@@ -1794,6 +1827,14 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_h2_ring(RingDev R, H2RingD
             h2_ring_push_run(r, lane, slot, H.off_rs, H.off_msgs, H.off_out, H.rs, H.msgs, per_run, H.out, region, H.first);
             ring_push(slot + H.off_replies + sp.off, H.replies + sp.off, sp.len, lane, 32);
             if (lane == 0) reinterpret_cast<b2_h2_reply_span*>(slot + H.off_spans)[r] = sp;
+        }
+        if constexpr (kReplies) {
+            if (s_args.n_resps) {   // the host replies' lengths, then a warp per reply its frames
+                const uint32_t n_resps = s_args.n_resps;
+                const uint32_t* offs = reinterpret_cast<const uint32_t*>(Q.turn + h2r_turn_offs_off(n_resps));
+                ring_push(slot + Q.off_resp_lens, reinterpret_cast<const uint8_t*>(Q.turn_lens), n_resps * 4u, tid, kSmallThreads);
+                for (uint32_t i = wid; i < n_resps; i += kSmallWarps) ring_push(slot + Q.off_resp_out + offs[i], Q.turn_out + offs[i], __ldcg(Q.turn_lens + i), lane, 32);
+            }
         }
         return false;
     });

@@ -864,6 +864,43 @@ typedef struct b2_h2_ring_result {    /* views into the ticket's pinned slot, va
 int  b2_h2_ring_enable(b2_ctx* ctx, uint32_t max_bytes, uint32_t msg_cap, uint32_t out_cap, uint32_t replies_cap);
 int  b2_h2_ring_submit(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs, uint32_t* ticket);
 int  b2_h2_ring_wait(b2_ctx* ctx, uint32_t ticket, b2_h2_ring_result* out);
+/* A gRPC server's TURN on the latency path: one ticket of k_h2_ring that serves what arrived, exactly as b2_h2_serve_batch, and then sends
+ * the replies user code produced for earlier calls, exactly as b2_h2_pack_responses — with no relaunch, launch, copy or stream
+ * synchronisation for the host's replies.  (b2_h2_pack_responses between tickets still works, and still retires the resident kernel.)
+ * Inside a turn the order is read, then write: a SETTINGS or WINDOW_UPDATE in the runs governs how that turn's host replies are framed and
+ * charged (max_frame_size, header_table_size 0 = never-indexed, a connection window that no longer covers a body gives
+ * RST_STREAM(FLOW_CONTROL_ERROR)), and the turn's device-answered replies take the HPACK encoder before the host's.  Per connection write
+ * its run's control bytes (ctrl_off / ctrl_len), then its device replies (spans[i]), then its host replies in record order.
+ * b2_h2_ring_turn_enable: everything b2_h2_ring_enable does, with the same rules and caps; max_resps and resp_out_cap are per turn and play
+ * the roles of b2_h2_pack_responses' n and out_cap (max_resps <= max_msgs, resp_out_cap and max_bytes <= max_resp_bytes, else
+ * B2_E_CAPACITY).  They add the host-reply parts to each slot and device scratch of their own.
+ * b2_h2_ring_turn_submit: the checks of b2_h2_ring_submit when n_runs > 0, then every check of b2_h2_pack_responses on the replies with the
+ * turn's caps: the connection in range, replies of one connection adjacent, fields inside `bytes`, content-type <= 256 and grpc-message
+ * <= 512 bytes (B2_E_INVAL), n_resps <= max_resps and room by h2_reply_bound within resp_out_cap (B2_E_CAPACITY).  The records are
+ * b2_h2_response, unchanged; their fields index the turn's own bytes, the same buffer as the runs.  B2_H2_RESP_BODY_IN_INPUT,
+ * _BODY_IN_OUT and _CT_IN_OUT are refused (B2_E_INVAL): they name the previous ticket's device buffers, which this ticket's pull
+ * overwrites.  A turn carries runs, replies or both, not neither (B2_E_INVAL); a reply-only turn sends replies without waiting for the next
+ * read.
+ * b2_h2_ring_turn_wait: tickets may be waited in any order.  For any sequence of turns the results equal, byte for byte, what a context
+ * returns for the same sequence of b2_h2_serve_batch(bytes, runs, ...) + b2_h2_pack_responses(bytes, resps, ...) with the same caps (a
+ * call whose list is empty skipped): `ring` as b2_h2_ring_wait fills it (ring.status B2_E_CAPACITY when the served half would fail; the
+ * host replies are packed all the same, as the two calls in a row would), each reply's frame bytes and length — and so does the
+ * connection state left behind (both HPACK tables, the windows, the deferred WINDOW_UPDATE, the stream pool).  After the wait of the most
+ * recent ticket, b2_h2_pack_responses resolves the zero-copy flags against it as after b2_h2_ring_wait.
+ * On a turn-enabled context b2_h2_ring_submit / _wait still serve tickets without replies; the turn calls on a b2_h2_ring_enable context
+ * fail with B2_E_INVAL.  Every refusal and retirement rule of b2_h2_ring_wait above applies.  Compressed replies stay with the batch calls. */
+typedef struct b2_h2_ring_turn_result {  /* views into the ticket's pinned slot, valid until the slot is reused by the 8th later submission */
+    b2_h2_ring_result ring;              /* the served half, as b2_h2_ring_wait returns it */
+    uint32_t n_resps, reserved;
+    const uint32_t* resp_offs;           /* host reply i: resp_out[resp_offs[i], + resp_lens[i]) */
+    const uint32_t* resp_lens;
+    const uint8_t* resp_out;
+} b2_h2_ring_turn_result;                /* 96 bytes */
+int  b2_h2_ring_turn_enable(b2_ctx* ctx, uint32_t max_bytes, uint32_t msg_cap, uint32_t out_cap, uint32_t replies_cap,
+                            uint32_t max_resps, uint32_t resp_out_cap);
+int  b2_h2_ring_turn_submit(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
+                            const b2_h2_response* resps, uint32_t n_resps, uint32_t* ticket);
+int  b2_h2_ring_turn_wait(b2_ctx* ctx, uint32_t ticket, b2_h2_ring_turn_result* out);
 /* h2/gRPC CLIENT connections on the latency path: b2_h2_client_process_batch followed by b2_h2_pack_requests inside a resident kernel
  * (k_h2_client_ring) fed through the same submit ring.  A ticket is one turn of a client's event loop: read what arrived, then send what
  * is queued.  The runs (the bytes read from client sockets, socket_id = connection) are parsed as by b2_h2_client_process_batch, then the
