@@ -124,6 +124,14 @@ class ClientRingResult(C.Structure):
 assert C.sizeof(ClientRingResult) == 104
 
 
+class RingTurnResult(C.Structure):
+    _fields_ = [("batch", BatchResult), ("n_replies", C.c_uint32), ("reserved", C.c_uint32), ("reply_offs", C.c_void_p), ("reply_lens", C.c_void_p),
+                ("reply_out", C.c_void_p)]
+
+
+assert C.sizeof(RingTurnResult) == 104
+
+
 class StreamRingResult(C.Structure):
     _fields_ = [("batch", BatchResult), ("n_writes", C.c_uint32), ("out_bytes", C.c_uint32), ("results", C.c_void_p), ("out", C.c_void_p)]
 
@@ -237,6 +245,9 @@ def _load():
     l.b2_client_ring_enable.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]
     l.b2_client_ring_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
     l.b2_client_ring_wait.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(ClientRingResult)]
+    l.b2_ring_turn_enable.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]
+    l.b2_ring_turn_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
+    l.b2_ring_turn_wait.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(RingTurnResult)]
     l.b2_h2_pack_responses.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     l.b2_pack_requests.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     l.b2_pack_responses.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
@@ -269,7 +280,8 @@ ABI_SYMBOLS = ["b2_ctx_create", "b2_ctx_destroy", "b2_last_error", "b2_version",
                "b2_h2_serve_batch", "b2_stream_configure", "b2_stream_open", "b2_stream_set_connected", "b2_stream_close", "b2_stream_query",
                "b2_stream_take_pending", "b2_stream_results", "b2_stream_write", "b2_stream_ring_enable", "b2_h2_ring_enable", "b2_h2_ring_submit",
                "b2_h2_ring_wait", "b2_h2_ring_turn_enable", "b2_h2_ring_turn_submit", "b2_h2_ring_turn_wait", "b2_h2_client_ring_enable", "b2_h2_client_ring_submit", "b2_h2_client_ring_wait", "b2_client_ring_enable",
-               "b2_client_ring_submit", "b2_client_ring_wait", "b2_stream_ring_write_enable", "b2_stream_ring_submit", "b2_stream_ring_wait"]
+               "b2_client_ring_submit", "b2_client_ring_wait", "b2_ring_turn_enable", "b2_ring_turn_submit", "b2_ring_turn_wait",
+               "b2_stream_ring_write_enable", "b2_stream_ring_submit", "b2_stream_ring_wait"]
 
 ECHO_METHOD = dict(service_full_name=b"example.EchoService", service_name=b"EchoService", method_name=b"Echo",
                    request_type_name=b"example.EchoRequest", handler=1, echo_attachment=1,
@@ -891,6 +903,32 @@ class Context:
         rs, msgs, resp = self._views(res.batch)
         offs, lens = _view(res.req_offs, 4 * res.n_reqs, np.uint32), _view(res.req_lens, 4 * res.n_reqs, np.uint32)
         frames = [C.string_at(res.req_out + int(o), int(n)) if n else b"" for o, n in zip(offs, lens)]
+        return rs, msgs, resp, self._info(res.batch), frames
+
+    # ---- baidu_std server turns on the latency path (b2_ring_turn_*) ----
+    def ring_turn_enable(self, max_bytes, max_resps, resp_out_cap):
+        """Serve server turns on the resident k_ring<RingBody::replies> with these per-turn caps (b2_ring_turn_enable): before the first ring call."""
+        _check(lib.b2_ring_turn_enable(self._h, max_bytes, max_resps, resp_out_cap))
+
+    def ring_turn_submit(self, data, runs, replies, ptr=None, nbytes=None):
+        """One turn of a server's event loop: runs (RUN_DT) are served as by ring_submit, then replies (REPLY_DT, the replies the host
+        produced, offsets into the same data) are packed as by pack_responses.  Either list may be empty, not both.  Returns the ticket."""
+        runs = np.ascontiguousarray(runs, dtype=RUN_DT); replies = np.ascontiguousarray(replies, dtype=REPLY_DT)
+        ptr, nbytes = self._ring_bytes(data, ptr, nbytes)
+        t = C.c_uint32(0)
+        _check(lib.b2_ring_turn_submit(self._h, ptr, nbytes, runs.ctypes.data if len(runs) else None, len(runs),
+                                       replies.ctypes.data if len(replies) else None, len(replies), C.byref(t)))
+        return t.value
+
+    def ring_turn_wait(self, ticket):
+        """ring_wait's (run_status, msgs, resp, info) of the turn's runs, then the frame of every reply (b"" where it was not packed, as
+        pack_responses returns them).  The first three are views of the ticket's pinned slot, valid until the 8th later submission; the
+        frames are copies."""
+        res = RingTurnResult()
+        _check(lib.b2_ring_turn_wait(self._h, ticket, C.byref(res)))
+        rs, msgs, resp = self._views(res.batch)
+        offs, lens = _view(res.reply_offs, 4 * res.n_replies, np.uint32), _view(res.reply_lens, 4 * res.n_replies, np.uint32)
+        frames = [C.string_at(res.reply_out + int(o), int(n)) if n else b"" for o, n in zip(offs, lens)]
         return rs, msgs, resp, self._info(res.batch), frames
 
     # ---- a Stream producer's turn on the latency path (b2_stream_ring_*) ----

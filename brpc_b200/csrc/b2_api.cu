@@ -47,9 +47,11 @@ constexpr uint32_t kSecEvents = 64, kSecMsgs = kSecEvents + kSmallMsgs * 80, kSe
 struct Stage { const char* name; cudaEvent_t ev; };
 // Which resident kernel a context's ring runs, fixed by its first ring call: k_ring (b2_ring_start / b2_ring_submit), k_ring with the
 // stream pass (b2_stream_ring_enable), k_ring<RingBody::stream_writes> with the stream pass and the write pass (b2_stream_ring_write_enable),
-// k_ring<RingBody::requests> with the request phase (b2_client_ring_enable), k_h2_ring (b2_h2_ring_enable) or k_h2_client_ring
-// (b2_h2_client_ring_enable)
-enum class RingKind { none, batch, batch_streams, batch_stream_writes, batch_client, h2_server, h2_client };
+// k_ring<RingBody::requests> with the request phase (b2_client_ring_enable), k_ring<RingBody::replies> with the reply phase
+// (b2_ring_turn_enable), k_h2_ring (b2_h2_ring_enable) or k_h2_client_ring (b2_h2_client_ring_enable)
+enum class RingKind { none, batch, batch_streams, batch_stream_writes, batch_client, batch_replies, h2_server, h2_client };
+// The kinds whose tickets pack records after the runs (k_ring<RingBody::requests> / <RingBody::replies>)
+bool ring_packs(RingKind k) { return k == RingKind::batch_client || k == RingKind::batch_replies; }
 // The kinds whose tickets run the stream pass: the table belongs to an outstanding ticket, tickets are collected in ticket order, the
 // kernel parks behind a ticket that overflows the compact block, and the slot carries a stream section
 bool ring_runs_streams(RingKind k) { return k == RingKind::batch_streams || k == RingKind::batch_stream_writes; }
@@ -75,7 +77,7 @@ struct b2_ctx {
     std::vector<uint8_t> h2_gunzip; uint8_t* d_h2_gz_merge = nullptr;     // host mirror of the kH2Gunzip bits; merge scratch, B2_H2_HEADER_BYTES per run
     // persistent latency kernel (b2_ring_*): pinned + mapped submit ring, its own stream.  ring_slots: allocated (by the first ring call
     // that needs them); the slot parts of each kind live in that kind's kernel arguments (ring_dev: runs, staged input, output, stream section)
-    RingKind ring_kind = RingKind::none; RingDev ring_dev = {}; ClientRingDev cr_dev = {}; H2RingDev h2r_dev = {}; H2ClientRingDev h2c_dev = {};
+    RingKind ring_kind = RingKind::none; RingDev ring_dev = {}; PackRingDev pr_dev = {}; H2RingDev h2r_dev = {}; H2ClientRingDev h2c_dev = {};
     uint8_t* ring_slots = nullptr; volatile uint32_t* ring_ctl = nullptr; uint32_t* d_ring_ticket = nullptr; cudaStream_t ring_stream = nullptr;
     uint32_t ring_next = 1, ring_stride = 0; bool ring_collected[8] = { true, true, true, true, true, true, true, true };
     const void* ring_bytes[8] = {}; const void* ring_pin_base = nullptr; unsigned long long ring_pin_dev = 0; uint64_t ring_launches = 0;
@@ -87,7 +89,7 @@ struct b2_ctx {
     uint32_t h2r_max_bytes = 0, h2r_msg_cap = 0, h2r_out_cap = 0, h2r_replies_cap = 0;
     uint32_t h2r_max_resps = 0, h2r_resp_out_cap = 0; H2TurnDev h2t_dev = {};   // ... and the host replies of a turn (b2_h2_ring_turn_enable)
     uint32_t h2c_max_bytes = 0, h2c_call_cap = 0, h2c_out_cap = 0, h2c_max_reqs = 0, h2c_req_out_cap = 0;
-    uint32_t cr_max_bytes = 0, cr_max_reqs = 0, cr_req_out_cap = 0;        // ... and of the client ring (k_ring<RingBody::requests>)
+    uint32_t pr_max_bytes = 0, pr_max_recs = 0, pr_out_cap = 0;            // ... and of the client ring or the turn ring (ring_packs)
     // the stream write ring (k_ring<RingBody::stream_writes>): its caps, its slot parts and the write pass's device scratch (d_swr)
     uint32_t swr_max_bytes = 0, swr_max_writes = 0, swr_out_cap = 0; SwRingDev swr_dev = {}; uint8_t* d_swr = nullptr;
     ulonglong2* d_iov = nullptr; b2_iovec* h_iov = nullptr; const void* host_bytes = nullptr;      // B2_RESP_IOVEC
@@ -205,20 +207,22 @@ static void ring_halt(b2_ctx* c);
 static void stream_free(b2_ctx* c);
 static bool ring_busy(const b2_ctx* c) { for (uint32_t k = 0; k < kRingSlots; k++) if (!c->ring_collected[k]) return true; return false; }
 static uint8_t* ring_slot(const b2_ctx* c, uint32_t ticket) { return c->ring_slots + (size_t)(ticket % kRingSlots) * c->ring_stride; }
-// Every call that uploads to the context or touches h2 state is refused while a ticket of an h2 ring (k_h2_ring or k_h2_client_ring) or
-// of the client ring (k_ring<RingBody::requests>) is outstanding: the ticket uses the same device scratch and connection state.  A call that writes h2
+// Every call that uploads to the context or touches h2 state is refused while a ticket of an h2 ring (k_h2_ring or k_h2_client_ring), of
+// the client ring (k_ring<RingBody::requests>) or of the turn ring (k_ring<RingBody::replies>) is outstanding: the ticket uses the same
+// device scratch and connection state.  A call that writes h2
 // connection state also retires an h2 ring's resident kernel first: that CTA reads the state through L1, and a launch boundary is where
 // L1 is known not to hold lines another kernel wrote since.
 static bool ring_refuses(b2_ctx* c, bool writes_h2_state) {
     const RingKind k = c->ring_kind;
-    if (k != RingKind::h2_server && k != RingKind::h2_client && k != RingKind::batch_client) return false;
+    if (k != RingKind::h2_server && k != RingKind::h2_client && !ring_packs(k)) return false;
     if (ring_busy(c)) {
         set_err(k == RingKind::h2_server ? "an h2 ring ticket is outstanding: b2_h2_ring_wait it first" :
                 k == RingKind::h2_client ? "an h2 client ring ticket is outstanding: b2_h2_client_ring_wait it first" :
-                                           "a client ring ticket is outstanding: b2_client_ring_wait it first");
+                k == RingKind::batch_client ? "a client ring ticket is outstanding: b2_client_ring_wait it first" :
+                                              "a ring turn is outstanding: b2_ring_turn_wait it first");
         return true;
     }
-    if (writes_h2_state && k != RingKind::batch_client) ring_halt(c);
+    if (writes_h2_state && !ring_packs(k)) ring_halt(c);
     return false;
 }
 extern "C" void b2_ctx_destroy(b2_ctx* c) {
@@ -1232,21 +1236,23 @@ static int ring_launch(b2_ctx* c) {
         break;
     }
     case RingKind::h2_client: { const H2ClientRingDev H = h2_client_ring_dev(c); k_h2_client_ring<<<1, kSmallThreads, kH2ClientRingSmem, c->ring_stream>>>(R, H); break; }
-    default: {                              // batch, batch_streams, batch_stream_writes, batch_client
+    default: {                              // batch, batch_streams, batch_stream_writes, batch_client, batch_replies
         const bool was_small = c->small; c->small = false;
         BatchPtrs B = make_ptrs(c);
         c->small = was_small;
         B.bytes = c->d_bytes;
         const StreamPass SP = ring_runs_streams(c->ring_kind) ? c->sp_ring : StreamPass{};   // (tab null: the ring runs no stream pass)
-        if (c->ring_kind == RingKind::batch_client) {
-            // the scratch of b2_pack_requests, except that the requests and their offsets go to d_msgs / d_refs, which k_ring leaves alone
-            ClientRingDev Q = c->cr_dev;
-            Q.reqs = reinterpret_cast<ReqDesc*>(c->d_msgs); Q.offs = reinterpret_cast<uint32_t*>(c->d_refs); Q.lens = Q.offs + c->opt.max_msgs;
+        if (ring_packs(c->ring_kind)) {
+            // the scratch of b2_pack_requests / b2_pack_responses, except that the records and their offsets go to d_msgs / d_refs, which
+            // k_ring leaves alone
+            PackRingDev Q = c->pr_dev;
+            Q.recs = reinterpret_cast<uint8_t*>(c->d_msgs); Q.offs = reinterpret_cast<uint32_t*>(c->d_refs); Q.lens = Q.offs + c->opt.max_msgs;
             Q.scratch = c->d_unz; Q.out = c->d_resp;
-            k_ring<RingBody::requests><<<1, kSmallThreads, sizeof(SmallSmem), c->ring_stream>>>(R, B, c->cfg, SP, Q);
+            if (c->ring_kind == RingKind::batch_client) k_ring<RingBody::requests><<<1, kSmallThreads, sizeof(SmallSmem), c->ring_stream>>>(R, B, c->cfg, SP, Q);
+            else k_ring<RingBody::replies><<<1, kSmallThreads, sizeof(SmallSmem), c->ring_stream>>>(R, B, c->cfg, SP, Q);
         } else if (c->ring_kind == RingKind::batch_stream_writes) {
             k_ring<RingBody::stream_writes><<<1, kSmallThreads, sizeof(SmallSmem), c->ring_stream>>>(R, B, c->cfg, SP, c->swr_dev);
-        } else k_ring<RingBody::batch><<<1, kSmallThreads, sizeof(SmallSmem), c->ring_stream>>>(R, B, c->cfg, SP, ClientRingDev{});
+        } else k_ring<RingBody::batch><<<1, kSmallThreads, sizeof(SmallSmem), c->ring_stream>>>(R, B, c->cfg, SP, PackRingDev{});
     }
     }
     c->ring_launches++;
@@ -1371,6 +1377,7 @@ extern "C" int b2_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, con
     if (c->ring_kind == RingKind::h2_server) { set_err("this context's ring serves h2 (b2_h2_ring_enable): use b2_h2_ring_submit"); return B2_E_INVAL; }
     if (c->ring_kind == RingKind::h2_client) { set_err("this context's ring serves h2 client connections (b2_h2_client_ring_enable): use b2_h2_client_ring_submit"); return B2_E_INVAL; }
     if (c->ring_kind == RingKind::batch_client) { set_err("this context's ring serves client turns (b2_client_ring_enable): use b2_client_ring_submit"); return B2_E_INVAL; }
+    if (c->ring_kind == RingKind::batch_replies) { set_err("this context's ring serves server turns (b2_ring_turn_enable): use b2_ring_turn_submit"); return B2_E_INVAL; }
     if (c->ring_kind == RingKind::batch_stream_writes) { set_err("this context's ring serves Stream producer turns (b2_stream_ring_write_enable): use b2_stream_ring_submit"); return B2_E_INVAL; }
     if (nbytes > kSmallBytes || n_runs > kSmallRuns) { set_err("b2_ring_submit serves batches up to 128 KiB / 512 runs: use b2_batch_submit"); return B2_E_CAPACITY; }
     if (!c->ring_slots) { int rc = b2_ring_start(c); if (rc != B2_OK) return rc; }
@@ -1387,6 +1394,7 @@ extern "C" int b2_ring_wait(b2_ctx* c, uint32_t ticket, b2_batch_result* out) {
     if (c && c->ring_kind == RingKind::h2_server) { set_err("this context's ring serves h2: use b2_h2_ring_wait"); return B2_E_INVAL; }
     if (c && c->ring_kind == RingKind::h2_client) { set_err("this context's ring serves h2 client connections: use b2_h2_client_ring_wait"); return B2_E_INVAL; }
     if (c && c->ring_kind == RingKind::batch_client) { set_err("this context's ring serves client turns: use b2_client_ring_wait"); return B2_E_INVAL; }
+    if (c && c->ring_kind == RingKind::batch_replies) { set_err("this context's ring serves server turns: use b2_ring_turn_wait"); return B2_E_INVAL; }
     if (c && c->ring_kind == RingKind::batch_stream_writes) { set_err("this context's ring serves Stream producer turns: use b2_stream_ring_wait"); return B2_E_INVAL; }
     int rc;
     uint8_t* slot = ring_collect(c, c && out, ticket, "bad ring ticket", rc);
@@ -2176,15 +2184,8 @@ extern "C" int b2_pack_requests(b2_ctx* c, const void* bytes, uint32_t nbytes, c
     return B2_OK;
 }
 
-// SendRpcResponse for replies the host produced: see include/b2rpc.h
-extern "C" int b2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_reply* reps, uint32_t n,
-                                 void* out, uint32_t out_cap, uint32_t* out_offs, uint32_t* out_lens) {
-    if (!c || (!bytes && nbytes) || !reps || !out || !out_offs || !out_lens) { set_err("null argument"); return B2_E_INVAL; }
-    if (ring_refuses(c, false)) return B2_E_INVAL;
-    static_assert(sizeof(b2_reply) == 88 && sizeof(ReplyDesc) == 88, "reply ABI layout");
-    if (nbytes > c->opt.max_batch_bytes || (uint64_t)n * sizeof(b2_reply) > (uint64_t)c->opt.max_msgs * 64 || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
-    if (n == 0) return B2_OK;
-    uint64_t total = 0;
+// the frame of every reply, placed with out_place at its worst-case size (b2_pack_responses, b2_ring_turn_submit); total: the bytes placed
+static int place_replies(const void* bytes, uint32_t nbytes, const b2_reply* reps, uint32_t n, uint32_t out_cap, uint32_t* out_offs, uint64_t& total) {
     for (uint32_t i = 0; i < n; i++) {
         const b2_reply& r = reps[i];
         if ((uint64_t)r.body_off + r.body_len > nbytes || (uint64_t)r.attachment_off + r.attachment_len > nbytes || (uint64_t)r.error_text_off + r.error_text_len > nbytes ||
@@ -2201,6 +2202,19 @@ extern "C" int b2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbytes, 
         const uint64_t need = 12 + 128 + r.error_text_len + r.checksum_value_len + 11ull * r.n_extra_streams + uf + body + r.attachment_len;
         if (!out_place(total, need, out_cap, &out_offs[i])) { set_err("out_cap too small"); return B2_E_CAPACITY; }
     }
+    return B2_OK;
+}
+// SendRpcResponse for replies the host produced: see include/b2rpc.h
+extern "C" int b2_pack_responses(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_reply* reps, uint32_t n,
+                                 void* out, uint32_t out_cap, uint32_t* out_offs, uint32_t* out_lens) {
+    if (!c || (!bytes && nbytes) || !reps || !out || !out_offs || !out_lens) { set_err("null argument"); return B2_E_INVAL; }
+    if (ring_refuses(c, false)) return B2_E_INVAL;
+    static_assert(sizeof(b2_reply) == 88 && sizeof(ReplyDesc) == 88, "reply ABI layout");
+    if (nbytes > c->opt.max_batch_bytes || (uint64_t)n * sizeof(b2_reply) > (uint64_t)c->opt.max_msgs * 64 || out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    if (n == 0) return B2_OK;
+    uint64_t total = 0;
+    const int rc = place_replies(bytes, nbytes, reps, n, out_cap, out_offs, total);
+    if (rc != B2_OK) return rc;
     CU(cudaSetDevice(c->opt.device));
     ReplyDesc* d_reps = reinterpret_cast<ReplyDesc*>(c->d_msgs);
     uint32_t* d_offs = c->d_frame_off; uint32_t* d_lens = c->d_slot;
@@ -2467,72 +2481,112 @@ extern "C" int b2_h2_client_ring_wait(b2_ctx* c, uint32_t ticket, b2_h2_client_r
     return B2_OK;
 }
 
-// ---- a baidu_std client's turn on the latency path: k_ring<RingBody::requests> on the same submit ring (include/b2rpc.h, b2_client_ring_enable) ----
-extern "C" int b2_client_ring_enable(b2_ctx* c, uint32_t max_bytes, uint32_t max_reqs, uint32_t req_out_cap) {
+// ---- baidu_std turns on the latency path: k_ring<RingBody::requests> (b2_client_ring_*) and k_ring<RingBody::replies> (b2_ring_turn_*)
+// on the same submit ring (include/b2rpc.h).  Both kinds pack one record per warp after the runs; they differ in the record and in what
+// checks and places it (place_requests / place_replies).
+struct PackRingNames { const char *enable, *submit, *wait, *recs, *max_recs; };
+static const PackRingNames kClientRing = { "b2_client_ring_enable", "b2_client_ring_submit", "b2_client_ring_wait", "requests", "max_reqs" };
+static const PackRingNames kTurnRing = { "b2_ring_turn_enable", "b2_ring_turn_submit", "b2_ring_turn_wait", "replies", "max_resps" };
+static int pack_ring_enable(b2_ctx* c, RingKind kind, const PackRingNames& nm, uint32_t max_bytes, uint32_t max_recs, uint32_t rec_bytes, uint32_t out_cap) {
     if (!c) { set_err("null argument"); return B2_E_INVAL; }
-    if (c->ring_kind != RingKind::none) { set_err("b2_client_ring_enable: once, before the context's first ring call, and not with another ring kind"); return B2_E_INVAL; }
-    if (c->has_streams) { set_err("b2_client_ring_enable: the client ring runs no stream pass, so not on a context with a stream table"); return B2_E_INVAL; }
-    if (max_bytes == 0 || max_reqs == 0 || req_out_cap == 0) { set_err("capacities must be non-zero"); return B2_E_INVAL; }
-    // the limits of b2_process_batch and b2_pack_requests, both of which read the ticket's bytes
-    if (max_bytes > c->opt.max_batch_bytes || max_reqs > c->opt.max_msgs || req_out_cap > c->opt.max_resp_bytes) { set_err("exceeds ctx capacity"); return B2_E_CAPACITY; }
+    if (c->ring_kind != RingKind::none) { set_err("%s: once, before the context's first ring call, and not with another ring kind", nm.enable); return B2_E_INVAL; }
+    if (c->has_streams) { set_err("%s: the ticket runs no stream pass, so not on a context with a stream table", nm.enable); return B2_E_INVAL; }
+    if (max_bytes == 0 || max_recs == 0 || out_cap == 0) { set_err("capacities must be non-zero"); return B2_E_INVAL; }
+    // the limits of b2_process_batch and of the batch pack call, both of which read the ticket's bytes; the records land in d_msgs
+    if (max_bytes > c->opt.max_batch_bytes || (uint64_t)max_recs * rec_bytes > (uint64_t)c->opt.max_msgs * 64 || out_cap > c->opt.max_resp_bytes) {
+        set_err("exceeds ctx capacity"); return B2_E_CAPACITY;
+    }
     CU(cudaSetDevice(c->opt.device));
-    static_assert(sizeof(RingSlotHdr) + sizeof(ClientRingArgs) <= 256, "client ring slot header");
-    // [RingSlotHdr | args | runs | staged input | requests + placed offsets | compact block | frame lengths | frames]
+    static_assert(sizeof(RingSlotHdr) + sizeof(PackRingArgs) <= 256, "pack ring slot header");
+    // [RingSlotHdr | args | runs | staged input | records + placed offsets | compact block | frame lengths | frames]
     SlotLayout L;
-    ClientRingDev& Q = c->cr_dev;
+    PackRingDev& Q = c->pr_dev;
     Q.off_args = sizeof(RingSlotHdr);
     c->ring_dev.off_runs = L.add(kSmallRuns * sizeof(b2_run));
     c->ring_dev.off_in = L.add((uint64_t)max_bytes + 16);
-    Q.off_reqs = L.add((uint64_t)max_reqs * (sizeof(b2_request) + 4));
+    Q.off_recs = L.add((uint64_t)max_recs * (rec_bytes + 4) + 16);      // (+16: the kernel pulls the records in whole 16-byte words)
     c->ring_dev.off_out = L.add(kSmallBlock);
-    Q.off_req_lens = L.add((uint64_t)max_reqs * 4);
-    Q.off_req_out = L.add((uint64_t)req_out_cap + 16);
+    Q.off_lens = L.add((uint64_t)max_recs * 4);
+    Q.off_out = L.add((uint64_t)out_cap + 16);
     int rc = ring_alloc(c, L.end); if (rc != B2_OK) return rc;
-    CU(cudaFuncSetAttribute(k_ring<RingBody::requests>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmallSmem)));
-    c->cr_max_bytes = max_bytes; c->cr_max_reqs = max_reqs; c->cr_req_out_cap = req_out_cap;
-    c->ring_kind = RingKind::batch_client;
+    if (kind == RingKind::batch_client) CU(cudaFuncSetAttribute(k_ring<RingBody::requests>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmallSmem)));
+    else CU(cudaFuncSetAttribute(k_ring<RingBody::replies>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmallSmem)));
+    c->pr_max_bytes = max_bytes; c->pr_max_recs = max_recs; c->pr_out_cap = out_cap;
+    c->ring_kind = kind;
     return B2_OK;
 }
-extern "C" int b2_client_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
-                                     const b2_request* reqs, uint32_t n_reqs, uint32_t* ticket) {
-    if (!c || !bytes || !ticket || (!runs && n_runs) || (!reqs && n_reqs)) { set_err("null argument"); return B2_E_INVAL; }
-    if (n_runs == 0 && n_reqs == 0) { set_err("a ticket carries runs, requests or both"); return B2_E_INVAL; }
-    if (c->ring_kind != RingKind::batch_client) { set_err("b2_client_ring_enable first"); return B2_E_INVAL; }
-    // the argument checks of b2_ring_submit and b2_pack_requests with the caps of b2_client_ring_enable
-    if (nbytes > c->cr_max_bytes) { set_err("ticket larger than b2_client_ring_enable's max_bytes: use the batch calls"); return B2_E_CAPACITY; }
-    if (n_runs > kSmallRuns || n_runs > c->opt.max_runs) { set_err("b2_client_ring_submit serves up to 512 runs: use the batch calls"); return B2_E_CAPACITY; }
-    if (n_reqs > c->cr_max_reqs) { set_err("more requests than b2_client_ring_enable's max_reqs"); return B2_E_CAPACITY; }
-    uint8_t* slot = ring_claim(c, "b2_client_ring_wait");
+// place(block + n_recs * rec_bytes, total): the kind's checks of its records, and their offsets placed right behind them in the slot
+template <class Place>
+static int pack_ring_submit(b2_ctx* c, RingKind kind, const PackRingNames& nm, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
+                            const void* recs, uint32_t n_recs, size_t rec_bytes, Place place, uint32_t* ticket) {
+    if (!c || !bytes || !ticket || (!runs && n_runs) || (!recs && n_recs)) { set_err("null argument"); return B2_E_INVAL; }
+    if (n_runs == 0 && n_recs == 0) { set_err("a ticket carries runs, %s or both", nm.recs); return B2_E_INVAL; }
+    if (c->ring_kind != kind) { set_err("%s first", nm.enable); return B2_E_INVAL; }
+    // the argument checks of b2_ring_submit and of the batch pack call with the enable-time caps
+    if (nbytes > c->pr_max_bytes) { set_err("ticket larger than %s's max_bytes: use the batch calls", nm.enable); return B2_E_CAPACITY; }
+    if (n_runs > kSmallRuns || n_runs > c->opt.max_runs) { set_err("%s serves up to 512 runs: use the batch calls", nm.submit); return B2_E_CAPACITY; }
+    if (n_recs > c->pr_max_recs) { set_err("more %s than the enable call's %s", nm.recs, nm.max_recs); return B2_E_CAPACITY; }
+    uint8_t* slot = ring_claim(c, nm.wait);
     if (!slot) return B2_E_CAPACITY;
     uint32_t extent = 0;                                         // (the compact block is sized for the bytes the runs cover)
     for (uint32_t r = 0; r < n_runs; r++) {
         if ((runs[r].offset & 15u) || (uint64_t)runs[r].offset + runs[r].length > nbytes) { set_err("run offset must be 16-aligned and inside the batch"); return B2_E_INVAL; }
         extent = std::max(extent, runs[r].offset + runs[r].length);
     }
-    uint8_t* block = slot + c->cr_dev.off_reqs;                  // the request block the kernel pulls: requests, then their placed offsets
+    uint8_t* block = slot + c->pr_dev.off_recs;                  // the record block the kernel pulls: records, then their placed offsets
     uint64_t total = 0;
-    int rc = place_requests(nbytes, reqs, n_reqs, c->cr_req_out_cap, reinterpret_cast<uint32_t*>(block + sizeof(b2_request) * (size_t)n_reqs), total);
+    int rc = place(reinterpret_cast<uint32_t*>(block + rec_bytes * n_recs), total);
     if (rc != B2_OK) return rc;
-    if (n_reqs) memcpy(block, reqs, sizeof(b2_request) * (size_t)n_reqs);
-    const ClientRingArgs a = { n_reqs, { 0, 0, 0 } };
+    if (n_recs) memcpy(block, recs, rec_bytes * n_recs);
+    const PackRingArgs a = { n_recs, { 0, 0, 0 } };
     RingSlotHdr* h = ring_fill(c, slot, bytes, nbytes, runs, n_runs);
     ring_compact(c, h, small_layout(std::min(extent, kSmallBytes), n_runs, c->opt.max_msgs));
-    memcpy(slot + c->cr_dev.off_args, &a, sizeof a);
+    memcpy(slot + c->pr_dev.off_args, &a, sizeof a);
     return ring_ring(c, h, bytes, ticket);
+}
+// the runs' result (an overflowing ticket's runs go through the big pipeline here) and views of the ticket's frames in its slot: out's
+// batch, then its count, offsets, lengths and frames (the members named)
+template <class Result>
+static int pack_ring_wait(b2_ctx* c, RingKind kind, const char* bad_ticket, uint32_t ticket, size_t rec_bytes, Result* out, uint32_t Result::*n_recs,
+                          const uint32_t* Result::*offs, const uint32_t* Result::*lens, const uint8_t* Result::*frames) {
+    int rc;
+    uint8_t* slot = ring_collect(c, c && out && c->ring_kind == kind, ticket, bad_ticket, rc);
+    if (!slot) return rc;
+    memset(out, 0, sizeof *out);
+    const PackRingDev& L = c->pr_dev;
+    const uint32_t n = reinterpret_cast<const PackRingArgs*>(slot + L.off_args)->n_recs;
+    out->*n_recs = n;
+    out->*offs = reinterpret_cast<const uint32_t*>(slot + L.off_recs + rec_bytes * n);
+    out->*lens = reinterpret_cast<const uint32_t*>(slot + L.off_lens);
+    out->*frames = slot + L.off_out;
+    return ring_batch_result(c, ticket, slot, &out->batch);
+}
+
+extern "C" int b2_client_ring_enable(b2_ctx* c, uint32_t max_bytes, uint32_t max_reqs, uint32_t req_out_cap) {
+    return pack_ring_enable(c, RingKind::batch_client, kClientRing, max_bytes, max_reqs, sizeof(b2_request), req_out_cap);
+}
+extern "C" int b2_client_ring_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
+                                     const b2_request* reqs, uint32_t n_reqs, uint32_t* ticket) {
+    return pack_ring_submit(c, RingKind::batch_client, kClientRing, bytes, nbytes, runs, n_runs, reqs, n_reqs, sizeof(b2_request),
+                            [&](uint32_t* offs, uint64_t& total) { return place_requests(nbytes, reqs, n_reqs, c->pr_out_cap, offs, total); }, ticket);
 }
 extern "C" int b2_client_ring_wait(b2_ctx* c, uint32_t ticket, b2_client_ring_result* out) {
     static_assert(sizeof(b2_client_ring_result) == 104, "client ring result ABI layout");
-    int rc;
-    uint8_t* slot = ring_collect(c, c && out && c->ring_kind == RingKind::batch_client, ticket, "bad client ring ticket", rc);
-    if (!slot) return rc;
-    memset(out, 0, sizeof *out);
-    const ClientRingDev& L = c->cr_dev;
-    const uint32_t n = reinterpret_cast<const ClientRingArgs*>(slot + L.off_args)->n_reqs;
-    out->n_reqs = n;
-    out->req_offs = reinterpret_cast<const uint32_t*>(slot + L.off_reqs + sizeof(b2_request) * (size_t)n);
-    out->req_lens = reinterpret_cast<const uint32_t*>(slot + L.off_req_lens);
-    out->req_out = slot + L.off_req_out;
-    return ring_batch_result(c, ticket, slot, &out->batch);      // (an overflowing ticket's runs go through the big pipeline here)
+    return pack_ring_wait(c, RingKind::batch_client, "bad client ring ticket", ticket, sizeof(b2_request), out, &b2_client_ring_result::n_reqs,
+                          &b2_client_ring_result::req_offs, &b2_client_ring_result::req_lens, &b2_client_ring_result::req_out);
+}
+extern "C" int b2_ring_turn_enable(b2_ctx* c, uint32_t max_bytes, uint32_t max_resps, uint32_t resp_out_cap) {
+    return pack_ring_enable(c, RingKind::batch_replies, kTurnRing, max_bytes, max_resps, sizeof(b2_reply), resp_out_cap);
+}
+extern "C" int b2_ring_turn_submit(b2_ctx* c, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
+                                   const b2_reply* replies, uint32_t n_replies, uint32_t* ticket) {
+    return pack_ring_submit(c, RingKind::batch_replies, kTurnRing, bytes, nbytes, runs, n_runs, replies, n_replies, sizeof(b2_reply),
+                            [&](uint32_t* offs, uint64_t& total) { return place_replies(bytes, nbytes, replies, n_replies, c->pr_out_cap, offs, total); }, ticket);
+}
+extern "C" int b2_ring_turn_wait(b2_ctx* c, uint32_t ticket, b2_ring_turn_result* out) {
+    static_assert(sizeof(b2_ring_turn_result) == 104, "ring turn result ABI layout");
+    return pack_ring_wait(c, RingKind::batch_replies, "bad ring turn ticket", ticket, sizeof(b2_reply), out, &b2_ring_turn_result::n_replies,
+                          &b2_ring_turn_result::reply_offs, &b2_ring_turn_result::reply_lens, &b2_ring_turn_result::reply_out);
 }
 
 // ---- a Stream producer's turn on the latency path: k_ring<RingBody::stream_writes> (include/b2rpc.h, b2_stream_ring_write_enable) ----

@@ -2522,6 +2522,81 @@ __device__ __forceinline__ uint32_t reply_user_fields_len(const uint8_t* uf, uin
     }
     return total;
 }
+// One reply by one warp: its frame at out + *out_off, *out_len by lane 0 (0: not packable), a snappy body compressed with the warp's
+// encoder table snappy_tab.  k_pack_responses and the reply phase of k_ring<RingBody::replies> run it.
+__device__ __forceinline__ void pack_response_one(const uint8_t* bytes, const ReplyDesc& R, uint8_t* out, const uint32_t* out_off, uint16_t* snappy_tab,
+                                                  uint32_t* out_len, uint32_t lane, const CrcTabs& ct) {
+    uint8_t* o = out + *out_off;
+    const int32_t err = R.error_code == -1 ? B2_EINTERNAL : R.error_code;                  // :333-337
+    const bool append_body = err == 0;                                                       // :316-330
+    if (append_body && R.compress_type != B2_COMPRESS_TYPE_NONE && R.compress_type != B2_COMPRESS_TYPE_SNAPPY) { if (lane == 0) *out_len = 0; return; }
+    const bool own_cks = append_body && R.checksum_type == B2_CHECKSUM_TYPE_CRC32C;
+    const uint32_t cks_len = own_cks ? 4u : R.checksum_value_len;
+    const uint32_t att_len = append_body ? R.attachment_len : 0u;
+    // RpcResponseMeta: error_code(1) [error_text(2)]
+    uint32_t rl = 1 + varint_len((uint64_t)(long long)err);
+    if (R.error_text_len) rl += 1 + varint_len(R.error_text_len) + R.error_text_len;
+    // StreamSettings: stream_id(1) need_feedback(2) writable(3) extra_stream_ids(4)*
+    uint32_t sl = 0;
+    const long long* extra = reinterpret_cast<const long long*>(bytes + R.extra_streams_off);
+    if (R.flags & B2_RSP_HAS_STREAM) {
+        sl = 1 + varint_len((uint64_t)R.stream_id) + 2 + 2;
+        for (uint32_t k = 0; k < R.n_extra_streams; k++) sl += 1 + varint_len((uint64_t)extra[k]);
+    }
+    const uint32_t ufl = R.n_user_fields ? reply_user_fields_len(bytes + R.user_fields_off, R.n_user_fields) : 0u;
+    uint32_t ml = 1 + varint_len(rl) + rl + 1 + varint_len((uint64_t)(long long)R.compress_type) + 1 + varint_len((uint64_t)R.correlation_id);
+    if (att_len) ml += 1 + varint_len(att_len);
+    if (R.flags & B2_RSP_HAS_STREAM) ml += 1 + varint_len(sl) + sl;
+    ml += ufl;
+    ml += 1 + varint_len((uint64_t)(long long)R.content_type) + 1 + varint_len((uint64_t)(long long)R.checksum_type) + 1 + varint_len(cks_len) + cks_len;
+    uint8_t* body = o + 12 + ml;
+    uint32_t body_len = 0;
+    if (append_body) {
+        if (R.compress_type == B2_COMPRESS_TYPE_SNAPPY)
+            body_len = warp_snappy_compress(bytes + R.body_off, R.body_len, body, snappy_tab, lane);
+        else { warp_copy(body, bytes + R.body_off, R.body_len, lane); body_len = R.body_len; }
+    }
+    __syncwarp();
+    uint32_t crc_be = 0;
+    if (own_cks) {                                                                           // Crc32cCompute over what goes on the wire
+        const uint8_t* src = R.compress_type == B2_COMPRESS_TYPE_SNAPPY ? body : bytes + R.body_off;
+        if (R.compress_type == B2_COMPRESS_TYPE_SNAPPY) __threadfence_block();
+        crc_be = crc32c_mask(warp_crc32c_update(0xffffffffu, src, body_len, lane, ct) ^ 0xffffffffu);
+    }
+    if (att_len) warp_copy(body + body_len, bytes + R.attachment_off, att_len, lane);
+    if (lane == 0) {
+        uint8_t* p = o;
+        p[0] = 'P'; p[1] = 'R'; p[2] = 'P'; p[3] = 'C'; put_be32(p + 4, ml + body_len + att_len); put_be32(p + 8, ml); p += 12;
+        *p++ = 0x12; p = put_varint(p, rl);
+        *p++ = 0x08; p = put_varint(p, (uint64_t)(long long)err);
+        if (R.error_text_len) { *p++ = 0x12; p = put_varint(p, R.error_text_len); for (uint32_t k = 0; k < R.error_text_len; k++) *p++ = bytes[R.error_text_off + k]; }
+        *p++ = 0x18; p = put_varint(p, (uint64_t)(long long)R.compress_type);
+        *p++ = 0x20; p = put_varint(p, (uint64_t)R.correlation_id);
+        if (att_len) { *p++ = 0x28; p = put_varint(p, att_len); }
+        if (R.flags & B2_RSP_HAS_STREAM) {
+            *p++ = 0x42; p = put_varint(p, sl);
+            *p++ = 0x08; p = put_varint(p, (uint64_t)R.stream_id);
+            *p++ = 0x10; *p++ = (R.flags & B2_RSP_STREAM_NEED_FEEDBACK) ? 1 : 0;
+            *p++ = 0x18; *p++ = (R.flags & B2_RSP_STREAM_WRITABLE) ? 1 : 0;
+            for (uint32_t k = 0; k < R.n_extra_streams; k++) { *p++ = 0x20; p = put_varint(p, (uint64_t)extra[k]); }
+        }
+        const uint8_t* uf = bytes + R.user_fields_off;
+        for (uint32_t k = 0; k < R.n_user_fields; k++) {                                     // map<string,string> user_fields = 9: entry {key = 1, value = 2}
+            const uint32_t kl = load_le32(uf), vl = load_le32(uf + 4);
+            const uint32_t el = 1 + varint_len(kl) + kl + 1 + varint_len(vl) + vl;
+            *p++ = 0x4a; p = put_varint(p, el);
+            *p++ = 0x0a; p = put_varint(p, kl); for (uint32_t q = 0; q < kl; q++) *p++ = uf[8 + q];
+            *p++ = 0x12; p = put_varint(p, vl); for (uint32_t q = 0; q < vl; q++) *p++ = uf[8 + kl + q];
+            uf += 8 + kl + vl;
+        }
+        *p++ = 0x50; p = put_varint(p, (uint64_t)(long long)R.content_type);
+        *p++ = 0x58; p = put_varint(p, (uint64_t)(long long)R.checksum_type);
+        *p++ = 0x62; p = put_varint(p, cks_len);
+        if (own_cks) p = put_be32(p, crc_be);
+        else for (uint32_t k = 0; k < cks_len; k++) *p++ = bytes[R.checksum_value_off + k];
+        *out_len = 12 + ml + body_len + att_len;
+    }
+}
 __global__ void __launch_bounds__(256) k_pack_responses(const uint8_t* bytes, const ReplyDesc* reps, uint32_t n, uint8_t* out, const uint32_t* out_offs,
                                                         uint32_t* out_lens, uint8_t* scratch, uint16_t* snappy_tab, const uint32_t* crc_adv) {
     __shared__ uint32_t s_hot[kCrcHotWords];
@@ -2530,76 +2605,7 @@ __global__ void __launch_bounds__(256) k_pack_responses(const uint8_t* bytes, co
     const uint32_t lane = threadIdx.x & 31, n_warps = (gridDim.x * blockDim.x) >> 5, warp_id = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     for (uint32_t i = warp_id; i < n; i += n_warps) {
         const ReplyDesc R = reps[i];
-        uint8_t* o = out + out_offs[i];
-        const int32_t err = R.error_code == -1 ? B2_EINTERNAL : R.error_code;                  // :333-337
-        const bool append_body = err == 0;                                                       // :316-330
-        if (append_body && R.compress_type != B2_COMPRESS_TYPE_NONE && R.compress_type != B2_COMPRESS_TYPE_SNAPPY) { if (lane == 0) out_lens[i] = 0; continue; }
-        const bool own_cks = append_body && R.checksum_type == B2_CHECKSUM_TYPE_CRC32C;
-        const uint32_t cks_len = own_cks ? 4u : R.checksum_value_len;
-        const uint32_t att_len = append_body ? R.attachment_len : 0u;
-        // RpcResponseMeta: error_code(1) [error_text(2)]
-        uint32_t rl = 1 + varint_len((uint64_t)(long long)err);
-        if (R.error_text_len) rl += 1 + varint_len(R.error_text_len) + R.error_text_len;
-        // StreamSettings: stream_id(1) need_feedback(2) writable(3) extra_stream_ids(4)*
-        uint32_t sl = 0;
-        const long long* extra = reinterpret_cast<const long long*>(bytes + R.extra_streams_off);
-        if (R.flags & B2_RSP_HAS_STREAM) {
-            sl = 1 + varint_len((uint64_t)R.stream_id) + 2 + 2;
-            for (uint32_t k = 0; k < R.n_extra_streams; k++) sl += 1 + varint_len((uint64_t)extra[k]);
-        }
-        const uint32_t ufl = R.n_user_fields ? reply_user_fields_len(bytes + R.user_fields_off, R.n_user_fields) : 0u;
-        uint32_t ml = 1 + varint_len(rl) + rl + 1 + varint_len((uint64_t)(long long)R.compress_type) + 1 + varint_len((uint64_t)R.correlation_id);
-        if (att_len) ml += 1 + varint_len(att_len);
-        if (R.flags & B2_RSP_HAS_STREAM) ml += 1 + varint_len(sl) + sl;
-        ml += ufl;
-        ml += 1 + varint_len((uint64_t)(long long)R.content_type) + 1 + varint_len((uint64_t)(long long)R.checksum_type) + 1 + varint_len(cks_len) + cks_len;
-        uint8_t* body = o + 12 + ml;
-        uint32_t body_len = 0;
-        if (append_body) {
-            if (R.compress_type == B2_COMPRESS_TYPE_SNAPPY)
-                body_len = warp_snappy_compress(bytes + R.body_off, R.body_len, body, snappy_tab + (size_t)(warp_id % kSnappyWarps) * kSnappyMaxTable, lane);
-            else { warp_copy(body, bytes + R.body_off, R.body_len, lane); body_len = R.body_len; }
-        }
-        __syncwarp();
-        uint32_t crc_be = 0;
-        if (own_cks) {                                                                           // Crc32cCompute over what goes on the wire
-            const uint8_t* src = R.compress_type == B2_COMPRESS_TYPE_SNAPPY ? body : bytes + R.body_off;
-            if (R.compress_type == B2_COMPRESS_TYPE_SNAPPY) __threadfence_block();
-            crc_be = crc32c_mask(warp_crc32c_update(0xffffffffu, src, body_len, lane, ct) ^ 0xffffffffu);
-        }
-        if (att_len) warp_copy(body + body_len, bytes + R.attachment_off, att_len, lane);
-        if (lane == 0) {
-            uint8_t* p = o;
-            p[0] = 'P'; p[1] = 'R'; p[2] = 'P'; p[3] = 'C'; put_be32(p + 4, ml + body_len + att_len); put_be32(p + 8, ml); p += 12;
-            *p++ = 0x12; p = put_varint(p, rl);
-            *p++ = 0x08; p = put_varint(p, (uint64_t)(long long)err);
-            if (R.error_text_len) { *p++ = 0x12; p = put_varint(p, R.error_text_len); for (uint32_t k = 0; k < R.error_text_len; k++) *p++ = bytes[R.error_text_off + k]; }
-            *p++ = 0x18; p = put_varint(p, (uint64_t)(long long)R.compress_type);
-            *p++ = 0x20; p = put_varint(p, (uint64_t)R.correlation_id);
-            if (att_len) { *p++ = 0x28; p = put_varint(p, att_len); }
-            if (R.flags & B2_RSP_HAS_STREAM) {
-                *p++ = 0x42; p = put_varint(p, sl);
-                *p++ = 0x08; p = put_varint(p, (uint64_t)R.stream_id);
-                *p++ = 0x10; *p++ = (R.flags & B2_RSP_STREAM_NEED_FEEDBACK) ? 1 : 0;
-                *p++ = 0x18; *p++ = (R.flags & B2_RSP_STREAM_WRITABLE) ? 1 : 0;
-                for (uint32_t k = 0; k < R.n_extra_streams; k++) { *p++ = 0x20; p = put_varint(p, (uint64_t)extra[k]); }
-            }
-            const uint8_t* uf = bytes + R.user_fields_off;
-            for (uint32_t k = 0; k < R.n_user_fields; k++) {                                     // map<string,string> user_fields = 9: entry {key = 1, value = 2}
-                const uint32_t kl = load_le32(uf), vl = load_le32(uf + 4);
-                const uint32_t el = 1 + varint_len(kl) + kl + 1 + varint_len(vl) + vl;
-                *p++ = 0x4a; p = put_varint(p, el);
-                *p++ = 0x0a; p = put_varint(p, kl); for (uint32_t q = 0; q < kl; q++) *p++ = uf[8 + q];
-                *p++ = 0x12; p = put_varint(p, vl); for (uint32_t q = 0; q < vl; q++) *p++ = uf[8 + kl + q];
-                uf += 8 + kl + vl;
-            }
-            *p++ = 0x50; p = put_varint(p, (uint64_t)(long long)R.content_type);
-            *p++ = 0x58; p = put_varint(p, (uint64_t)(long long)R.checksum_type);
-            *p++ = 0x62; p = put_varint(p, cks_len);
-            if (own_cks) p = put_be32(p, crc_be);
-            else for (uint32_t k = 0; k < cks_len; k++) *p++ = bytes[R.checksum_value_off + k];
-            out_lens[i] = 12 + ml + body_len + att_len;
-        }
+        pack_response_one(bytes, R, out, out_offs + i, snappy_tab + (size_t)(warp_id % kSnappyWarps) * kSnappyMaxTable, out_lens + i, lane, ct);
     }
 }
 
@@ -3544,16 +3550,18 @@ __device__ __forceinline__ void stream_write_block(const SwPass& P, uint32_t* wa
     for (uint32_t t = tid; t < n_touched; t += kSmallThreads) { const uint32_t s = P.touched[t]; P.cnt[s] = 0; P.fill[s] = 0; }
 }
 
-// k_ring<RingBody::requests>: a client's turn (b2_client_ring_*).  The runs as k_ring serves them (a client ticket has no stream pass), then
-// the ticket's requests as k_pack_requests packs them, a warp per request.  The requests do not depend on the runs, so they are packed whether or not the runs
-// overflowed the compact block.  Their records and host-placed offsets are pulled from the slot into scratch small_body does not touch
-// here (d_msgs, d_refs: k_ring's descriptors and refs live in the compact block); the snappy scratch (d_unz) and the frames (d_resp) are
-// batch scratch that the pack phase only writes once small_body's results are final.  Only out_len bytes of each frame are pushed.
-struct ClientRingArgs { uint32_t n_reqs, pad[3]; };   // per ticket, from the host, at the slot's off_args
-struct ClientRingDev {
-    // the slot's parts behind RingSlotHdr (runs, staged input, compact block: RingDev); off_reqs: [requests | placed offsets] of the ticket
-    uint32_t off_args, off_reqs, off_req_lens, off_req_out;
-    ReqDesc* reqs; uint32_t* offs; uint32_t* lens;      // the pulled requests and offsets, the frame lengths
+// k_ring<RingBody::requests>: a client's turn (b2_client_ring_*); k_ring<RingBody::replies>: a server's turn (b2_ring_turn_*).  The runs as
+// k_ring serves them (neither ticket has a stream pass), then the ticket's records, a warp per record: requests as k_pack_requests packs
+// them, replies the host produced as k_pack_responses packs them.  baidu_std keeps no connection state on the device, so the records do
+// not depend on the runs and are packed whether or not the runs overflowed the compact block.  The records and their host-placed offsets
+// are pulled from the slot into scratch small_body does not touch here (d_msgs, d_refs: k_ring's descriptors and refs live in the compact
+// block); the snappy scratch (d_unz) and the frames (d_resp) are batch scratch that the pack phase only writes once small_body's results
+// are final.  Only out_len bytes of each frame are pushed.
+struct PackRingArgs { uint32_t n_recs, pad[3]; };    // per ticket, from the host, at the slot's off_args
+struct PackRingDev {
+    // the slot's parts behind RingSlotHdr (runs, staged input, compact block: RingDev); off_recs: [records | placed offsets] of the ticket
+    uint32_t off_args, off_recs, off_lens, off_out;
+    uint8_t* recs; uint32_t* offs; uint32_t* lens;      // the pulled records (ReqDesc / ReplyDesc) and offsets, the frame lengths
     uint8_t* scratch; uint8_t* out;                     // k_pack_requests' snappy scratch and frames
 };
 // k_ring<RingBody::stream_writes>: a Stream producer's turn (b2_stream_ring_*).  The runs and the stream pass as in a stream-ring ticket,
@@ -3568,14 +3576,15 @@ struct SwRingDev {
     uint32_t off_args, off_recs, off_res, off_wout;
     SwPass pass;                                        // table, seg and the pass's device scratch (n: per ticket)
 };
-enum class RingBody { batch, requests, stream_writes };
-template <RingBody> struct RingBodyOf { using Args = RingNoArgs; using Dev = ClientRingDev; };
-template <> struct RingBodyOf<RingBody::requests> { using Args = ClientRingArgs; using Dev = ClientRingDev; };
+enum class RingBody { batch, requests, stream_writes, replies };
+template <RingBody> struct RingBodyOf { using Args = RingNoArgs; using Dev = PackRingDev; };
+template <> struct RingBodyOf<RingBody::requests> { using Args = PackRingArgs; using Dev = PackRingDev; using Rec = ReqDesc; };
+template <> struct RingBodyOf<RingBody::replies> { using Args = PackRingArgs; using Dev = PackRingDev; using Rec = ReplyDesc; };
 template <> struct RingBodyOf<RingBody::stream_writes> { using Args = SwRingArgs; using Dev = SwRingDev; };
 template <RingBody kBody>
 __global__ void __launch_bounds__(kSmallThreads, 1) k_ring(RingDev R, BatchPtrs B0, DevConfig C, StreamPass SP, typename RingBodyOf<kBody>::Dev Q) {
     using Args = typename RingBodyOf<kBody>::Args;
-    constexpr bool kRequests = kBody == RingBody::requests, kWrites = kBody == RingBody::stream_writes;
+    constexpr bool kRequests = kBody == RingBody::requests, kPacks = kRequests || kBody == RingBody::replies, kWrites = kBody == RingBody::stream_writes;
     extern __shared__ __align__(128) uint8_t small_raw[];
     SmallSmem& S = *reinterpret_cast<SmallSmem*>(small_raw);
     const uint32_t tid = threadIdx.x;
@@ -3591,12 +3600,13 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_ring(RingDev R, BatchPtrs 
     };
     ring_serve<Args>(R, Q.off_args, prep, [&](uint8_t* slot, const RingSlotHdr& s_hdr, const Args& s_args, unsigned long long (&t)[4]) __attribute__((always_inline)) {
         const uint32_t n_runs = s_hdr.n_runs;
-        if constexpr (kRequests) {          // the request block (read by the pack phase only, behind small_body's barriers)
-            const uint32_t n = s_args.n_reqs;
-            const uint4* src = reinterpret_cast<const uint4*>(slot + Q.off_reqs);
-            uint4* dst = reinterpret_cast<uint4*>(Q.reqs);
-            for (uint32_t k = tid; k < n * (uint32_t)sizeof(ReqDesc) / 16u; k += kSmallThreads) dst[k] = src[k];
-            const uint32_t* so = reinterpret_cast<const uint32_t*>(slot + Q.off_reqs + n * (uint32_t)sizeof(ReqDesc));
+        if constexpr (kPacks) {             // the record block (read by the pack phase only, behind small_body's barriers)
+            using Rec = typename RingBodyOf<kBody>::Rec;
+            const uint32_t n = s_args.n_recs;
+            const uint4* src = reinterpret_cast<const uint4*>(slot + Q.off_recs);
+            uint4* dst = reinterpret_cast<uint4*>(Q.recs);
+            for (uint32_t k = tid; k < (n * (uint32_t)sizeof(Rec) + 15u) / 16u; k += kSmallThreads) dst[k] = src[k];
+            const uint32_t* so = reinterpret_cast<const uint32_t*>(slot + Q.off_recs + n * (uint32_t)sizeof(Rec));
             for (uint32_t k = tid; k < n; k += kSmallThreads) Q.offs[k] = so[k];
         }
         if constexpr (kWrites) {            // the write records (read by the write pass only, behind small_body's barriers)
@@ -3630,12 +3640,15 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_ring(RingDev R, BatchPtrs 
                 __syncthreads();
             }
         }
-        if constexpr (kRequests) {
+        if constexpr (kPacks) {
+            using Rec = typename RingBodyOf<kBody>::Rec;
             const uint32_t lane = tid & 31, wid = tid >> 5;
             CrcTabs ct; ct.hot = S.s_hot; ct.tree = B0.crc_adv + kCrcHotWords;
-            for (uint32_t i = wid; i < s_args.n_reqs; i += kSmallWarps) {
-                const ReqDesc q = Q.reqs[i];
-                pack_request_one(R.d_bytes, q, B0.methods, Cb.n_methods, Q.out, Q.scratch, Q.offs + i, B0.snappy_tab + (size_t)wid * kSnappyMaxTable, Q.lens + i, lane, ct);
+            uint16_t* tab = B0.snappy_tab + (size_t)wid * kSnappyMaxTable;
+            for (uint32_t i = wid; i < s_args.n_recs; i += kSmallWarps) {
+                const Rec q = reinterpret_cast<const Rec*>(Q.recs)[i];
+                if constexpr (kRequests) pack_request_one(R.d_bytes, q, B0.methods, Cb.n_methods, Q.out, Q.scratch, Q.offs + i, tab, Q.lens + i, lane, ct);
+                else pack_response_one(R.d_bytes, q, Q.out, Q.offs + i, tab, Q.lens + i, lane, ct);
             }
             __threadfence();
             __syncthreads();
@@ -3643,12 +3656,12 @@ __global__ void __launch_bounds__(kSmallThreads, 1) k_ring(RingDev R, BatchPtrs 
         if (tid == 0) t[3] = globaltimer_ns();
         // push the compact block [totals | run_status | msgs | refs | resp] into the slot's output area
         ring_push(slot + R.off_out, R.d_small, (B.totals[2] & 3u) ? 64u : s_hdr.off_resp + ((B.totals[1] + 15u) & ~15u), tid, kSmallThreads);
-        if constexpr (kRequests) {          // ... the frame lengths, and of every frame its out_len bytes
+        if constexpr (kPacks) {             // ... the frame lengths, and of every frame its out_len bytes
             const uint32_t lane = tid & 31, wid = tid >> 5;
-            ring_push(slot + Q.off_req_lens, reinterpret_cast<const uint8_t*>(Q.lens), s_args.n_reqs * 4u, tid, kSmallThreads);
-            for (uint32_t i = wid; i < s_args.n_reqs; i += kSmallWarps) {
+            ring_push(slot + Q.off_lens, reinterpret_cast<const uint8_t*>(Q.lens), s_args.n_recs * 4u, tid, kSmallThreads);
+            for (uint32_t i = wid; i < s_args.n_recs; i += kSmallWarps) {
                 const uint32_t off = Q.offs[i];
-                ring_push(slot + Q.off_req_out + off, Q.out + off, __ldcg(Q.lens + i), lane, 32);
+                ring_push(slot + Q.off_out + off, Q.out + off, __ldcg(Q.lens + i), lane, 32);
             }
         }
         if (streams && !overflow) {   // ... and the stream section [counters | events | msgs | ctrl | run_ctrl | out], the used part of each

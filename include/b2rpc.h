@@ -480,8 +480,8 @@ int  b2_pack_requests(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2_
  * (correlation ids live on the host), so a ticket's requests do not depend on its runs: they are packed even when the runs overflow the
  * compact block.  Runs are served whatever their flags: server runs in a client ticket are answered as b2_ring_submit answers them.
  * For each socket hand its reads over first, then write its request frames in request order.
- * A context runs one ring kind: b2_ring_submit / _wait, b2_stream_ring_enable and the b2_h2_*ring* calls refuse a context that runs this
- * one, and b2_client_ring_* refuse a context of another kind.
+ * A context runs one ring kind: b2_ring_submit / _wait, b2_stream_ring_enable, b2_ring_turn_* and the b2_h2_*ring* calls refuse a
+ * context that runs this one, and b2_client_ring_* refuse a context of another kind.
  * b2_client_ring_enable: once, before the context's first ring call, and not on a context with a stream table (else B2_E_INVAL; the
  * ticket runs no stream pass).  max_bytes bounds a ticket's whole `bytes` (the runs' bytes plus the request payloads, <= max_batch_bytes,
  * so a turn may exceed b2_ring_submit's 128 KiB); max_reqs (<= max_msgs) and req_out_cap (<= max_resp_bytes) play the roles of
@@ -544,6 +544,45 @@ typedef struct b2_reply {
 } b2_reply;                          /* 88 bytes */
 int  b2_pack_responses(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2_reply* replies, uint32_t n,
                        void* out, uint32_t out_cap, uint32_t* out_offs, uint32_t* out_lens);
+/* baidu_std SERVER turns on the latency path: b2_process_batch followed by b2_pack_responses inside the resident k_ring
+ * (k_ring<RingBody::replies>) fed through the same submit ring.  A ticket is one turn of a server's event loop: read what arrived, then
+ * send the replies user code produced for B2_HANDLER_HOST methods since the last turn.  The runs are served as by b2_ring_submit (device
+ * methods are answered in the compact block as before), then the replies are packed as by b2_pack_responses; their fields index the same
+ * `bytes` as the runs.  A baidu_std server keeps no connection state on the device, so a turn's replies do not depend on its runs: they
+ * are packed even when the runs overflow the compact block.  baidu_std clients match replies by correlation_id, so the order in which
+ * the host writes a socket's device-answered replies and its host replies does not matter.
+ * A context runs one ring kind: b2_ring_submit / _wait, b2_stream_ring_enable, b2_client_ring_* and the b2_h2_*ring* calls refuse a
+ * context that runs this one, and b2_ring_turn_* refuse a context of another kind.
+ * b2_ring_turn_enable: once, before the context's first ring call, and not on a context with a stream table (else B2_E_INVAL; the turn
+ * runs no stream pass: a reply that accepts a Stream goes through the batch calls).  Every cap must be non-zero (else B2_E_INVAL).
+ * max_bytes bounds a turn's whole `bytes` (the runs' bytes plus the reply bodies, <= max_batch_bytes, so a turn may exceed
+ * b2_ring_submit's 128 KiB); max_resps (max_resps * 88 <= max_msgs * 64, as for b2_pack_responses' n) and resp_out_cap
+ * (<= max_resp_bytes) play the roles of b2_pack_responses' n and out_cap.  Caps above those limits fail with B2_E_CAPACITY; they fix the
+ * slot layout.  b2_ring_stop, b2_ring_launches, b2_ring_phase_ns ([2]: runs served and replies packed) and B2_RING_IDLE_MS apply as
+ * to k_ring.
+ * b2_ring_turn_submit: n_runs or n_replies may be 0, not both.  Every check of b2_ring_submit (<= 512 runs, 16-aligned runs inside
+ * `bytes`) and of b2_pack_responses (reply fields inside `bytes`, every frame placed at its worst-case size within resp_out_cap) applies
+ * with the enable-time caps and the same codes; a failed check claims no slot and leaves the next ticket number unchanged.  The runs keep
+ * the compact block's limits (1024 messages, its reply bytes), sized from the extent the runs cover.  Bytes in b2_block_alloc memory are
+ * pulled in place, others staged into the slot.
+ * b2_ring_turn_wait: tickets may be waited in any order.  For any sequence of turns `batch` equals b2_process_batch(bytes, runs), and
+ * each reply's offset, length and frame bytes equal b2_pack_responses(bytes, replies, resp_out_cap), on a context with the same settings,
+ * byte for byte.  gzip / zlib replies come back with length 0, as from b2_pack_responses.  A turn whose runs overflow the compact block has
+ * them served through the big pipeline inside the wait, as b2_ring_wait does (every other ticket collected first); its replies still come
+ * from the kernel.  B2_RESP_BY_REF / B2_RESP_IOVEC apply to the runs only, as in b2_ring_wait.  While a turn is outstanding every call
+ * that uploads to the context (b2_process_batch, b2_batch_*, b2_pack_requests, b2_pack_responses, the crc32c / snappy / hpack / h2
+ * calls) fails with B2_E_INVAL. */
+typedef struct b2_ring_turn_result {     /* views into the ticket's pinned slot, valid until the 8th later submission */
+    b2_batch_result batch;               /* the runs, exactly as b2_ring_wait returns them */
+    uint32_t n_replies, reserved;
+    const uint32_t* reply_offs;          /* as b2_pack_responses' out_offs */
+    const uint32_t* reply_lens;          /* as its out_lens: 0 = could not be packed */
+    const uint8_t*  reply_out;           /* reply i's frame at reply_out + reply_offs[i] */
+} b2_ring_turn_result;                   /* 104 bytes */
+int  b2_ring_turn_enable(b2_ctx* ctx, uint32_t max_bytes, uint32_t max_resps, uint32_t resp_out_cap);
+int  b2_ring_turn_submit(b2_ctx* ctx, const void* bytes, uint32_t nbytes, const b2_run* runs, uint32_t n_runs,
+                         const b2_reply* replies, uint32_t n_replies, uint32_t* ticket);
+int  b2_ring_turn_wait(b2_ctx* ctx, uint32_t ticket, b2_ring_turn_result* out);
 
 /* ---- h2 / gRPC (SURVEY §8a a15): leaf calls first, then the whole server-side parser and the reply framing -----
  * b2_h2_scan_batch: H2Context::ConsumeFrameHead (src/brpc/policy/http2_rpc_protocol.cpp:438-465)
